@@ -311,16 +311,26 @@ int udb_reflect_border_fill_nhwc_f16(void* buf, int32_t B, int32_t H, int32_t W,
 
 /* V1 pre-processing + stem im2col (unidepthv1.py:49-63,298-317; convnext.py:371-383): uint8 / f32 NCHW -> (/255) ->
  * ImageNet normalise -> antialiased bilinear to (rh, rw) -> zero pad (pad_l, pad_t) into (net_h, net_w) -> f16 rows
- * [B*gh*gw, 64] of the 4x4 stride-4 patches (column c*16 + py*4 + px, 48 used; gh = (net_h-4)/4+1). */
+ * [B*gh*gw, 64] of the 4x4 stride-4 patches (column c*16 + py*4 + px, 48 used; gh = (net_h-4)/4+1).
+ * patch == 14 (DINOv2 encoder): rows [B*(net_h/14)*(net_w/14), 640] of the 14x14 patches instead, column
+ * c*196 + py*14 + px (588 used, the rest zero: the layout udb_preprocess_patchify writes for the V2 patch embedding). */
 typedef struct udb_v1_preprocess_t {
   const void* rgb;
   int32_t rgb_is_u8, scale255, normalize;
   int32_t B, H, W;
   int32_t rh, rw, pad_l, pad_t;
   int32_t net_h, net_w;
+  int32_t patch;          /* 0 or 4: the ConvNeXt stem layout above; 14: DINOv2 patch rows */
   void* patches;
 } udb_v1_preprocess_t;
 int udb_v1_preprocess(const udb_v1_preprocess_t* p, void* stream);
+
+/* DINOv2 block output -> UniDepthV1 decoder level (unidepthv1.py:322-326 adds each block's cls token to its patch tokens;
+ * decoder.py:371-379 takes the max over a slice of blocks).  x f32 [B, 1+N, D] (cls row first):
+ *   acc[b*N + t, :] = first ? f16(x[b,1+t,:] + x[b,0,:]) : max(acc[b*N + t, :], f16(x[b,1+t,:] + x[b,0,:]))
+ * f16 round-to-nearest is monotone, so the running max kept in f16 equals f16 of the f32 max.  cls_out (may be NULL)
+ * [B, D] f32 = x[b,0,:], the raw cls row the camera head reads.  D % 8 == 0. */
+int udb_vit_tap(const float* x, void* acc, float* cls_out, int32_t B, int32_t N, int32_t D, int32_t first, void* stream);
 
 /* LayerNorm over the last dim for widths that are multiples of 64 up to 1536 (ConvNeXt channel LayerNorm / LayerNorm2d,
  * convnext.py:214,252-263; decoder LayerNorms).  in row r at in + r*ld_in (+ add[(r % add_mod)*dim ..] when add != NULL:
@@ -548,18 +558,23 @@ typedef struct udb_infer_args_t {
 int udb_infer_v2(udb_engine* e, const udb_infer_args_t* a, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * UniDepthV1 engine: the whole `UniDepthV1.infer` path (ConvNeXt encoder) as one call (SURVEY.md section 8b
+ * UniDepthV1 engine: the whole `UniDepthV1.infer` path (ConvNeXt or DINOv2 encoder) as one call (SURVEY.md section 8b
  * `udb_infer_v1`; reference unidepth/models/unidepthv1/unidepthv1.py:288-373).  Same contract as the V2 engine: the
  * caller owns packed weights (names listed in unidepth_b200/unidepthv1.py::_pack), workspace and outputs; nothing is
  * allocated, copied or synchronised inside udb_infer_v1.
  * ------------------------------------------------------------------------------------------- */
 typedef struct udb_engine_v1 udb_engine_v1;
 
+#define UDB_V1_ENCODER_CONVNEXT 0
+#define UDB_V1_ENCODER_DINOV2 1
+
 typedef struct udb_v1_config_t {
-  int32_t depths[4];      /* ConvNeXt blocks per stage (convnext_large: 3,3,27,3) */
-  int32_t dims[4];        /* stage widths (192,384,768,1536) */
+  int32_t depths[4];      /* ConvNeXt blocks per stage (convnext_large: 3,3,27,3); DINOv2: blocks per max-pooled slice
+                             (ViT-L: 5,7,6,6 = output_idx 5,12,18,24) */
+  int32_t dims[4];        /* stage widths (192,384,768,1536); DINOv2: the embedding width four times */
   int32_t hidden, heads, expansion;
   int32_t dec_depths[3];  /* attention blocks at 1/16, Nystrom blocks at 1/8 and 1/4 (config pixel_decoder.depths) */
+  int32_t encoder;        /* UDB_V1_ENCODER_*; 0 (ConvNeXt) for zero-initialised configs */
   int32_t net_h, net_w;   /* fixed network input (config data.image_shape: 462 x 616) */
 } udb_v1_config_t;
 

@@ -129,7 +129,8 @@ class InferArgs(C.Structure):
 class V1Preprocess(C.Structure):
     _fields_ = [
         ("rgb", vp), ("rgb_is_u8", i32), ("scale255", i32), ("normalize", i32), ("B", i32), ("H", i32), ("W", i32),
-        ("rh", i32), ("rw", i32), ("pad_l", i32), ("pad_t", i32), ("net_h", i32), ("net_w", i32), ("patches", vp),
+        ("rh", i32), ("rw", i32), ("pad_l", i32), ("pad_t", i32), ("net_h", i32), ("net_w", i32), ("patch", i32),
+        ("patches", vp),
     ]
 
 
@@ -158,7 +159,7 @@ class V1Postprocess(C.Structure):
 class V1Config(C.Structure):
     _fields_ = [
         ("depths", i32 * 4), ("dims", i32 * 4), ("hidden", i32), ("heads", i32), ("expansion", i32),
-        ("dec_depths", i32 * 3), ("net_h", i32), ("net_w", i32),
+        ("dec_depths", i32 * 3), ("encoder", i32), ("net_h", i32), ("net_w", i32),
     ]
 
 
@@ -214,6 +215,7 @@ EXPORTS = {
     "udb_dwconv7_nhwc_f16": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, vp]),
     "udb_max_accum_f16": (i32, [vp, vp, i64, i32, vp]),
     "udb_spatial_mean_f32": (i32, [vp, vp, i32, i32, i32, vp]),
+    "udb_vit_tap": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
     "udb_aa_resize_nhwc_f16": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, vp]),
     "udb_v1_rays_sh81": (i32, [C.POINTER(V1Rays), vp]),
     "udb_v1_camera_intrinsics": (i32, [vp, vp, i32, i32, i32, f32, i32, i32, i32, vp, vp, vp, vp]),

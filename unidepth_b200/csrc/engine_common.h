@@ -229,4 +229,77 @@ static inline std::string idx2(const char* fmt, int i, int j) {
   return b;
 }
 
+// ------------------------------------------------------------------------------------------ DINOv2 blocks
+// Shape and packing mode of the DINOv2 block loop (UniDepthV2 uses every mode; UniDepthV1 ViT-L the default f16 one).
+struct VitBlocks {
+  int B, T, D, heads, depth;
+  bool split = false;          // split-f16 precise mode: operands are [hi | lo] pairs, weights [N, 3K] = [hi | hi | lo]
+  bool fuse = false;           // fused LayerNorm: norm1 / norm2 folded into qkv / fc1 (udb_gemm_t.ln_*)
+  __half* x16 = nullptr;       // fused mode: f16 copy of x and its per-part LayerNorm statistics, kept up to date by the
+  float* stats = nullptr;      // GEMMs that write x (the patch embedding included)
+  int ln_parts = 0, ln_pc = 0;
+};
+
+// `depth` pre-norm transformer blocks (metadinov2/block.py:84-109, LayerNorm eps 1e-6) on the f32 residual stream
+// x [B*T, D], weights "<prefix><i>.<operand>" as unidepthv2.pack_vit_encoder packs them.  after_block(i) runs once block
+// i has updated x (the engines read their encoder outputs there).  The scratch it allocates is released on return.
+template <class Hook>
+static inline void vit_blocks(Ctx& c, const std::string& prefix, float* x, const VitBlocks& v, Hook&& after_block) {
+  Arena& ar = *c.ar;
+  const int D = v.D;
+  const size_t BT = static_cast<size_t>(v.B) * v.T;
+  const bool sp = v.split, fuse = v.fuse;
+  const int sx = sp ? 2 : 1;
+  __half* x16 = v.x16;
+  float* stats = v.stats;
+  const int ln_parts = v.ln_parts, ln_pc = v.ln_pc;
+  const size_t m = ar.mark();
+  __half* h = fuse ? nullptr : ar.h(BT * D * sx);
+  __half* qkv = ar.h(BT * 3 * D * sx);
+  __half* att = ar.h(BT * D * sx);
+  __half* mid = ar.h(BT * 4 * D * sx);
+  const int kx = sp ? 3 : 1;          // logical K multiplier of a split operand
+  for (int i = 0; i < v.depth; ++i) {
+    const std::string b = prefix + idx("%d.", i);
+    // a weight packed for another mode (or transposed) must be refused, not read with the wrong leading dimension
+    c.expect2(b + (fuse ? "qkv_wf" : "qkv_w"), 3 * D, D * kx);
+    c.expect2(b + (fuse ? "fc1_wf" : "fc1_w"), 4 * D, D * kx);
+    c.expect2(b + "proj_w", D, D * kx);
+    c.expect2(b + "fc2_w", D, 4 * D * kx);
+    if (fuse) {
+      Ctx::G q{x16, c.H(b + "qkv_wf"), static_cast<int>(BT), 3 * D, D};
+      q.bias = c.F(b + "qkv_c2"); q.ln_stats_in = stats; q.ln_c1 = c.F(b + "qkv_c1"); q.ln_parts = ln_parts; q.ln_part_cols = ln_pc;
+      q.ln_eps = 1e-6f; q.out = qkv; c.gemm(q);
+    } else {
+      c.layernorm(x, 1, h, 0, c.F(b + "n1w"), c.F(b + "n1b"), static_cast<int>(BT), D, 1e-6f, 0, 0, 0, 0, sp ? D : 0);
+      Ctx::G q{h, c.H(b + "qkv_w"), static_cast<int>(BT), 3 * D, D * kx}; q.lda = D * sx; q.a_split_k = sp ? D : 0;
+      q.bias = c.F(b + "qkv_b"); q.out = qkv; q.ldc = 3 * D * sx; q.out_split = sp ? 3 * D : 0; c.gemm(q);
+    }
+    c.attention(qkv, qkv, qkv, att, v.B, v.heads, v.T, v.T, 3 * D * sx, 3 * D * sx, 3 * D * sx, D * sx, 0, D, 2 * D, 0.125f,
+                sp ? 3 * D : 0, sp ? D : 0);
+    { Ctx::G q{att, c.H(b + "proj_w"), static_cast<int>(BT), D, D * kx}; q.lda = D * sx; q.a_split_k = sp ? D : 0;
+      q.bias = c.F(b + "proj_b"); q.gamma = c.F(b + "ls1");
+      q.resid = x; q.resid_f32 = 1; q.out = x; q.out_f32 = 1;
+      if (fuse) { q.out2 = x16; q.out2_leaky = 0; q.ln_stats_out = stats; q.ln_parts = ln_parts; q.ln_part_cols = ln_pc; }
+      c.gemm(q); }
+    if (fuse) {
+      Ctx::G q{x16, c.H(b + "fc1_wf"), static_cast<int>(BT), 4 * D, D};
+      q.bias = c.F(b + "fc1_c2"); q.ln_stats_in = stats; q.ln_c1 = c.F(b + "fc1_c1"); q.ln_parts = ln_parts; q.ln_part_cols = ln_pc;
+      q.ln_eps = 1e-6f; q.act = UDB_ACT_GELU; q.out = mid; c.gemm(q);
+    } else {
+      c.layernorm(x, 1, h, 0, c.F(b + "n2w"), c.F(b + "n2b"), static_cast<int>(BT), D, 1e-6f, 0, 0, 0, 0, sp ? D : 0);
+      Ctx::G q{h, c.H(b + "fc1_w"), static_cast<int>(BT), 4 * D, D * kx}; q.lda = D * sx; q.a_split_k = sp ? D : 0;
+      q.bias = c.F(b + "fc1_b"); q.act = UDB_ACT_GELU;
+      q.out = mid; q.ldc = 4 * D * sx; q.out_split = sp ? 4 * D : 0; c.gemm(q);
+    }
+    { Ctx::G q{mid, c.H(b + "fc2_w"), static_cast<int>(BT), D, 4 * D * kx}; q.lda = 4 * D * sx; q.a_split_k = sp ? 4 * D : 0;
+      q.bias = c.F(b + "fc2_b"); q.gamma = c.F(b + "ls2");
+      q.resid = x; q.resid_f32 = 1; q.out = x; q.out_f32 = 1;
+      if (fuse) { q.out2 = x16; q.out2_leaky = 0; q.ln_stats_out = stats; q.ln_parts = ln_parts; q.ln_part_cols = ln_pc; }
+      c.gemm(q); }
+    after_block(i);
+  }
+  ar.release(m);
+}
+
 }  // namespace udb

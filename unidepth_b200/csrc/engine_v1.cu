@@ -1,4 +1,5 @@
-// Whole-path engine for UniDepthV1.infer with the ConvNeXt encoder (BASELINE config 4), behind udb_v1_create /
+// Whole-path engine for UniDepthV1.infer with the ConvNeXt encoder (BASELINE config 4) or the DINOv2 ViT-L/14 encoder
+// (config_v1_vitl14; the block loop is the one UniDepthV2 runs, engine_common.h `vit_blocks`), behind udb_v1_create /
 // udb_v1_set_weight / udb_v1_workspace_bytes / udb_infer_v1 (include/udb.h).  Host-side schedule only: it enqueues the
 // kernels of this library on the caller's stream over a bump-allocated workspace (no allocation, copy or sync inside
 // udb_infer_v1, so the call is graph-capturable).  Reference call stack it replaces:
@@ -197,15 +198,67 @@ static void conv_upsample(V1Ctx& c, const std::string& p, const float* lat, cons
   ar.release(m);
 }
 
+// DINOv2 encoder of UniDepthV1 (unidepthv1.py:316-326; dinov2.py:306-347 with use_norm=False): 14x14 patch rows of the
+// pre-processed image -> patch GEMM with the pack-time position table ("pos" [1 + gh*gw, D], cls row first: offset-0.1
+// bicubic resize of the 37x37 grid) as row-mapped residual -> cls rows -> the shared block loop.  After every block the
+// tap kernel folds (patch tokens + cls token) into the running max of its slice (levels[s], decoder.py:371-379; slice s
+// holds cf.depths[s] blocks) and copies the raw cls rows of the last four blocks into clsbuf[k] (block last - k).
+static void dino_encoder(V1Ctx& c, const udb_v1_config_t& cf, const udb_infer_v1_args_t& a, const V1Geom& g, int gh, int gw,
+                         __half* const* levels, float* const* clsbuf) {
+  Arena& ar = *c.ar;
+  const int B = a.B, D = cf.dims[0], N = gh * gw, T = N + 1;
+  const size_t BN = static_cast<size_t>(B) * N, BT = static_cast<size_t>(B) * T;
+  int depth = 0;
+  for (int i = 0; i < 4; ++i) depth += cf.depths[i];
+  const size_t m = ar.mark();
+  __half* patches = ar.h(BN * 640);
+  if (!c.dry) {
+    udb_v1_preprocess_t p;
+    memset(&p, 0, sizeof(p));
+    p.rgb = a.rgb; p.rgb_is_u8 = a.rgb_is_u8; p.scale255 = a.scale255; p.normalize = a.normalize; p.B = B; p.H = a.H; p.W = a.W;
+    p.rh = g.rh; p.rw = g.rw; p.pad_l = g.pad_l; p.pad_t = g.pad_t; p.net_h = cf.net_h; p.net_w = cf.net_w; p.patches = patches;
+    p.patch = 14;
+    c.done(udb_v1_preprocess(&p, c.st));
+  }
+  float* x = ar.f(BT * D);           // fp32 residual stream [B, 1 + N, D]
+  {
+    c.expect2("patch_w", D, 640);
+    c.expect2("pos", T, D);
+    const float* pos = c.F("pos");
+    const float* cls = c.F("cls");     // looked up here so that a dry run names it when it is missing
+    Ctx::G q{patches, c.H("patch_w"), static_cast<int>(BN), D, 640};
+    q.bias = c.F("patch_b"); q.resid = pos; q.resid_f32 = 1; q.ldr = D; q.out = x; q.out_f32 = 1;
+    q.rows_per_group = N; q.group_stride = T; q.row_offset = 1; q.resid_mod = N; q.resid_row_offset = 1;
+    c.gemm(q);
+    if (!c.dry && !c.rc) c.done(udb_set_cls_rows(x, cls, pos, B, T, D, c.st));
+  }
+  VitBlocks v{B, T, D, D / 64, depth};
+  int slice = 0, start = 0;
+  vit_blocks(c, "blocks.", x, v, [&](int i) {
+    if (i == start + cf.depths[slice]) { start = i; ++slice; }
+    const int from_end = depth - 1 - i;
+    if (!c.dry && !c.rc)
+      c.done(udb_vit_tap(x, levels[slice], from_end < 4 ? clsbuf[from_end] : nullptr, B, N, D, i == start, c.st));
+    if (i == 0) c.tap("enc_block0", x, sizeof(float) * BT * D);
+  });
+  c.tap("enc_last", x, sizeof(float) * BT * D);
+  ar.release(m);
+}
+
 static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, void* st) {
   const udb_v1_config_t& cf = e->cfg;
   V1Ctx c;
   c.e = e; c.ar = &ar; c.st = st; c.dry = ar.dry;
   const int B = a.B, net_h = cf.net_h, net_w = cf.net_w, hid = cf.hidden;
   const V1Geom g = v1_geometry(a.H, a.W, net_h, net_w);
+  const bool dino = cf.encoder == UDB_V1_ENCODER_DINOV2;
   int sh[4], sw[4];
-  sh[0] = (net_h - 4) / 4 + 1; sw[0] = (net_w - 4) / 4 + 1;
-  for (int i = 1; i < 4; ++i) { sh[i] = sh[i - 1] / 2; sw[i] = sw[i - 1] / 2; }
+  if (dino) {                       // one 14-pixel patch grid for every level (decoder.py:381-396: flat_interpolate is the identity)
+    for (int i = 0; i < 4; ++i) { sh[i] = net_h / 14; sw[i] = net_w / 14; }
+  } else {
+    sh[0] = (net_h - 4) / 4 + 1; sw[0] = (net_w - 4) / 4 + 1;
+    for (int i = 1; i < 4; ++i) { sh[i] = sh[i - 1] / 2; sw[i] = sw[i - 1] / 2; }
+  }
   Stage stage;
 
   // ---- pre-processing + stem (convnext.py:371-383: conv k4 s4 as an im2col GEMM, then LayerNorm2d)
@@ -224,7 +277,10 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
     if (k != 4) { set_error("udb_infer_v1: the encoder needs at least four blocks"); return 1; }
   }
   for (int k = 0; k < 4; ++k) clsbuf[k] = ar.f(static_cast<size_t>(B) * cls_dim[k]);     // clsbuf[k]: block (last - k)
-  {
+  if (dino) {
+    stage.next("udb_v1:dinov2_encoder");
+    dino_encoder(c, cf, a, g, sh[0], sw[0], levels, clsbuf);
+  } else {
     const size_t enc_mark = ar.mark();
     const long long n0 = static_cast<long long>(B) * sh[0] * sw[0];
     __half* patches = ar.h(n0 * 64);
@@ -494,6 +550,18 @@ extern "C" {
 
 int udb_v1_create(const udb_v1_config_t* cfg, udb_engine_v1** out) {
   if (!cfg || !out) { set_error("udb_v1_create: null argument"); return 1; }
+  if (cfg->encoder != UDB_V1_ENCODER_CONVNEXT && cfg->encoder != UDB_V1_ENCODER_DINOV2) {
+    set_error("udb_v1_create: encoder %d unknown (0 ConvNeXt, 1 DINOv2)", cfg->encoder);
+    return 1;
+  }
+  if (cfg->encoder == UDB_V1_ENCODER_DINOV2) {
+    if (cfg->net_h % 14 || cfg->net_w % 14) {
+      set_error("udb_v1_create: DINOv2 network shape %dx%d must be a multiple of the 14-pixel patch", cfg->net_h, cfg->net_w);
+      return 1;
+    }
+    for (int i = 1; i < 4; ++i)
+      if (cfg->dims[i] != cfg->dims[0]) { set_error("udb_v1_create: DINOv2 slices must all have the embedding width"); return 1; }
+  }
   for (int i = 0; i < 4; ++i)
     if (cfg->dims[i] <= 0 || cfg->dims[i] % 64 || cfg->dims[i] > 1536 || cfg->depths[i] <= 0) {
       set_error("udb_v1_create: stage %d (depth %d, width %d): widths must be multiples of 64 up to 1536", i, cfg->depths[i], cfg->dims[i]);

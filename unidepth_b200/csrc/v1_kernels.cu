@@ -62,25 +62,28 @@ __device__ __forceinline__ AAxis aa_axis(int i, int in_size, float scale) {
 
 // ------------------------------------------------------------------------------------------------------------------
 // V1 pre-processing (unidepthv1.py:49-63,298-317): u8 / f32 NCHW -> /255 -> ImageNet normalise -> antialiased bilinear
-// to (rh, rw) -> zero pad to the fixed network shape -> 4x4 stride-4 patch rows [B*gh*gw, 64] f16 (48 used:
-// column c*16 + py*4 + px, the stem conv's im2col, convnext.py:371-383).
+// to (rh, rw) -> zero pad to the fixed network shape -> P x P stride-P patch rows f16:
+//   P = 4:  [B*gh*gw, 64]  (48 used: column c*16 + py*4 + px, the ConvNeXt stem conv's im2col, convnext.py:371-383)
+//   P = 14: [B*gh*gw, 640] (588 used: column c*196 + py*14 + px, the DINOv2 patch embedding's im2col, patch_embed.py)
 // ------------------------------------------------------------------------------------------------------------------
+template <int P>
 __global__ void __launch_bounds__(256) v1_preprocess_kernel(const udb_v1_preprocess_t p, int gh, int gw, float sh, float sw) {
-  const long long total = (long long)p.B * gh * gw * 8;   // 8 x (8 columns) per patch row
+  constexpr int COLS = P == 4 ? 64 : 640, USED = 3 * P * P, NV8 = COLS / 8;
+  const long long total = (long long)p.B * gh * gw * NV8;   // NV8 x (8 columns) per patch row
   const float mean[3] = {0.485f, 0.456f, 0.406f};
   const float stdv[3] = {0.229f, 0.224f, 0.225f};
   for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
-    const int v8 = (int)(idx & 7);
-    const long long row = idx >> 3;
+    const int v8 = (int)(idx % NV8);
+    const long long row = idx / NV8;
     const int gx = (int)(row % gw), gy = (int)((row / gw) % gh), b = (int)(row / ((long long)gw * gh));
     float val[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const int col = v8 * 8 + j;
       float acc = 0.f;
-      if (col < 48) {
-        const int c = col >> 4, py = (col >> 2) & 3, px = col & 3;
-        const int Y = gy * 4 + py - p.pad_t, X = gx * 4 + px - p.pad_l;     // position in the resized image
+      if (col < USED) {
+        const int c = col / (P * P), py = (col % (P * P)) / P, px = col % P;
+        const int Y = gy * P + py - p.pad_t, X = gx * P + px - p.pad_l;     // position in the resized image
         if (Y >= 0 && Y < p.rh && X >= 0 && X < p.rw) {
           const AAxis ay = aa_axis(Y, p.H, sh), ax = aa_axis(X, p.W, sw);
           for (int jy = 0; jy < ay.xsize; ++jy) {
@@ -99,7 +102,7 @@ __global__ void __launch_bounds__(256) v1_preprocess_kernel(const udb_v1_preproc
       }
       val[j] = acc;
     }
-    *reinterpret_cast<uint4*>(reinterpret_cast<__half*>(p.patches) + row * 64 + v8 * 8) =
+    *reinterpret_cast<uint4*>(reinterpret_cast<__half*>(p.patches) + row * COLS + v8 * 8) =
         make_uint4(pack_half2(val[0], val[1]), pack_half2(val[2], val[3]), pack_half2(val[4], val[5]), pack_half2(val[6], val[7]));
   }
 }
@@ -271,6 +274,44 @@ __global__ void __launch_bounds__(256) max_accum_kernel(const uint4* __restrict_
       for (int j = 0; j < 4; ++j) sh[j] = __hmax2(sh[j], dh[j]);
     }
     dst[i] = s;
+  }
+}
+
+// DINOv2 block output -> decoder level (unidepthv1.py:322-326, decoder.py:371-379): one thread per 8 channels of a patch
+// token, acc = first ? f16(x_tok + x_cls) : max(acc, f16(x_tok + x_cls)); the trailing B*D/8 work items copy the raw cls
+// rows to cls_out.  HBM-bound: 32 B of x read and 16 (first) or 32 B of acc moved per item; the cls row stays in L1/L2.
+__global__ void __launch_bounds__(256) vit_tap_kernel(const float* __restrict__ x, uint4* __restrict__ acc, float* __restrict__ cls_out,
+                                                     int B, int N, int D, int first) {
+  const int d8 = D / 8;
+  const long long n_acc = (long long)B * N * d8;
+  const long long total = n_acc + (cls_out ? (long long)B * d8 : 0);
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    if (i >= n_acc) {
+      const long long j = i - n_acc;
+      const int b = (int)(j / d8), c = (int)(j % d8) * 8;
+      const float4* src = reinterpret_cast<const float4*>(x + (long long)b * (N + 1) * D + c);
+      float4* dst = reinterpret_cast<float4*>(cls_out + (long long)b * D + c);
+      dst[0] = src[0];
+      dst[1] = src[1];
+      continue;
+    }
+    const int c = (int)(i % d8) * 8;
+    const long long r = i / d8;                     // b*N + t
+    const int b = (int)(r / N);
+    const long long t = r - (long long)b * N;
+    const float4* tok = reinterpret_cast<const float4*>(x + ((long long)b * (N + 1) + 1 + t) * D + c);
+    const float4* cls = reinterpret_cast<const float4*>(x + (long long)b * (N + 1) * D + c);
+    const float4 a0 = tok[0], a1 = tok[1], c0 = __ldg(cls), c1 = __ldg(cls + 1);
+    uint4 v = make_uint4(pack_half2(a0.x + c0.x, a0.y + c0.y), pack_half2(a0.z + c0.z, a0.w + c0.w),
+                         pack_half2(a1.x + c1.x, a1.y + c1.y), pack_half2(a1.z + c1.z, a1.w + c1.w));
+    if (!first) {
+      const uint4 d = acc[i];
+      __half2* vh = reinterpret_cast<__half2*>(&v);
+      const __half2* dh = reinterpret_cast<const __half2*>(&d);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) vh[j] = __hmax2(vh[j], dh[j]);
+    }
+    acc[i] = v;
   }
 }
 
@@ -825,10 +866,17 @@ using namespace udb;
 extern "C" {
 
 int udb_v1_preprocess(const udb_v1_preprocess_t* p, void* stream) {
+  const float sh = (float)p->H / (float)p->rh, sw = (float)p->W / (float)p->rw;
+  if (p->patch == 14) {
+    if (p->net_h % 14 || p->net_w % 14) { set_error("udb_v1_preprocess: network shape %dx%d is not a multiple of 14", p->net_h, p->net_w); return 1; }
+    const int gh = p->net_h / 14, gw = p->net_w / 14;
+    v1_preprocess_kernel<14><<<grid_1d((long long)p->B * gh * gw * 80), 256, 0, ST(stream)>>>(*p, gh, gw, sh, sw);
+    return check_launch("v1_preprocess_kernel<14>");
+  }
+  if (p->patch != 0 && p->patch != 4) { set_error("udb_v1_preprocess: patch %d unsupported (0 / 4 or 14)", p->patch); return 1; }
   if (p->net_h < 4 || p->net_w < 4) { set_error("udb_v1_preprocess: bad network shape"); return 1; }
   const int gh = (p->net_h - 4) / 4 + 1, gw = (p->net_w - 4) / 4 + 1;
-  const float sh = (float)p->H / (float)p->rh, sw = (float)p->W / (float)p->rw;
-  v1_preprocess_kernel<<<grid_1d((long long)p->B * gh * gw * 8), 256, 0, ST(stream)>>>(*p, gh, gw, sh, sw);
+  v1_preprocess_kernel<4><<<grid_1d((long long)p->B * gh * gw * 8), 256, 0, ST(stream)>>>(*p, gh, gw, sh, sw);
   return check_launch("v1_preprocess_kernel");
 }
 
@@ -874,6 +922,14 @@ int udb_max_accum_f16(const void* src, void* dst, int64_t n, int32_t first, void
   note_work(0.0, (first ? 4.0 : 6.0) * n);
   max_accum_kernel<<<grid_1d(n / 8), 256, 0, ST(stream)>>>(reinterpret_cast<const uint4*>(src), reinterpret_cast<uint4*>(dst), n / 8, first);
   return check_launch("max_accum_kernel");
+}
+
+int udb_vit_tap(const float* x, void* acc, float* cls_out, int32_t B, int32_t N, int32_t D, int32_t first, void* stream) {
+  if (D % 8 || D <= 0 || N <= 0 || B <= 0) { set_error("udb_vit_tap: bad shape B=%d N=%d D=%d (D %% 8 == 0)", B, N, D); return 1; }
+  const long long items = (long long)B * N * (D / 8) + (cls_out ? (long long)B * (D / 8) : 0);
+  note_work((double)B * N * D, (double)B * N * D * (4.0 + (first ? 2.0 : 4.0)) + (cls_out ? 8.0 * B * D : 0.0));
+  vit_tap_kernel<<<grid_1d(items), 256, 0, ST(stream)>>>(x, reinterpret_cast<uint4*>(acc), cls_out, B, N, D, first);
+  return check_launch("vit_tap_kernel");
 }
 
 int udb_spatial_mean_f32(const float* x, float* out, int32_t B, int32_t HW, int32_t C, void* stream) {

@@ -1,12 +1,14 @@
-"""Static description of UniDepthV1 (ConvNeXt encoder) for the inference path: hyper-parameters read from the
-reference's config format, the parameter table under the reference's state-dict names, and the fixed-shape
+"""Static description of UniDepthV1 (ConvNeXt-L or DINOv2 ViT-L/14 encoder) for the inference path: hyper-parameters
+read from the reference's config format, the parameter table under the reference's state-dict names, and the fixed-shape
 arithmetic of `infer` (reference: unidepth/models/unidepthv1/unidepthv1.py:30-46 `_paddings` / `_shapes`,
-:423-447 `build`; unidepthv1/decoder.py:465-533 `Decoder.build`; backbones/convnext.py:301-448)."""
+:416-447 `build`; unidepthv1/decoder.py:465-533 `Decoder.build`; backbones/convnext.py:301-448, backbones/dinov2.py)."""
 from __future__ import annotations
 
 import math
 from collections import OrderedDict
 from typing import Dict, Tuple
+
+from .spec import PATCH, vit_encoder_shapes
 
 CONVNEXT_ARCHS = {
     # encoder.py:127-136 (`convnext_large`): depths / dims / per-stage end indices used as `output_idx`
@@ -14,25 +16,46 @@ CONVNEXT_ARCHS = {
     "convnext_large_pt": dict(depths=(3, 3, 27, 3), dims=(192, 384, 768, 1536)),
 }
 
+# DINOv2 encoders of UniDepthV1 (encoder.py:173-178 `dinov2_vitl14`): width, blocks, heads, output_idx.  The decoder takes
+# the max over the block slices between consecutive output_idx entries, so they play the role of the ConvNeXt stages.
+DINO_ARCHS = {
+    "dinov2_vitl14": dict(dim=1024, depth=24, heads=16, output_idx=(5, 12, 18, 24)),
+}
+# unidepthv1.py:423: every V1 DINOv2 encoder is built with interpolate_offset 0.1 (the V2 factories use 0)
+V1_INTERPOLATE_OFFSET = 0.1
+
+ENCODER_CONVNEXT, ENCODER_DINOV2 = 0, 1        # udb_v1_config_t.encoder (include/udb.h)
+
 
 class V1Spec:
     def __init__(self, config: dict):
         m = config["model"]
         enc = m["pixel_encoder"]
         name = enc["name"]
-        if name not in CONVNEXT_ARCHS and "arch" not in enc:
-            raise NotImplementedError(f"UniDepthV1 encoder '{name}': only the ConvNeXt encoders are implemented "
-                                      "(config_v1_cnvnxtl.json); the DINOv2 V1 variant is not")
-        arch = enc.get("arch", CONVNEXT_ARCHS.get(name))       # "arch": test-only override {depths, dims}
-        self.depths = tuple(arch["depths"])
-        self.dims = tuple(arch["dims"])
+        self.encoder_name = name
+        if name in DINO_ARCHS:
+            a = DINO_ARCHS[name]
+            self.encoder = ENCODER_DINOV2
+            self.embed_dim, self.enc_depth, self.enc_heads = a["dim"], a["depth"], a["heads"]
+            ends = tuple(a["output_idx"])
+            # slices [0, 5), [5, 12), [12, 18), [18, 24) of the 24 blocks (decoder.py:371-379), all 1024 wide
+            self.depths = tuple(e - s for s, e in zip((0,) + ends[:-1], ends))
+            self.dims = (self.embed_dim,) * 4
+        elif name in CONVNEXT_ARCHS or "arch" in enc:
+            self.encoder = ENCODER_CONVNEXT
+            arch = enc.get("arch", CONVNEXT_ARCHS.get(name))       # "arch": test-only override {depths, dims}
+            self.depths = tuple(arch["depths"])
+            self.dims = tuple(arch["dims"])
+        else:
+            raise NotImplementedError(f"UniDepthV1 encoder '{name}': only ConvNeXt-L (config_v1_cnvnxtl.json) and DINOv2 "
+                                      "ViT-L/14 (config_v1_vitl14.json) are implemented")
         ends, acc = [], 0
         for d in self.depths:
             acc += d
             ends.append(acc)
         self.output_idx = tuple(enc.get("output_idx", ends))   # encoder.py:131 default [3, 6, 33, 36]
         if tuple(self.output_idx) != tuple(ends):
-            raise NotImplementedError("output_idx must be the last block of each ConvNeXt stage")
+            raise NotImplementedError("output_idx must be the last block of each ConvNeXt stage / DINOv2 block slice")
         self.hidden = m["pixel_decoder"]["hidden_dim"]
         self.dec_depths = tuple(m["pixel_decoder"]["depths"])    # blocks at 1/16, 1/8 (Nystrom), 1/4 (Nystrom)
         self.heads = m["num_heads"]
@@ -43,6 +66,18 @@ class V1Spec:
         self.cls_dims = tuple(per_block[-i - 1] for i in range(4))
         if self.hidden % 64 or (self.hidden // self.heads) != 64:
             raise NotImplementedError("decoder needs 64-wide heads (hidden_dim / num_heads == 64)")
+        if self.encoder == ENCODER_DINOV2 and (self.image_shape[0] % PATCH or self.image_shape[1] % PATCH):
+            raise NotImplementedError(f"network shape {self.image_shape} is not a multiple of the {PATCH}-pixel patch")
+
+    def common_grid(self) -> Tuple[int, int]:
+        """(hc, wc): the decoder's common token grid (decoder.py:381-392, the second-smallest level).  ConvNeXt: stride-4
+        stem then two 2x downsamples; DINOv2: the single 14-pixel patch grid (462x616 -> 33x44)."""
+        if self.encoder == ENCODER_DINOV2:
+            return self.image_shape[0] // PATCH, self.image_shape[1] // PATCH
+        sh = [(self.image_shape[0] - 4) // 4 + 1, (self.image_shape[1] - 4) // 4 + 1]
+        for _ in range(2):
+            sh = [sh[0] // 2, sh[1] // 2]
+        return sh[0], sh[1]
 
 
 def v1_shapes(image_hw: Tuple[int, int], network_hw: Tuple[int, int]):
@@ -67,11 +102,14 @@ def param_shapes(config: dict) -> "OrderedDict[str, tuple]":
     out: "OrderedDict[str, tuple]" = OrderedDict()
     pe = "pixel_encoder."
     d0 = s.dims[0]
-    out[pe + "mask_token"] = (1, d0, 1, 1)
-    out[pe + "stem.0.weight"], out[pe + "stem.0.bias"] = (d0, 3, 4, 4), (d0,)
-    out[pe + "stem.1.weight"], out[pe + "stem.1.bias"] = (d0,), (d0,)
+    if s.encoder == ENCODER_DINOV2:
+        vit_encoder_shapes(out, s.embed_dim, s.enc_depth, pe)
+    else:
+        out[pe + "mask_token"] = (1, d0, 1, 1)
+        out[pe + "stem.0.weight"], out[pe + "stem.0.bias"] = (d0, 3, 4, 4), (d0,)
+        out[pe + "stem.1.weight"], out[pe + "stem.1.bias"] = (d0,), (d0,)
     prev = d0
-    for i, (depth, c) in enumerate(zip(s.depths, s.dims)):
+    for i, (depth, c) in enumerate(zip(s.depths, s.dims) if s.encoder == ENCODER_CONVNEXT else ()):
         st = f"{pe}stages.{i}."
         if i > 0:
             out[st + "downsample.0.weight"], out[st + "downsample.0.bias"] = (prev,), (prev,)

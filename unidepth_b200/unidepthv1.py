@@ -1,4 +1,4 @@
-"""UniDepthV1 (ConvNeXt encoder) -- drop-in for the reference's inference API, running on libudb.so (sm_90a).
+"""UniDepthV1 (ConvNeXt-L or DINOv2 ViT-L/14 encoder) -- drop-in for the reference's inference API, running on libudb.so (sm_90a).
 
 Mirrors `unidepth.models.UniDepthV1` for the inference path only (reference:
 unidepth/models/unidepthv1/unidepthv1.py:96-110 constructor, :288-373 `infer`, :375-392 `load_pretrained`,
@@ -30,10 +30,25 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _cabi as cabi
-from .spec_v1 import V1Spec, param_shapes, v1_paddings, v1_shapes
-from .unidepthv2 import PyTorchModelHubMixin, _HAS_HF, _register
+from .spec_v1 import (ENCODER_CONVNEXT, ENCODER_DINOV2, V1_INTERPOLATE_OFFSET, V1Spec, param_shapes, v1_paddings,
+                      v1_shapes)
+from .unidepthv2 import PyTorchModelHubMixin, _HAS_HF, _register, pack_vit_encoder
 
 f16, f32 = torch.float16, torch.float32
+
+
+def _offset_pos_embed(pos: torch.Tensor, gh: int, gw: int, offset: float) -> torch.Tensor:
+    """DINOv2 position table of a gh x gw patch grid with a nonzero interpolate_offset (dinov2.py:267-304): bicubic
+    resize of the M x M grid with scale factors ((gh + offset) / M, (gw + offset) / M), height first, so the sampling
+    positions use 1 / scale_factor rather than M / gh.  pos [1 + M*M, D] -> [1 + gh*gw, D], cls row first.  UniDepthV1
+    runs one fixed network shape, so this is a constant of the weights, evaluated at pack time."""
+    D = pos.shape[1]
+    M = math.isqrt(pos.shape[0] - 1)
+    grid = pos[1:].float().reshape(1, M, M, D).permute(0, 3, 1, 2)
+    g = F.interpolate(grid, scale_factor=((gh + offset) / M, (gw + offset) / M), mode="bicubic", antialias=False)
+    if tuple(g.shape[-2:]) != (gh, gw):
+        raise ValueError(f"position grid resized to {tuple(g.shape[-2:])}, expected {(gh, gw)}")
+    return torch.cat([pos[:1].float(), g.permute(0, 2, 3, 1).reshape(gh * gw, D)], dim=0)
 
 
 def _sine_position_embedding(h: int, w: int, num_pos_feats: int, device) -> torch.Tensor:
@@ -147,11 +162,22 @@ class UniDepthV1(nn.Module, PyTorchModelHubMixin,
             T[dst + "w2"], T[dst + "b2"] = h16(sd[f"{src}{fc2}.weight"]), c32(sd[f"{src}{fc2}.bias"])
             T[dst + "gamma"] = c32(sd[f"{src}gamma"])
 
+        hc, wc = s.common_grid()
         # ---- encoder
-        T["stem_w"] = h16(zpad(sd[pe + "stem.0.weight"].reshape(s.dims[0], 48), s.dims[0], 64))
-        T["stem_b"] = c32(sd[pe + "stem.0.bias"])
-        T["stem_ln_w"], T["stem_ln_b"] = c32(sd[pe + "stem.1.weight"]), c32(sd[pe + "stem.1.bias"])
-        for i, depth in enumerate(s.depths):
+        if s.encoder == ENCODER_DINOV2:
+            # default f16 packing of the V2 encoder; the final norm, mask token and register tokens are never read
+            # (use_norm=False, dinov2.py:173-178)
+            E = pack_vit_encoder(sd, s.embed_dim, s.enc_depth, dev)
+            T["patch_w"], T["patch_b"], T["cls"] = E["patch_w"], E["patch_b"], E["cls"]
+            for i, blk in enumerate(E["blocks"]):
+                for k, v in blk.items():
+                    T[f"blocks.{i}.{k}"] = v
+            T["pos"] = c32(_offset_pos_embed(E["pos"], hc, wc, V1_INTERPOLATE_OFFSET))
+        for i, depth in enumerate(s.depths if s.encoder == ENCODER_CONVNEXT else ()):
+            if i == 0:
+                T["stem_w"] = h16(zpad(sd[pe + "stem.0.weight"].reshape(s.dims[0], 48), s.dims[0], 64))
+                T["stem_b"] = c32(sd[pe + "stem.0.bias"])
+                T["stem_ln_w"], T["stem_ln_b"] = c32(sd[pe + "stem.1.weight"]), c32(sd[pe + "stem.1.bias"])
             st = f"{pe}stages.{i}."
             if i > 0:
                 w = sd[st + "downsample.1.weight"]                               # [C, Cp, 2, 2] -> [C, (dy,dx,ci)]
@@ -170,10 +196,6 @@ class UniDepthV1(nn.Module, PyTorchModelHubMixin,
             T[f"tok.{l}.w"], T[f"tok.{l}.b"] = c32(sd[t + ".1.weight"]), c32(sd[t + ".1.bias"])
         # level embedding MLP of the four learned level vectors + sine position embedding of the common grid
         # (decoder.py:410-433): constants of (weights, network shape), folded once here
-        sh = [(s.image_shape[0] - 4) // 4 + 1, (s.image_shape[1] - 4) // 4 + 1]
-        for _ in range(2):
-            sh = [sh[0] // 2, sh[1] // 2]
-        hc, wc = sh
         le = F.linear(F.gelu(F.linear(sd[pd + "level_embeds"].float(), sd[pd + "level_embed_layer.0.weight"].float(),
                                       sd[pd + "level_embed_layer.0.bias"].float())),
                       sd[pd + "level_embed_layer.2.weight"].float(), sd[pd + "level_embed_layer.2.bias"].float())
@@ -286,6 +308,7 @@ class UniDepthV1(nn.Module, PyTorchModelHubMixin,
         for i in range(3):
             cfg.dec_depths[i] = s.dec_depths[i]
         cfg.net_h, cfg.net_w = self.image_shape
+        cfg.encoder = s.encoder
         return cfg
 
     @staticmethod
