@@ -61,19 +61,24 @@ typedef struct udb_gemm_t {
    * W f16 [N,K] row-major (ldw elements).  K-extent is zero-extended to a multiple of 64. */
   const void* a;
   const void* w;
-  int32_t M, N, K;
+  int32_t M, N, K;  /* all >= 1; N % 32 == 0 */
   int32_t lda, ldw;
   int32_t a_mode;
   /* UDB_A_CONV3X3: input [B, H(+2), W(+2), C] f16 NHWC; K = 9*C ordered (dy,dx,c); the output
    * pixel (y,x) reads input (y+dy+off, x+dx+off), off = -1 for zero padding (out-of-range taps
    * read 0 through TMA out-of-bounds fill) or 0 when the input was padded by the caller
-   * (reflect padding, in_H = H+2, in_W = W+2). */
+   * (reflect padding, in_H = H+2, in_W = W+2).  Checked: conv_off is 0 or -1, and conv_inH / conv_inW are H+2 / W+2
+   * when it is 0, H / W when it is -1. */
   int32_t conv_B, conv_H, conv_W, conv_C, conv_inH, conv_inW, conv_off, conv_TH, conv_TW;
   /* the input may be a channel slice [conv_coff, conv_coff + conv_C) of a wider NHWC buffer with
    * conv_cstride channels per pixel (0 = conv_C) */
   int32_t conv_cstride, conv_coff;
   /* epilogue: v = acc + bias[n]; v = act(v); v *= gamma[n]; v += resid[...]; out = v;
-   * out2 = f16(v) or f16(leaky(v)) (optional second f16 copy, e.g. the next conv's input) */
+   * out2 = f16(v) or f16(leaky(v)) (optional second f16 copy, e.g. the next conv's input)
+   * Alignment (the epilogue moves 4 columns per vector access): bias / gamma / ln_c1 / head_w 16-byte aligned; f32
+   * out / resid 16-byte, f16 out / out2 / resid 8-byte aligned (HEAD: f32 out, 4-byte); ldc and ldr multiples of 4 (ROWS
+   * and CONVTILE stores).  The epilogue keeps each row's element offset in 32 bits: the last row written through out /
+   * out2 / resid must start below 2^32 elements. */
   const float* bias;
   const float* gamma;
   const void* resid;
@@ -84,13 +89,13 @@ typedef struct udb_gemm_t {
   int32_t out2_leaky; /* 1: out2 = f16(leaky(v)); 0: out2 = f16(v) */
   int32_t act;
   int32_t store_mode;
-  int64_t ldc; /* elements between consecutive output rows / pixels */
+  int64_t ldc; /* elements between consecutive output rows / pixels; ROWS / CONVTILE: >= N + out_split */
   /* UDB_STORE_ROWS: out_row = (m / rows_per_group)*group_stride + m % rows_per_group + row_offset
    * (rows_per_group <= 0: identity).  resid row = resid_mod > 0 ? m % resid_mod + resid_row_offset
-   * : out_row, with leading dimension ldr. */
+   * : out_row, with leading dimension ldr.  group_stride, row_offset and resid_row_offset >= 0. */
   int32_t rows_per_group, group_stride, row_offset;
   int32_t resid_mod, resid_row_offset;
-  int64_t ldr;
+  int64_t ldr; /* 0 = ldc; with a residual (ROWS / CONVTILE): >= N */
   /* UDB_STORE_CONVT: row m = (b, y, x) of a [B,h,w] grid; column n = (dy*k+dx)*Cout + co;
    * writes NHWC pixel (b, y*k+dy+pad, x*k+dx+pad, co) of a [B, h*k+2*pad, w*k+2*pad, Cout] map
    * (pad > 0: the interior of a buffer whose border udb_reflect_border_fill_nhwc_f16 fills). */
@@ -137,11 +142,11 @@ int udb_gemm_f16(const udb_gemm_t* g, void* stream);
 typedef struct udb_conv_halo_t {
   const void* x;
   const void* w;
-  const float* bias;
-  int32_t B, H, W, C, cstride, coff, cout, act;
-  void* out;
-  int64_t ldc;
-  const float* head_w;
+  const float* bias;   /* [cout], required */
+  int32_t B, H, W, C, cstride, coff, cout, act;   /* B, H, W >= 1; coff + C <= cstride (0 = C) */
+  void* out;           /* 4-byte aligned */
+  int64_t ldc;         /* 0 = cout; even and >= cout */
+  const float* head_w; /* required when head_out is set */
   float head_b, head_add;
   float* head_out;
 } udb_conv_halo_t;
@@ -157,10 +162,11 @@ typedef struct udb_attn_t {
   const void* q;
   const void* k;
   const void* v;
-  void* out;
-  int32_t B, heads, seq_q, seq_k, head_dim;
+  void* out; /* 4-byte aligned (f16 pairs are stored as 32-bit words) */
+  int32_t B, heads, seq_q, seq_k, head_dim; /* B, heads, seq_q, seq_k >= 1; head_dim 64 */
+  /* multiples of 8; each >= its col0 + heads*64 (+ its lo_off_* in split mode) */
   int32_t ldq, ldk, ldv, ldo;
-  int32_t q_col0, k_col0, v_col0, o_col0;
+  int32_t q_col0, k_col0, v_col0, o_col0; /* >= 0; o_col0 (and lo_off_o) even */
   float scale; /* 1/sqrt(head_dim) */
   /* Split-f16 ("precise") mode: when split != 0 the lo halves of q / k / v / out live lo_off_* elements to the right of
    * the hi halves (value = hi + lo) and the attention runs in an fp32 CUDA-core kernel (exact exp, f32 products):

@@ -244,16 +244,20 @@ def test_split_f16_gemm_layernorm_attention():
     assert err < 1e-5
 
 
-@pytest.mark.parametrize("D", [1024, 768, 384])
+@pytest.mark.parametrize("D", [1024, 768, 384, 640, 320, 96])
 def test_fused_layernorm_producer_consumer(D):
     """udb_gemm_t.ln_*: a residual-updating GEMM writes per-part row statistics + the f16 copy of its rows; the next GEMM
-    applies LayerNorm algebraically in its epilogue.  Reference: LayerNorm(x) @ W^T + b in float64 on the producer's f32 output."""
+    applies LayerNorm algebraically in its epilogue.  Reference: LayerNorm(x) @ W^T + b in float64 on the producer's f32 output.
+    D picks the producer's tile width (256, 192, 128, 64 and 32: at 32 one column group, so parts of 32 columns); below
+    D = 384 the consumer is D wide too, so it also runs the 64- and 32-column tiles."""
     from unidepth_b200 import ops
     dev = _dev()
     g = torch.Generator(device="cpu").manual_seed(D)
-    M, K0, N2 = 1500, 256, 640
-    bn = 256 if D % 256 == 0 else (192 if D % 192 == 0 else 128)
-    parts, pc = D // bn * 2, bn // 2
+    M, K0 = 1500, 256
+    N2 = 640 if D >= 384 else D
+    bn = next(b for b in (256, 192, 128, 64, 32) if D % b == 0)
+    groups = 2 if bn >= 64 else 1
+    parts, pc = D // bn * groups, bn // groups
     a = torch.randn(M, K0, generator=g).to(dev).half()
     w0 = (torch.randn(D, K0, generator=g) / 16).to(dev).half()
     x_in = (torch.randn(M, D, generator=g) * 1.5 + 0.3).to(dev)            # residual stream with a non-zero mean

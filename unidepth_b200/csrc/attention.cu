@@ -342,6 +342,31 @@ extern "C" int udb_attention_f16(const udb_attn_t* a, void* stream) {
   using namespace udb;
   if (a->head_dim != 64) { set_error("udb_attention_f16: head_dim %d unsupported (64 only)", a->head_dim); return 1; }
   if ((a->ldq | a->ldk | a->ldv | a->ldo) % 8) { set_error("udb_attention_f16: leading dims must be multiples of 8"); return 1; }
+  // Layout checks, all before the first CUDA call.  seq_k == 0 would leave every row sum at 0 (NaN outputs); the
+  // epilogue stores f16 pairs as 32-bit words at out + row*ldo + o_col0 + head*64 + even column.
+  if (a->B < 1 || a->heads < 1 || a->seq_q < 1 || a->seq_k < 1) {
+    set_error("udb_attention_f16: B=%d heads=%d seq_q=%d seq_k=%d must be >= 1", a->B, a->heads, a->seq_q, a->seq_k); return 1;
+  }
+  if (!a->q || !a->k || !a->v || !a->out) { set_error("udb_attention_f16: null q / k / v / out"); return 1; }
+  if (reinterpret_cast<uintptr_t>(a->out) & 3) { set_error("udb_attention_f16: `out` %p must be 4-byte aligned", a->out); return 1; }
+  const int lo_q = a->split ? a->lo_off_q : 0, lo_k = a->split ? a->lo_off_k : 0, lo_v = a->split ? a->lo_off_v : 0;
+  const int lo_o = a->split ? a->lo_off_o : 0;
+  if (a->o_col0 < 0 || (a->o_col0 & 1)) { set_error("udb_attention_f16: `o_col0`=%d must be even and >= 0", a->o_col0); return 1; }
+  if (lo_o < 0 || (lo_o & 1)) { set_error("udb_attention_f16: `lo_off_o`=%d must be even and >= 0", lo_o); return 1; }
+  if (lo_q < 0 || lo_k < 0 || lo_v < 0) { set_error("udb_attention_f16: `lo_off_q/k/v` must be >= 0"); return 1; }
+  const long long span = (long long)a->heads * 64;
+  if (a->ldo < a->o_col0 + span + lo_o) {
+    set_error("udb_attention_f16: `ldo`=%d < o_col0 + heads*64 + lo_off_o = %lld", a->ldo, a->o_col0 + span + lo_o); return 1;
+  }
+  if (a->q_col0 < 0 || a->ldq < a->q_col0 + span + lo_q) {
+    set_error("udb_attention_f16: `ldq`=%d < q_col0 + heads*64 = %lld (q_col0 >= 0)", a->ldq, a->q_col0 + span + lo_q); return 1;
+  }
+  if (a->k_col0 < 0 || a->ldk < a->k_col0 + span + lo_k) {
+    set_error("udb_attention_f16: `ldk`=%d < k_col0 + heads*64 = %lld (k_col0 >= 0)", a->ldk, a->k_col0 + span + lo_k); return 1;
+  }
+  if (a->v_col0 < 0 || a->ldv < a->v_col0 + span + lo_v) {
+    set_error("udb_attention_f16: `ldv`=%d < v_col0 + heads*64 = %lld (v_col0 >= 0)", a->ldv, a->v_col0 + span + lo_v); return 1;
+  }
   if (a->split) {
     static std::atomic<uint64_t> sp_mask{0};
     if (first_on_device(sp_mask)) {

@@ -189,6 +189,22 @@ extern "C" int udb_conv3x3_halo_f16(const udb_conv_halo_t* c, void* stream) {
   using namespace udb;
   if (c->C % 64 || (c->cout != 32 && c->cout != 64)) { set_error("udb_conv3x3_halo_f16: needs C %% 64 == 0 and Cout in {32, 64}"); return 1; }
   const int cs = c->cstride > 0 ? c->cstride : c->C;
+  // Layout checks, all before the first CUDA call: channels past cstride would read as TMA zero fill, and the f16 output
+  // is stored as 32-bit channel pairs at out + pixel*ldc + even channel.
+  if (c->B < 1 || c->H < 1 || c->W < 1) { set_error("udb_conv3x3_halo_f16: B=%d H=%d W=%d must be >= 1", c->B, c->H, c->W); return 1; }
+  if (!c->x || !c->w || !c->bias) { set_error("udb_conv3x3_halo_f16: null x / w / bias"); return 1; }
+  if (c->coff < 0 || (long long)c->coff + c->C > cs) {
+    set_error("udb_conv3x3_halo_f16: `coff`=%d + C=%d exceeds `cstride`=%d", c->coff, c->C, cs); return 1;
+  }
+  if (c->head_out) {
+    if (!c->head_w) { set_error("udb_conv3x3_halo_f16: `head_w` is null while head_out is set"); return 1; }
+    if (reinterpret_cast<uintptr_t>(c->head_out) & 3) { set_error("udb_conv3x3_halo_f16: `head_out` must be 4-byte aligned"); return 1; }
+  } else {
+    const long long ldc = c->ldc > 0 ? c->ldc : c->cout;
+    if (!c->out) { set_error("udb_conv3x3_halo_f16: `out` is null (and no head_out)"); return 1; }
+    if (reinterpret_cast<uintptr_t>(c->out) & 3) { set_error("udb_conv3x3_halo_f16: `out` %p must be 4-byte aligned", c->out); return 1; }
+    if ((ldc & 1) || ldc < c->cout) { set_error("udb_conv3x3_halo_f16: `ldc`=%lld must be even and >= cout=%d", ldc, c->cout); return 1; }
+  }
   HaloArgs a{};
   a.B = c->B; a.H = c->H; a.W = c->W;
   a.slabs = c->C / 64; a.coff = c->coff;

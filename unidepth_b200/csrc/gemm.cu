@@ -483,12 +483,104 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const Gem
   return check_launch("gemm_f16_kernel");
 }
 
+static bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
+// Layouts the epilogue's vector accesses and 32-bit row offsets can handle (include/udb.h, udb_gemm_t).  Host-only: runs
+// before any CUDA call, so a rejected call launches nothing.
+static int check_gemm_layout(const udb_gemm_t* g) {
+  const int sm = g->store_mode;
+  if (g->M < 1 || g->N < 1 || g->K < 1) { set_error("udb_gemm_f16: M=%d N=%d K=%d must be >= 1", g->M, g->N, g->K); return 1; }
+  if (sm < UDB_STORE_ROWS || sm > UDB_STORE_HEAD) { set_error("udb_gemm_f16: unknown store_mode %d", sm); return 1; }
+  const long long ldr = g->ldr > 0 ? g->ldr : g->ldc;
+  // every vector load / store of the epilogue: f32 rows move as float4, f16 rows as 4 halves (uint2)
+  if (sm == UDB_STORE_HEAD) {
+    if (!g->out || !g->out_f32 || !aligned(g->out, 4)) { set_error("udb_gemm_f16: HEAD store needs a 4-byte aligned f32 `out`"); return 1; }
+    if (!g->head_w || !aligned(g->head_w, 16)) { set_error("udb_gemm_f16: `head_w` must be non-null and 16-byte aligned"); return 1; }
+  } else {
+    if (g->out && !aligned(g->out, g->out_f32 ? 16 : 8)) {
+      set_error("udb_gemm_f16: `out` %p must be %d-byte aligned", g->out, g->out_f32 ? 16 : 8); return 1;
+    }
+    if (g->out2 && !aligned(g->out2, 8)) { set_error("udb_gemm_f16: `out2` %p must be 8-byte aligned", g->out2); return 1; }
+    if (g->resid && !aligned(g->resid, g->resid_f32 ? 16 : 8)) {
+      set_error("udb_gemm_f16: `resid` %p must be %d-byte aligned", g->resid, g->resid_f32 ? 16 : 8); return 1;
+    }
+    if (sm != UDB_STORE_CONVT) {   // CONVT addresses its pixels through ct_cout, not ldc / ldr
+      if ((g->out || g->out2) && (g->ldc < 1 || g->ldc % 4)) { set_error("udb_gemm_f16: `ldc`=%lld must be a positive multiple of 4", (long long)g->ldc); return 1; }
+      if (g->resid && (ldr < 1 || ldr % 4)) { set_error("udb_gemm_f16: `ldr`=%lld must be a positive multiple of 4", ldr); return 1; }
+      if ((g->out || g->out2) && g->ldc < (long long)g->N + g->out_split) {
+        set_error("udb_gemm_f16: `ldc`=%lld < N + out_split = %lld: rows would overlap", (long long)g->ldc, (long long)g->N + g->out_split);
+        return 1;
+      }
+      if (g->resid && ldr < g->N) { set_error("udb_gemm_f16: `ldr`=%lld < N=%d: residual rows would overlap", ldr, g->N); return 1; }
+    }
+  }
+  if (g->out_split < 0 || g->out_split % 4) { set_error("udb_gemm_f16: `out_split`=%d must be a non-negative multiple of 4", g->out_split); return 1; }
+  if (!aligned(g->bias, 16)) { set_error("udb_gemm_f16: `bias` %p must be 16-byte aligned", (const void*)g->bias); return 1; }
+  if (!aligned(g->gamma, 16)) { set_error("udb_gemm_f16: `gamma` %p must be 16-byte aligned", (const void*)g->gamma); return 1; }
+  if (!aligned(g->ln_c1, 16)) { set_error("udb_gemm_f16: `ln_c1` %p must be 16-byte aligned", (const void*)g->ln_c1); return 1; }
+  if (!aligned(g->ln_stats_out, 8) || !aligned(g->ln_stats_in, 8)) { set_error("udb_gemm_f16: `ln_stats_*` must be 8-byte aligned"); return 1; }
+
+  // the epilogue keeps each row's element offset in 32 bits (EpiWarp::roff_out / roff_res)
+  long long out_row = 0, res_row = 0;   // element offset of the last row written / read
+  if (sm == UDB_STORE_ROWS) {
+    const int m = g->M - 1;
+    long long orow = m;
+    if (g->rows_per_group > 0) {
+      if (g->group_stride < 0 || g->row_offset < 0) {
+        set_error("udb_gemm_f16: `group_stride`=%d and `row_offset`=%d must be >= 0", g->group_stride, g->row_offset); return 1;
+      }
+      const long long rpg = g->rows_per_group, grp = m / rpg;
+      orow = grp * g->group_stride + m % rpg + g->row_offset;
+      if (grp > 0 && (grp - 1) * g->group_stride + rpg - 1 + g->row_offset > orow) orow = (grp - 1) * g->group_stride + rpg - 1 + g->row_offset;
+    }
+    long long rrow = orow;
+    if (g->resid_mod > 0) {
+      if (g->resid_row_offset < 0) { set_error("udb_gemm_f16: `resid_row_offset`=%d must be >= 0", g->resid_row_offset); return 1; }
+      rrow = (long long)(g->resid_mod < g->M ? g->resid_mod : g->M) - 1 + g->resid_row_offset;
+    }
+    out_row = orow * g->ldc;
+    res_row = rrow * ldr;
+  } else if (sm == UDB_STORE_CONVT) {
+    if (g->ct_k < 1 || g->ct_h < 1 || g->ct_w < 1 || g->ct_pad < 0 || g->ct_cout < 1) {
+      set_error("udb_gemm_f16: CONVT geometry `ct_k`=%d `ct_h`=%d `ct_w`=%d `ct_pad`=%d `ct_cout`=%d", g->ct_k, g->ct_h, g->ct_w, g->ct_pad,
+                g->ct_cout);
+      return 1;
+    }
+    if (g->N != g->ct_k * g->ct_k * g->ct_cout) { set_error("udb_gemm_f16: CONVT needs N == ct_k^2 * ct_cout (N=%d)", g->N); return 1; }
+    const long long m = g->M - 1, hw = (long long)g->ct_h * g->ct_w, b = m / hw, r = m % hw, y = r / g->ct_w, x = r % g->ct_w;
+    const long long W2 = (long long)g->ct_w * g->ct_k + 2 * g->ct_pad, H2 = (long long)g->ct_h * g->ct_k + 2 * g->ct_pad;
+    out_row = res_row = ((b * H2 + y * g->ct_k + g->ct_pad) * W2 + x * g->ct_k + g->ct_pad) * g->ct_cout;
+  } else {
+    if (g->conv_B < 1 || g->conv_H < 1 || g->conv_W < 1) {
+      set_error("udb_gemm_f16: conv_B=%d conv_H=%d conv_W=%d must be >= 1", g->conv_B, g->conv_H, g->conv_W); return 1;
+    }
+    const long long last_px = (long long)g->conv_B * g->conv_H * g->conv_W - 1;
+    out_row = last_px * g->ldc;
+    res_row = last_px * ldr;
+  }
+  const long long lim = 1ll << 32;
+  if ((g->out || g->out2) && out_row >= lim) { set_error("udb_gemm_f16: `out` row offset %lld exceeds 2^32 elements", out_row); return 1; }
+  if (g->resid && res_row >= lim) { set_error("udb_gemm_f16: `resid` row offset %lld exceeds 2^32 elements", res_row); return 1; }
+
+  if (g->a_mode == UDB_A_CONV3X3) {
+    const int pad = g->conv_off == 0 ? 2 : (g->conv_off == -1 ? 0 : -1);
+    if (pad < 0) { set_error("udb_gemm_f16: `conv_off`=%d must be 0 (prepadded) or -1 (zero padding)", g->conv_off); return 1; }
+    if (g->conv_inH != g->conv_H + pad || g->conv_inW != g->conv_W + pad) {
+      set_error("udb_gemm_f16: `conv_inH`x`conv_inW` = %dx%d must be %dx%d for conv_off %d", g->conv_inH, g->conv_inW, g->conv_H + pad,
+                g->conv_W + pad, g->conv_off);
+      return 1;
+    }
+  }
+  return 0;
+}
+
 }  // namespace udb
 
 extern "C" int udb_gemm_f16(const udb_gemm_t* g, void* stream) {
   using namespace udb;
   if (!g || !g->a || !g->w) { set_error("udb_gemm_f16: null operand"); return 1; }
   if (g->N % 32 != 0) { set_error("udb_gemm_f16: N=%d must be a multiple of 32", g->N); return 1; }
+  if (check_gemm_layout(g)) return 1;
   GemmArgs a{};
   a.M = g->M; a.N = g->N; a.K = g->K;
   a.num_kb = (g->K + BK - 1) / BK;

@@ -46,6 +46,12 @@ def _ptr(t: Optional[torch.Tensor]):
     return C.c_void_p(t.data_ptr())
 
 
+def _unit_stride(*tensors):
+    """The kernels address every operand as rows of contiguous elements (vector loads / stores along the last dim)."""
+    for t in tensors:
+        assert t is None or t.stride(-1) == 1, f"udb ops need stride(-1) == 1, got strides {tuple(t.stride())}"
+
+
 def _is32(t):
     if t.dtype == f32:
         return 1
@@ -72,6 +78,7 @@ def gemm(a: torch.Tensor, w: torch.Tensor, *, bias=None, act=ACT_NONE, gamma=Non
     if out is None:
         out = torch.empty((out_rows if out_rows is not None else M, 2 * N if out_split else N), device=a.device,
                           dtype=f16 if out_split else out_dtype)
+    _unit_stride(out, out2, resid)
     g = cabi.Gemm()
     g.a, g.w = _ptr(a), _ptr(w)
     g.M, g.N, g.K = M, N, K
@@ -105,6 +112,7 @@ def conv3x3(x: torch.Tensor, w: torch.Tensor, *, bias=None, act=ACT_NONE, gamma=
     H, W = (inH - 2, inW - 2) if prepadded else (inH, inW)
     N = w.shape[0]
     assert w.shape[1] == 9 * Cin and c_off + Cin <= Ctot
+    _unit_stride(out, out2, resid)
     g = cabi.Gemm()
     g.a, g.w = _ptr(x), _ptr(w)
     g.M, g.N, g.K = B * H * W, N, 9 * Cin
@@ -145,6 +153,7 @@ def conv3x3_halo(x: torch.Tensor, w: torch.Tensor, *, bias, act=ACT_NONE, c_off=
     Cin = c_used if c_used is not None else Ctot
     H, W, N = PH - 2, PW - 2, w.shape[0]
     assert w.shape[1] == 9 * Cin
+    _unit_stride(out)
     c = cabi.ConvHalo()
     c.x, c.w, c.bias = _ptr(x), _ptr(w), _ptr(bias)
     c.B, c.H, c.W, c.C, c.cstride, c.coff, c.cout, c.act = B, H, W, Cin, Ctot, c_off, N, act
@@ -173,6 +182,7 @@ def conv_transpose_ks(x: torch.Tensor, w: torch.Tensor, k: int, cout: int, grid_
     B = M // (h * ww)
     if out is None:
         out = torch.empty((B, h * k + 2 * pad, ww * k + 2 * pad, cout), device=x.device, dtype=out_dtype)
+    _unit_stride(x, w, out, out2, resid)
     g = cabi.Gemm()
     g.a, g.w = _ptr(x), _ptr(w)
     g.M, g.N, g.K = M, k * k * cout, K
@@ -193,6 +203,7 @@ def conv_transpose_ks(x: torch.Tensor, w: torch.Tensor, k: int, cout: int, grid_
 def attention(q, k, v, out, *, B, heads, seq_q, seq_k, head_dim, q_col0=0, k_col0=0, v_col0=0, o_col0=0, scale=None,
               lo_off_in=0, lo_off_out=0):
     """lo_off_in > 0: split-f16 operands (lo halves lo_off_in columns to the right), fp32 CUDA-core kernel."""
+    _unit_stride(q, k, v, out)
     a = cabi.Attn()
     a.q, a.k, a.v, a.out = _ptr(q), _ptr(k), _ptr(v), _ptr(out)
     a.B, a.heads, a.seq_q, a.seq_k, a.head_dim = B, heads, seq_q, seq_k, head_dim
