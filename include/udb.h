@@ -129,6 +129,11 @@ typedef struct udb_gemm_t {
 } udb_gemm_t;
 
 int udb_gemm_f16(const udb_gemm_t* g, void* stream);
+/* Epilogue of the last udb_gemm_f16 call on the calling thread that got past its checks: 1 = the TMA-store epilogue
+ * (plain ROWS store with an identity row map, no out2 / out_split / ln_stats_*, 16-byte aligned out and row pitch, and
+ * a residual only as f32 with an f32 out), 0 = the general one.  Both give bit-identical outputs; setting the
+ * environment variable UDB_GEMM_TMA_EPILOGUE=0 routes every call to the general one. */
+int udb_gemm_tma_epilogue_used(void);
 
 /* ---------------------------------------------------------------------------------------------
  * 3x3 convolution with few output channels over a PRE-PADDED NHWC f16 image [B, H+2, W+2, cstride]

@@ -184,6 +184,7 @@ EXPORTS = {
     "udb_profile_begin": (i32, [vp]),
     "udb_profile_end": (i32, [C.POINTER(ProfileEntry), i32]),
     "udb_gemm_f16": (i32, [C.POINTER(Gemm), vp]),
+    "udb_gemm_tma_epilogue_used": (i32, []),
     "udb_conv3x3_halo_f16": (i32, [C.POINTER(ConvHalo), vp]),
     "udb_attention_f16": (i32, [C.POINTER(Attn), vp]),
     "udb_layernorm": (i32, [C.POINTER(LayerNorm), vp]),

@@ -91,8 +91,8 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
-int make_tmap_f16(CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
-                  const uint64_t* strides_bytes, const uint32_t* box, bool swizzle128) {
+int make_tmap(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+              const uint32_t* box, CUtensorMapDataType dtype, CUtensorMapSwizzle swizzle) {
   EncodeTiledFn fn = get_encode();
   if (!fn) return 1;
   cuuint64_t gdim[5];
@@ -115,10 +115,9 @@ int make_tmap_f16(CUtensorMap* map, const void* base, int rank, const uint64_t* 
       return 1;
     }
   }
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(base),
-                  gdim, gstr, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = fn(map, dtype, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx, es,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("cuTensorMapEncodeTiled failed: CUresult %d (rank %d dims %llu,%llu box %u,%u)", (int)r,
               rank, (unsigned long long)dims[0], (unsigned long long)(rank > 1 ? dims[1] : 0), box[0],

@@ -64,7 +64,12 @@ inline cudaError_t launch_ex(Kernel kernel, dim3 grid, dim3 block, size_t smem, 
 
 // cuTensorMapEncodeTiled through the runtime's driver entry point (no link-time libcuda).
 // dims/strides innermost first; strides_bytes has rank-1 entries (stride of dim 1..rank-1).
-int make_tmap_f16(CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
-                  const uint64_t* strides_bytes, const uint32_t* box, bool swizzle128);
+int make_tmap(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+              const uint32_t* box, CUtensorMapDataType dtype, CUtensorMapSwizzle swizzle);
+inline int make_tmap_f16(CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
+                         const uint64_t* strides_bytes, const uint32_t* box, bool swizzle128) {
+  return make_tmap(map, base, rank, dims, strides_bytes, box, CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
+                   swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE);
+}
 
 }  // namespace udb

@@ -11,6 +11,16 @@
 // NHWC image (4-D tensor map, one (dy,dx,64-channel) slab per k-block; zero padding comes from TMA
 // out-of-bounds fill), so linear layers, 1x1 / 3x3 convolutions and k=s transposed convolutions all
 // run through this one kernel.  See include/udb.h (udb_gemm) for the reference call sites.
+//
+// Two epilogues.  The general one (epilogue_tile) transposes each 32-column chunk through per-warp shared-memory tiles
+// and stores rows with st.global; it serves every store mode.  The TMA epilogue (epilogue_tile_tma; plain ROWS stores
+// with an identity row map, see tma_epilogue_ok) stages each warpgroup's 64 x 32 chunk in a swizzled box, stores it with
+// an asynchronous TMA store and goes on to the next chunk / tile's MMAs while the store drains; warp 9 of the producer
+// warpgroup prefetches the f32 residual into the same boxes.  Both run the same per-element arithmetic, so their
+// outputs are bit-identical.
+#include <stdlib.h>
+#include <string.h>
+
 #include "common.h"
 #include "ptx.cuh"
 
@@ -57,19 +67,38 @@ struct GemmArgs {
   float ln_eps;
 };
 
-template <int BN>
+// TMA epilogue staging box: one warpgroup's 64 rows x 32 columns, f32 (128 B rows, 128B swizzle) or f16 (64 B rows,
+// 64B swizzle, first half of the box).  Two buffers; buffer b holds both warpgroups' boxes back to back, so one 128-row
+// TMA load fills it with a residual chunk of the whole tile.
+constexpr int kEpiBox = 64 * 32 * 4;
+
+template <int BN, bool TMAE = false>
 struct GemmCfg {
   // as many operand stages as fit next to the epilogue staging in 227 KB
-  static constexpr int kStages = BN >= 256 ? 3 : (BN >= 192 ? 4 : (BN >= 128 ? 5 : 7));
+  static constexpr int kStages = TMAE ? (BN >= 192 ? 4 : (BN >= 128 ? 6 : 8))
+                                      : (BN >= 256 ? 3 : (BN >= 192 ? 4 : (BN >= 128 ? 5 : 7)));
   static constexpr int kABytes = BM * BK * 2;
   static constexpr int kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
   // epilogue staging: per epilogue warp a 32x32 f32 transpose tile and 2 x 32 row offsets, so that global loads/stores
-  // are row-contiguous (coalesced) per instruction
-  static constexpr int kStagingBytes = kEpiWarps * (32 * kTP * 4 + 2 * 32 * 4);
+  // are row-contiguous (coalesced) per instruction -- or, for the TMA epilogue, 2 buffers x 2 warpgroups x kEpiBox
+  static constexpr int kStagingBytes = TMAE ? 2 * 2 * kEpiBox : kEpiWarps * (32 * kTP * 4 + 2 * 32 * 4);
   static constexpr int kSmemBytes = kStages * kStageBytes + kStagingBytes + 256 /*barriers*/;
   static_assert(kSmemBytes <= 232448, "shared memory per block");
+  static_assert(2 * kStages + 4 <= 32, "barriers");
 };
+
+// The activation step of the epilogue arithmetic (bias -> activation -> gamma -> + residual), shared by both epilogues.
+template <int N>
+__device__ __forceinline__ void apply_act(const int act, float (&v)[N]) {
+  if (act == UDB_ACT_GELU) {
+#pragma unroll
+    for (int j = 0; j < N; j += 2) gelu_erf_pair(v[j], v[j + 1]);
+  } else if (act == UDB_ACT_LEAKY) {
+#pragma unroll
+    for (int j = 0; j < N; ++j) v[j] = leaky(v[j]);
+  }
+}
 
 // One accumulator tile (128 rows x BN columns; warpgroup g holds rows [64g, 64g+64) in registers) -> global memory.
 // `mt` indexes this CTA's 128-row block (matrix rows mt*128.. or spatial conv tile mt), `nt` the BN-wide column block.
@@ -196,13 +225,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmArgs& p, const EpiWarp& 
         v[4 * j] += b4.x; v[4 * j + 1] += b4.y; v[4 * j + 2] += b4.z; v[4 * j + 3] += b4.w;
       }
     }
-    if (p.act == UDB_ACT_GELU) {
-#pragma unroll
-      for (int j = 0; j < 32; j += 2) gelu_erf_pair(v[j], v[j + 1]);
-    } else if (p.act == UDB_ACT_LEAKY) {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = leaky(v[j]);
-    }
+    apply_act(p.act, v);
     if (p.store_mode == UDB_STORE_HEAD) {
       float head = p.head_b;
 #pragma unroll
@@ -346,11 +369,105 @@ __device__ __forceinline__ void epilogue_tile(const GemmArgs& p, const EpiWarp& 
   }
 }
 
-template <int BN, bool LNF>
+// Shared-memory state of the TMA epilogue.  `chunk` counts this warpgroup's 32-column chunks over all its tiles; chunk i
+// uses buffer i & 1.  With a residual, the residual producer (warp 9) fills a buffer (full[b], expect_tx) once both
+// warpgroups have released it (empty[b], one arrival per warpgroup after its TMA store has read the box).
+struct EpiTma {
+  uint8_t* buf;        // [2 buffers][2 warpgroups][kEpiBox]
+  uint64_t* full;      // [2]
+  uint64_t* empty;     // [2]
+  uint32_t chunk;
+};
+
+// TMA epilogue of one tile (ROWS store, identity row map; udb_gemm_f16 checks the conditions in tma_epilogue_ok).
+// Thread (warp wq, lane) of warpgroup g holds rows 16 wq + lane / 4 (+ 8) and columns 8 j + 2 (lane % 4) (+ 1) of every
+// 32-column chunk; it applies the epilogue arithmetic there and writes the result into the swizzled box, one elected
+// thread per warpgroup stores the box with TMA.  Rows past M are clipped by the tensor map.
+template <int BN>
+__device__ __forceinline__ void epilogue_tile_tma(const GemmArgs& p, const CUtensorMap* tmC, EpiTma& e,
+                                                  const float (&acc)[BN / 2], const int mt, const int nt, const int wg,
+                                                  const int wq, const int lane) {
+  const bool leader = wq == 0 && lane == 0;   // issues, commits and waits for this warpgroup's stores
+  const int q = lane & 3, rr = lane >> 2;     // rr == row & 7 for both fragment rows
+  const bool has_res = p.resid != nullptr;
+  const int row0 = mt * BM + 64 * wg;
+#pragma unroll
+  for (int c = 0; c < BN / 32; ++c, ++e.chunk) {
+    const int b = e.chunk & 1;
+    uint8_t* box = e.buf + (2 * b + wg) * kEpiBox;
+    if (has_res) {
+      mbar_wait(&e.full[b], (e.chunk >> 1) & 1);   // residual chunk landed (and the box's previous store has read it)
+    } else {
+      if (leader) bulk_wait_read<1>();             // the store issued from this box two chunks ago has read it
+      bar_sync(1 + wg, 128);
+    }
+    const int n0 = nt * BN + 32 * c;
+    float v[16];   // v[4 j + 2 h + x]: row 16 wq + rr + 8 h, column n0 + 8 j + 2 q + x
+#pragma unroll
+    for (int j = 0; j < 16; ++j) v[j] = acc[16 * c + j];
+    if (p.bias) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 b2 = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + 8 * j + 2 * q));
+        v[4 * j] += b2.x; v[4 * j + 1] += b2.y; v[4 * j + 2] += b2.x; v[4 * j + 3] += b2.y;
+      }
+    }
+    apply_act(p.act, v);
+    if (p.gamma) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 g2 = __ldg(reinterpret_cast<const float2*>(p.gamma + n0 + 8 * j + 2 * q));
+        v[4 * j] *= g2.x; v[4 * j + 1] *= g2.y; v[4 * j + 2] *= g2.x; v[4 * j + 3] *= g2.y;
+      }
+    }
+    if (p.out_f32) {
+      // 128B swizzle: 16-byte unit u of row r sits at unit u ^ (r & 7); conflict-free 8-byte accesses
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = 16 * wq + rr + 8 * h;
+          float2* s = reinterpret_cast<float2*>(box + r * 128 + (((2 * j + (q >> 1)) ^ rr) << 4) + 8 * (q & 1));
+          float x0 = v[4 * j + 2 * h], x1 = v[4 * j + 2 * h + 1];
+          if (has_res) {
+            const float2 t = *s;
+            x0 += t.x; x1 += t.y;
+          }
+          *s = make_float2(x0, x1);
+        }
+      }
+    } else {
+      // 64B swizzle: 16-byte unit u of row r sits at unit u ^ ((r >> 1) & 3)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = 16 * wq + rr + 8 * h;
+          *reinterpret_cast<uint32_t*>(box + r * 64 + ((j ^ ((r >> 1) & 3)) << 4) + 4 * q) =
+              pack_half2(v[4 * j + 2 * h], v[4 * j + 2 * h + 1]);
+        }
+      }
+    }
+    fence_proxy_async_smem();   // the box's generic-proxy writes -> visible to the TMA store
+    bar_sync(1 + wg, 128);
+    if (leader) {
+      if (row0 < p.M) tma_store_2d(tmC, box, n0, row0);
+      bulk_commit();
+      if (has_res) {
+        bulk_wait_read<0>();
+        mbar_arrive(&e.empty[b]);
+      }
+    }
+  }
+}
+
+// TMAE: TMA epilogue (tmC: `out`, box 32 x 64; tmR: f32 `resid`, box 32 x 128; both unused otherwise)
+template <int BN, bool LNF, bool TMAE>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                const GemmArgs p) {
-  using Cfg = GemmCfg<BN>;
+                const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR, const GemmArgs p) {
+  static_assert(!(TMAE && LNF), "the TMA epilogue carries no fused-LayerNorm code");
+  using Cfg = GemmCfg<BN, TMAE>;
   constexpr int kStages = Cfg::kStages;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sA = smem;
@@ -359,6 +476,8 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   uint64_t* bars = reinterpret_cast<uint64_t*>(staging + Cfg::kStagingBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + kStages;
+  uint64_t* epi_full = bars + 2 * kStages;    // TMA epilogue: [2] residual chunk landed in buffer b
+  uint64_t* epi_empty = epi_full + 2;         //               [2] both warpgroups' stores have read buffer b
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -372,6 +491,14 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], kEpiWarps);   // every consumer warp releases the stage after its own wgmma wait
     }
+    if constexpr (TMAE) {
+      prefetch_tmap(&tmC);
+      if (p.resid) prefetch_tmap(&tmR);
+      for (int i = 0; i < 2; ++i) {
+        mbar_init(&epi_full[i], 1);
+        mbar_init(&epi_empty[i], 2);
+      }
+    }
     fence_barrier_init();
   }
   __syncthreads();
@@ -381,6 +508,28 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 
   if (warp >= kEpiWarps) {
     setmaxnreg_dec<40>();
+    if constexpr (TMAE) {
+      if (warp == kEpiWarps + 1 && p.resid) {
+        // ---------------------------------------------------------------- residual producer (TMA epilogue)
+        // Loads every 32-column residual chunk of this CTA's tiles, in the order the consumers store them, as soon as
+        // the buffer is free; the first two chunks of a tile so arrive during its main loop.
+        const bool elected = elect_one();
+        uint32_t chunk = 0;
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+          const int mt = tile / p.tiles_n;
+          const int nt = tile % p.tiles_n;
+          for (int c = 0; c < BN / 32; ++c, ++chunk) {
+            const int b = chunk & 1;
+            mbar_wait(&epi_empty[b], ((chunk >> 1) & 1) ^ 1);
+            if (elected) {
+              mbar_arrive_expect_tx(&epi_full[b], 2 * kEpiBox);
+              tma_load_2d(staging + 2 * b * kEpiBox, &tmR, &epi_full[b], nt * BN + 32 * c, mt * BM);
+            }
+            __syncwarp();
+          }
+        }
+      }
+    }
     if (warp != kEpiWarps) return;
     // ------------------------------------------------------------------ TMA producer
     // (whole warp in the control flow, one elected lane issues: keeps addresses/descriptors in uniform
@@ -428,6 +577,7 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     float* Twg = reinterpret_cast<float*>(staging) + wg * 4 * 32 * kTP;
     uint32_t* roff = reinterpret_cast<uint32_t*>(staging + kEpiWarps * 32 * kTP * 4) + warp * 64;
     const EpiWarp ctx{Twg + wq * 32 * kTP, Twg, roff, roff + 32, wg, wq, wq >> 1, lane, 64 * wg + 32 * (wq & 1) + lane};
+    EpiTma etma{staging, epi_full, epi_empty, 0};
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
@@ -456,17 +606,22 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
       if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
-      epilogue_tile<BN, LNF>(p, ctx, acc, mt, nt);
+      if constexpr (TMAE) epilogue_tile_tma<BN>(p, &tmC, etma, acc, mt, nt, wg, wq, lane);
+      else epilogue_tile<BN, LNF>(p, ctx, acc, mt, nt);
+    }
+    if constexpr (TMAE) {
+      if (wq == 0 && lane == 0) bulk_wait<0>();   // the last stores have written global memory before the CTA retires
     }
   }
 }
 
-template <int BN, bool LNF>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmArgs& a, cudaStream_t st) {
-  using Cfg = GemmCfg<BN>;
+template <int BN, bool LNF, bool TMAE>
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const CUtensorMap& tmR,
+                       const GemmArgs& a, cudaStream_t st) {
+  using Cfg = GemmCfg<BN, TMAE>;
   static std::atomic<uint64_t> attr_mask{0};
   if (first_on_device(attr_mask)) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_f16_kernel<BN, LNF>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(gemm_f16_kernel<BN, LNF, TMAE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          Cfg::kSmemBytes);
     if (e != cudaSuccess) {
       set_error("gemm: cudaFuncSetAttribute(%d B smem): %s", Cfg::kSmemBytes, cudaGetErrorString(e));
@@ -475,7 +630,8 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const Gem
   }
   const int tiles = a.tiles_m * a.tiles_n;
   const int grid = tiles < num_sms() ? tiles : num_sms();
-  cudaError_t e = launch_ex(gemm_f16_kernel<BN, LNF>, dim3(grid), dim3(kThreads), Cfg::kSmemBytes, st, 1, tmA, tmB, a);
+  cudaError_t e = launch_ex(gemm_f16_kernel<BN, LNF, TMAE>, dim3(grid), dim3(kThreads), Cfg::kSmemBytes, st, 1, tmA, tmB, tmC,
+                            tmR, a);
   if (e != cudaSuccess) {
     set_error("gemm_f16_kernel launch: %s", cudaGetErrorString(e));
     return 1;
@@ -574,7 +730,25 @@ static int check_gemm_layout(const udb_gemm_t* g) {
   return 0;
 }
 
+// Calls the TMA epilogue serves: a plain ROWS store (identity row map, no second output, split output or fused LayerNorm
+// statistics) whose `out` -- and f32 `resid`, if any, with an f32 `out` -- TMA can address: 16-byte aligned bases and row
+// pitches.  The rest run the general epilogue; this only chooses the path and never fails a call.
+// UDB_GEMM_TMA_EPILOGUE=0 (read on every call) sends every call to the general epilogue, for A/B comparisons.
+static bool tma_epilogue_ok(const udb_gemm_t* g) {
+  const char* env = getenv("UDB_GEMM_TMA_EPILOGUE");
+  if (env && atoi(env) == 0) return false;
+  if (g->store_mode != UDB_STORE_ROWS || g->a_mode != UDB_A_MATRIX || g->rows_per_group > 0 || g->resid_mod > 0) return false;
+  if (g->out_split || g->out2 || g->ln_stats_out || g->ln_stats_in || !g->out) return false;
+  if (!aligned(g->out, 16) || (g->ldc * (g->out_f32 ? 4 : 2)) % 16) return false;
+  const long long ldr = g->ldr > 0 ? g->ldr : g->ldc;
+  return !g->resid || (g->resid_f32 && g->out_f32 && aligned(g->resid, 16) && (ldr * 4) % 16 == 0);
+}
+
+static thread_local int g_last_tma_epilogue = 0;
+
 }  // namespace udb
+
+extern "C" int udb_gemm_tma_epilogue_used(void) { return udb::g_last_tma_epilogue; }
 
 extern "C" int udb_gemm_f16(const udb_gemm_t* g, void* stream) {
   using namespace udb;
@@ -680,6 +854,24 @@ extern "C" int udb_gemm_f16(const udb_gemm_t* g, void* stream) {
     const uint32_t box[2] = {(uint32_t)BK, (uint32_t)bn};
     if (make_tmap_f16(&tmB, g->w, 2, dims, str, box, true)) return 1;
   }
+  const bool tmae = tma_epilogue_ok(g);
+  CUtensorMap tmC, tmR;
+  memset(&tmC, 0, sizeof(tmC));
+  memset(&tmR, 0, sizeof(tmR));
+  if (tmae) {
+    const uint64_t dims[2] = {(uint64_t)g->N, (uint64_t)g->M};
+    const uint64_t str_c[1] = {(uint64_t)g->ldc * (g->out_f32 ? 4 : 2)};
+    const uint32_t box_c[2] = {32, 64};
+    if (make_tmap(&tmC, g->out, 2, dims, str_c, box_c, g->out_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
+                  g->out_f32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B))
+      return 1;
+    if (g->resid) {
+      const uint64_t str_r[1] = {(uint64_t)a.ldr * 4};
+      const uint32_t box_r[2] = {32, BM};
+      if (make_tmap(&tmR, g->resid, 2, dims, str_r, box_r, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, CU_TENSOR_MAP_SWIZZLE_128B)) return 1;
+    }
+  }
+  g_last_tma_epilogue = tmae ? 1 : 0;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   note_work(2.0 * a.M * (double)g->N * g->K,
             2.0 * ((double)a.M * (g->a_mode == UDB_A_CONV3X3 ? g->conv_C : (g->a_split_k ? 2 * g->a_split_k : g->K)) + (double)g->N * g->K) +
@@ -687,18 +879,27 @@ extern "C" int udb_gemm_f16(const udb_gemm_t* g, void* stream) {
   const bool lnf = g->ln_stats_out || g->ln_stats_in;
   if (lnf) {
     switch (bn) {
-      case 256: return launch_gemm<256, true>(tmA, tmB, a, st);
-      case 192: return launch_gemm<192, true>(tmA, tmB, a, st);
-      case 128: return launch_gemm<128, true>(tmA, tmB, a, st);
-      case 64: return launch_gemm<64, true>(tmA, tmB, a, st);
-      default: return launch_gemm<32, true>(tmA, tmB, a, st);
+      case 256: return launch_gemm<256, true, false>(tmA, tmB, tmC, tmR, a, st);
+      case 192: return launch_gemm<192, true, false>(tmA, tmB, tmC, tmR, a, st);
+      case 128: return launch_gemm<128, true, false>(tmA, tmB, tmC, tmR, a, st);
+      case 64: return launch_gemm<64, true, false>(tmA, tmB, tmC, tmR, a, st);
+      default: return launch_gemm<32, true, false>(tmA, tmB, tmC, tmR, a, st);
+    }
+  }
+  if (tmae) {
+    switch (bn) {
+      case 256: return launch_gemm<256, false, true>(tmA, tmB, tmC, tmR, a, st);
+      case 192: return launch_gemm<192, false, true>(tmA, tmB, tmC, tmR, a, st);
+      case 128: return launch_gemm<128, false, true>(tmA, tmB, tmC, tmR, a, st);
+      case 64: return launch_gemm<64, false, true>(tmA, tmB, tmC, tmR, a, st);
+      default: return launch_gemm<32, false, true>(tmA, tmB, tmC, tmR, a, st);
     }
   }
   switch (bn) {
-    case 256: return launch_gemm<256, false>(tmA, tmB, a, st);
-    case 192: return launch_gemm<192, false>(tmA, tmB, a, st);
-    case 128: return launch_gemm<128, false>(tmA, tmB, a, st);
-    case 64: return launch_gemm<64, false>(tmA, tmB, a, st);
-    default: return launch_gemm<32, false>(tmA, tmB, a, st);
+    case 256: return launch_gemm<256, false, false>(tmA, tmB, tmC, tmR, a, st);
+    case 192: return launch_gemm<192, false, false>(tmA, tmB, tmC, tmR, a, st);
+    case 128: return launch_gemm<128, false, false>(tmA, tmB, tmC, tmR, a, st);
+    case 64: return launch_gemm<64, false, false>(tmA, tmB, tmC, tmR, a, st);
+    default: return launch_gemm<32, false, false>(tmA, tmB, tmC, tmR, a, st);
   }
 }
