@@ -454,16 +454,21 @@ int udb_v1_postprocess(const udb_v1_postprocess_t* p, void* stream);
 /* ---------------------------------------------------------------------------------------------
  * Output assembly (unidepthv2.py:80-89, 311-339, 375-377; unidepthv2/decoder.py:456-462):
  * radius/confidence f32 [B,net_h,net_w] (already exp'ed), rays from intr4 (or rays_in) ->
- * points = rays*radius -> bilinear (align_corners=False) to (padded_h, padded_w) -> crop pads ->
- * confidence[B,1,H,W], radius[B,1,H,W]=|points|, depth[B,1,H,W]=points.z, points[B,3,H,W],
- * rays[B,3,H,W] renormalised.  All f32.
+ * points = rays*radius -> resize (F.interpolate(mode, align_corners=False), no antialias) to
+ * (padded_h, padded_w) -> crop pads -> confidence[B,1,H,W], radius[B,1,H,W]=|points|,
+ * depth[B,1,H,W]=points.z, points[B,3,H,W], rays[B,3,H,W] renormalised.  All f32.
+ * mode: the reference's `interpolation_mode` (unidepthv2.py:80-89), UDB_INTERP_BILINEAR (0) or
+ * UDB_INTERP_BICUBIC (1, ATen upsample_bicubic2d: A = -0.75, border taps clamped; the result is not
+ * clamped, so depth and confidence can overshoot to <= 0 at edges).  Any other value fails before launch.
  * ------------------------------------------------------------------------------------------- */
+enum { UDB_INTERP_BILINEAR = 0, UDB_INTERP_BICUBIC = 1 };
 typedef struct udb_postprocess_t {
   const float* radius;
   const float* confidence;
   const float* intr4;
   const float* rays_in; /* optional [B, net_h*net_w, 3] */
   int32_t B, net_h, net_w, padded_h, padded_w, pad_l, pad_t, H, W;
+  int32_t mode;         /* UDB_INTERP_*; fills the alignment slot before the output pointers (the size is unchanged) */
   float* out_confidence;
   float* out_radius;
   float* out_depth;
@@ -546,6 +551,8 @@ typedef struct udb_infer_args_t {
   int32_t rgb_is_u8, normalize;
   int32_t B, H, W;
   int32_t resolution_level;   /* 0..9 or -1 */
+  int32_t interpolation;      /* UDB_INTERP_* of the output resize (the reference's `interpolation_mode`); 0, what a
+                                 zero-initialised struct holds, is bilinear, the reference's default */
   const float* camera_k;      /* optional [B,3,3] pinhole K in input-image pixels (infer(camera=K),
                                  unidepthv2.py:267-303): rays come from it, intrinsics stay predicted */
   const float* camera_rays;   /* optional [B, net_h*net_w, 3] unit rays at network-input resolution produced by the

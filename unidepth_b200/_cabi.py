@@ -12,6 +12,8 @@ LIB_PATH = os.environ.get("UDB_LIB", os.path.join(_HERE, "libudb.so"))   # UDB_L
 A_MATRIX, A_CONV3X3 = 0, 1
 ACT_NONE, ACT_GELU, ACT_LEAKY = 0, 1, 2
 STORE_ROWS, STORE_CONVT, STORE_CONVTILE, STORE_HEAD = 0, 1, 2, 3
+INTERP_BILINEAR, INTERP_BICUBIC = 0, 1
+INTERP_MODES = {"bilinear": INTERP_BILINEAR, "bicubic": INTERP_BICUBIC}
 
 vp, i32, i64, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_float
 
@@ -89,6 +91,7 @@ class Postprocess(C.Structure):
         ("radius", vp), ("confidence", vp), ("intr4", vp), ("rays_in", vp),
         ("B", i32), ("net_h", i32), ("net_w", i32), ("padded_h", i32), ("padded_w", i32),
         ("pad_l", i32), ("pad_t", i32), ("H", i32), ("W", i32),
+        ("mode", i32),
         ("out_confidence", vp), ("out_radius", vp), ("out_depth", vp), ("out_points", vp), ("out_rays", vp),
     ]
 
@@ -119,7 +122,7 @@ class V1Geometry(C.Structure):
 class InferArgs(C.Structure):
     _fields_ = [
         ("rgb", vp), ("rgb_is_u8", i32), ("normalize", i32), ("B", i32), ("H", i32), ("W", i32),
-        ("resolution_level", i32), ("camera_k", vp), ("camera_rays", vp), ("ray_scales", vp), ("workspace", vp),
+        ("resolution_level", i32), ("interpolation", i32), ("camera_k", vp), ("camera_rays", vp), ("ray_scales", vp), ("workspace", vp),
         ("workspace_bytes", C.c_size_t),
         ("confidence", vp), ("intrinsics", vp), ("radius", vp), ("depth", vp), ("points", vp), ("rays", vp),
         ("depth_features", vp),

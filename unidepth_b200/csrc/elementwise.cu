@@ -531,6 +531,23 @@ __global__ void __launch_bounds__(256) reflect_border_fill_kernel(uint4* __restr
 }
 
 // ------------------------------------------------------------------------------------ output assembly
+// radius = |points|, depth = points.z, rays / max(|rays|, 1e-5) of one resampled output pixel
+__device__ __forceinline__ void store_outputs(const udb_postprocess_t& p, int b, int y, int x, float conf, float px, float py,
+                                              float pz, float rx, float ry, float rz) {
+  const long long plane = (long long)p.H * p.W;
+  const long long pix = (long long)y * p.W + x;
+  p.out_confidence[b * plane + pix] = conf;
+  p.out_radius[b * plane + pix] = sqrtf(px * px + py * py + pz * pz);
+  p.out_depth[b * plane + pix] = pz;
+  p.out_points[(b * 3 + 0) * plane + pix] = px;
+  p.out_points[(b * 3 + 1) * plane + pix] = py;
+  p.out_points[(b * 3 + 2) * plane + pix] = pz;
+  const float rn = fmaxf(sqrtf(rx * rx + ry * ry + rz * rz), 1e-5f);
+  p.out_rays[(b * 3 + 0) * plane + pix] = rx / rn;
+  p.out_rays[(b * 3 + 1) * plane + pix] = ry / rn;
+  p.out_rays[(b * 3 + 2) * plane + pix] = rz / rn;
+}
+
 __global__ void __launch_bounds__(256) postprocess_kernel(const udb_postprocess_t p) {
   const long long total = (long long)p.B * p.H * p.W;
   const float sh = (float)p.net_h / (float)p.padded_h, sw = (float)p.net_w / (float)p.padded_w;
@@ -563,18 +580,59 @@ __global__ void __launch_bounds__(256) postprocess_kernel(const udb_postprocess_
       conf += wy[a] * c_r; px += wy[a] * px_r; py += wy[a] * py_r; pz += wy[a] * pz_r;
       rx += wy[a] * rx_r; ry += wy[a] * ry_r; rz += wy[a] * rz_r;
     }
-    const long long plane = (long long)p.H * p.W;
-    const long long pix = (long long)y * p.W + x;
-    p.out_confidence[b * plane + pix] = conf;
-    p.out_radius[b * plane + pix] = sqrtf(px * px + py * py + pz * pz);
-    p.out_depth[b * plane + pix] = pz;
-    p.out_points[(b * 3 + 0) * plane + pix] = px;
-    p.out_points[(b * 3 + 1) * plane + pix] = py;
-    p.out_points[(b * 3 + 2) * plane + pix] = pz;
-    const float rn = fmaxf(sqrtf(rx * rx + ry * ry + rz * rz), 1e-5f);
-    p.out_rays[(b * 3 + 0) * plane + pix] = rx / rn;
-    p.out_rays[(b * 3 + 1) * plane + pix] = ry / rn;
-    p.out_rays[(b * 3 + 2) * plane + pix] = rz / rn;
+    store_outputs(p, b, y, x, conf, px, py, pz, rx, ry, rz);
+  }
+}
+
+// ATen upsample_bicubic2d (align_corners=False): source index scale*(dst+0.5)-0.5 NOT clamped at 0, x0 = floor,
+// taps x0-1 .. x0+2 clamped to [0, in-1], Keys coefficients (A = -0.75) in get_cubic_upsample_coefficients' order.
+__device__ __forceinline__ void bicubic_src(float scale, int dst, int in_size, int (&idx)[4], float (&w)[4]) {
+  const float src = scale * ((float)dst + 0.5f) - 0.5f;
+  const float f = floorf(src);
+  const float t = src - f;
+  const int i0 = (int)f;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) idx[k] = min(max(i0 - 1 + k, 0), in_size - 1);
+  const float A = -0.75f;
+  const float t2 = 1.f - t;
+  w[0] = cubic2(t + 1.f, A); w[1] = cubic1(t, A); w[2] = cubic1(t2, A); w[3] = cubic2(t2 + 1.f, A);
+}
+
+// Same fusion as postprocess_kernel (points = rays*radius per tap; confidence, points and rays resampled with the same
+// weights; radius / depth / ray normalisation afterwards), bicubic weights: per output pixel, four horizontal 1-D
+// interpolations of the seven channels (one per tap row), then one vertical, in the order of ATen's CUDA kernel.
+// No clamping of the result: near depth edges the overshoot can make depth and confidence <= 0, as in the reference.
+__global__ void __launch_bounds__(256) postprocess_bicubic_kernel(const udb_postprocess_t p) {
+  const long long total = (long long)p.B * p.H * p.W;
+  const float sh = (float)p.net_h / (float)p.padded_h, sw = (float)p.net_w / (float)p.padded_w;
+  for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
+       idx += (long long)gridDim.x * blockDim.x) {
+    const int x = (int)(idx % p.W), y = (int)((idx / p.W) % p.H), b = (int)(idx / ((long long)p.W * p.H));
+    int ys[4], xs[4];
+    float wy[4], wx[4];
+    bicubic_src(sh, y + p.pad_t, p.net_h, ys, wy);
+    bicubic_src(sw, x + p.pad_l, p.net_w, xs, wx);
+    float4 k = make_float4(1.f, 1.f, 0.f, 0.f);
+    if (!p.rays_in) k = *reinterpret_cast<const float4*>(p.intr4 + b * 4);
+    float conf = 0.f, px = 0.f, py = 0.f, pz = 0.f, rx = 0.f, ry = 0.f, rz = 0.f;
+#pragma unroll
+    for (int a = 0; a < 4; ++a) {
+      float c_r = 0.f, px_r = 0.f, py_r = 0.f, pz_r = 0.f, rx_r = 0.f, ry_r = 0.f, rz_r = 0.f;
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        const long long o = ((long long)b * p.net_h + ys[a]) * p.net_w + xs[c];
+        float3 r;
+        if (p.rays_in) { const float* rp = p.rays_in + o * 3; r = make_float3(rp[0], rp[1], rp[2]); }
+        else r = unit_ray(k, ys[a], xs[c]);
+        const float rad = p.radius[o];
+        c_r += p.confidence[o] * wx[c];
+        px_r += (r.x * rad) * wx[c]; py_r += (r.y * rad) * wx[c]; pz_r += (r.z * rad) * wx[c];
+        rx_r += r.x * wx[c]; ry_r += r.y * wx[c]; rz_r += r.z * wx[c];
+      }
+      conf += c_r * wy[a]; px += px_r * wy[a]; py += py_r * wy[a]; pz += pz_r * wy[a];
+      rx += rx_r * wy[a]; ry += ry_r * wy[a]; rz += rz_r * wy[a];
+    }
+    store_outputs(p, b, y, x, conf, px, py, pz, rx, ry, rz);
   }
 }
 
@@ -743,7 +801,16 @@ extern "C" int udb_reflect_border_fill_nhwc_f16(void* buf, int32_t B, int32_t H,
 }
 
 extern "C" int udb_postprocess(const udb_postprocess_t* p, void* stream) {
+  if (p->mode != UDB_INTERP_BILINEAR && p->mode != UDB_INTERP_BICUBIC) {
+    set_error("udb_postprocess: `mode` %d is neither UDB_INTERP_BILINEAR (0) nor UDB_INTERP_BICUBIC (1)", p->mode);
+    return 1;
+  }
   note_work(0.0, 4.0 * p->B * (2.0 * p->net_h * p->net_w + 9.0 * p->H * p->W));
-  postprocess_kernel<<<grid_for((long long)p->B * p->H * p->W), 256, 0, ST(stream)>>>(*p);
+  const int grid = grid_for((long long)p->B * p->H * p->W);
+  if (p->mode == UDB_INTERP_BICUBIC) {
+    postprocess_bicubic_kernel<<<grid, 256, 0, ST(stream)>>>(*p);
+    return check_launch("postprocess_bicubic_kernel");
+  }
+  postprocess_kernel<<<grid, 256, 0, ST(stream)>>>(*p);
   return check_launch("postprocess_kernel");
 }

@@ -316,6 +316,7 @@ static int run(udb_engine* e, const udb_infer_args_t& a, const udb_geometry_t& g
     p.B = B; p.net_h = nh; p.net_w = nw; p.padded_h = g.padded_h; p.padded_w = g.padded_w; p.pad_l = g.pad_l; p.pad_t = g.pad_t;
     p.H = a.H; p.W = a.W;
     p.out_confidence = a.confidence; p.out_radius = a.radius; p.out_depth = a.depth; p.out_points = a.points; p.out_rays = a.rays;
+    p.mode = a.interpolation;
     c.done(udb_postprocess(&p, st));
   }
   if (!c.rc && ar.overflow) { set_error("engine: workspace too small (%zu bytes needed)", ar.peak); return 1; }
@@ -467,6 +468,10 @@ int udb_infer_v2(udb_engine* e, const udb_infer_args_t* a, void* stream) {
   if (!e || !a || !a->rgb || !a->workspace) { set_error("udb_infer_v2: null argument"); return 1; }
   if (!a->confidence || !a->intrinsics || !a->radius || !a->depth || !a->points || !a->rays || !a->depth_features) {
     set_error("udb_infer_v2: all seven output pointers are required");
+    return 1;
+  }
+  if (a->interpolation != UDB_INTERP_BILINEAR && a->interpolation != UDB_INTERP_BICUBIC) {
+    set_error("udb_infer_v2: `interpolation` %d is neither UDB_INTERP_BILINEAR (0) nor UDB_INTERP_BICUBIC (1)", a->interpolation);
     return 1;
   }
   udb_geometry_t g;

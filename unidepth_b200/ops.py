@@ -341,7 +341,11 @@ def reflect_border_fill(buf):
     return buf
 
 
-def postprocess(radius, confidence, intr4, B, net_hw, padded_hw, pad_l, pad_t, out_hw, rays_in=None):
+def postprocess(radius, confidence, intr4, B, net_hw, padded_hw, pad_l, pad_t, out_hw, rays_in=None, mode="bilinear"):
+    """Output assembly (udb_postprocess): resize points = rays*radius, confidence and rays from the network to the padded
+    input size with F.interpolate(mode, align_corners=False) semantics, crop the paddings; mode "bilinear" or "bicubic"."""
+    if mode not in cabi.INTERP_MODES:
+        raise ValueError(f"postprocess: mode {mode!r} is not one of {sorted(cabi.INTERP_MODES)}")
     H, W = out_hw
     dev = radius.device
     outs = {
@@ -357,6 +361,8 @@ def postprocess(radius, confidence, intr4, B, net_hw, padded_hw, pad_l, pad_t, o
     p.padded_h, p.padded_w, p.pad_l, p.pad_t, p.H, p.W = padded_hw[0], padded_hw[1], pad_l, pad_t, H, W
     p.out_confidence, p.out_radius, p.out_depth = _ptr(outs["confidence"]), _ptr(outs["radius"]), _ptr(outs["depth"])
     p.out_points, p.out_rays = _ptr(outs["points"]), _ptr(outs["rays"])
-    cabi.check(_launch("postprocess_kernel", 0.0, lambda: cabi.lib().udb_postprocess(C.byref(p), _stream()),
+    p.mode = cabi.INTERP_MODES[mode]
+    kernel = "postprocess_bicubic_kernel" if mode == "bicubic" else "postprocess_kernel"
+    cabi.check(_launch(kernel, 0.0, lambda: cabi.lib().udb_postprocess(C.byref(p), _stream()),
                        _nb(radius, confidence, rays_in, *outs.values())), "udb_postprocess")
     return outs

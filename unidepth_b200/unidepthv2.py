@@ -496,6 +496,7 @@ class UniDepthV2(nn.Module, PyTorchModelHubMixin,
         a = cabi.InferArgs()
         a.rgb, a.rgb_is_u8, a.normalize = rgb.data_ptr(), int(rgb.dtype == torch.uint8), int(normalize)
         a.B, a.H, a.W, a.resolution_level = B, H, W, lvl
+        a.interpolation = cabi.INTERP_MODES[geom.get("interpolation", "bilinear")]
         a.camera_k = camera_k.data_ptr() if camera_k is not None else None
         a.camera_rays = rays_in.data_ptr() if rays_in is not None else None
         a.ray_scales = geom["scales"].data_ptr()
@@ -687,7 +688,7 @@ class UniDepthV2(nn.Module, PyTorchModelHubMixin,
         # a18: output assembly
         pl, pr_, pt, pb = geom["paddings"]
         out = ops.postprocess(radius, confidence, ray_intr, B, (nh, nw), geom["padded_hw"], pl, pt, geom["out_hw"],
-                              rays_in=rays_in)
+                              rays_in=rays_in, mode=geom.get("interpolation", "bilinear"))
         out["intrinsics"] = k_out
         out["depth_features"] = init_latents.view(B, gh, gw, hid).permute(0, 3, 1, 2)
         return out
@@ -745,8 +746,11 @@ class UniDepthV2(nn.Module, PyTorchModelHubMixin,
     @torch.no_grad()
     def infer(self, rgb: torch.Tensor, camera=None, normalize: bool = True):
         """Same contract as the reference `UniDepthV2.infer` (unidepthv2.py:239-339)."""
-        if self.interpolation_mode != "bilinear":
-            raise NotImplementedError("interpolation_mode other than 'bilinear' is not implemented")
+        mode = self.interpolation_mode
+        if mode not in cabi.INTERP_MODES:
+            raise NotImplementedError(
+                f"interpolation_mode {mode!r} is not supported: the reference resizes its outputs with "
+                f"F.interpolate(..., align_corners=False), which accepts only 'bilinear' and 'bicubic'")
         level = getattr(self, "resolution_level", None)
         if level is None:
             warnings.warn("!! self.resolution_level not set, using default bounds !!")
@@ -757,8 +761,8 @@ class UniDepthV2(nn.Module, PyTorchModelHubMixin,
         rgb = self._to_device_input(rgb)
         paddings, (ph, pw) = get_paddings((H, W), self.shape_constraints["ratio_bounds"])
         factor, (nh, nw) = get_resize_factor((ph, pw), bounds)
-        geom = dict(paddings=paddings, padded_hw=(ph, pw), factor=factor, net_hw=(nh, nw), out_hw=(H, W))
-        key = (level, tuple(self.shape_constraints["ratio_bounds"]), bounds)
+        geom = dict(paddings=paddings, padded_hw=(ph, pw), factor=factor, net_hw=(nh, nw), out_hw=(H, W), interpolation=mode)
+        key = (level, tuple(self.shape_constraints["ratio_bounds"]), bounds, mode)
         return self._run(rgb, geom, level, normalize, camera, key)
 
     NETWORK_ONLY = -2      # udb.h: UDB_LEVEL_NETWORK_ONLY
