@@ -281,6 +281,30 @@ int udb_camera_intrinsics(const float* x, int32_t B, int32_t net_h, int32_t net_
 int udb_camera_adjust_k(const float* K, int32_t B, float factor, int32_t pad_l, int32_t pad_t,
                         float* intr4, void* stream);
 
+/* GT-camera rays for infer(camera=<Camera object>) (unidepthv2.py:267-303,361-362; utils/camera.py): the unit rays
+ * [B, net_h*net_w, 3] f32 of each image's camera at the network-input pixel centres (u + 0.5, v + 0.5), i.e.
+ * BatchCamera.from_camera(cam).crop(-pads).resize(factor).get_rays((B, net_h, net_w)) in the layout rays_in takes.
+ * The camera is given in INPUT-image pixels, as the caller passes it to infer; the kernel applies the class's crop /
+ * resize rules (Spherical also updates its W, H and half-FOVs) and its unproject arithmetic:
+ *   UDB_CAM_PINHOLE     K (skew kept), inverted in the kernel; xyz / clip(z, 1e-4)
+ *   UDB_CAM_EUCM        closed form                            UDB_CAM_SPHERICAL   closed form (equirectangular)
+ *   UDB_CAM_OPENCV      16-parameter layout: undo tangential + thin prism (10 Newton steps), then radial k1..k3 (25)
+ *   UDB_CAM_FISHEYE624  16-parameter layout: same, radial k1..k6 on theta, r = tan(theta)
+ *   UDB_CAM_MEI         undo tangential (20 steps), radial k1, k2 (25), then the xi lift (xi == 1 handled)
+ * params: [B, UDB_CAM_STRIDE] f32, 16-byte aligned, one row per image:
+ *   [0..8]   Pinhole: K row-major;  other models: the class's params (fx fy cx cy ...), zero-padded to 16 ([0..15])
+ *   [16..18] use_radial, use_tangential, use_thin_prism (1 or 0) as the class decided them on its parameters (a part
+ *            whose coefficients sum to <= 1e-6 in absolute value is skipped); [19] unused
+ * Rays are normalised as get_rays does (norm clamped at 1e-4).  Checked before launch, udb_last_error() naming the
+ * argument: model known, B, net_h, net_w >= 1, params / rays non-null and aligned (16 / 4 bytes). */
+enum {
+  UDB_CAM_NONE = 0, UDB_CAM_PINHOLE = 1, UDB_CAM_EUCM = 2, UDB_CAM_SPHERICAL = 3, UDB_CAM_OPENCV = 4,
+  UDB_CAM_FISHEYE624 = 5, UDB_CAM_MEI = 6
+};
+#define UDB_CAM_STRIDE 20
+int udb_camera_rays(int32_t model, const float* params, int32_t B, int32_t net_h, int32_t net_w, int32_t pad_l,
+                    int32_t pad_r, int32_t pad_t, int32_t pad_b, float factor, float* rays, void* stream);
+
 typedef struct udb_ray_embed_t {
   const float* intr4;
   const float* rays_in;
@@ -558,7 +582,11 @@ typedef struct udb_infer_args_t {
   const float* camera_rays;   /* optional [B, net_h*net_w, 3] unit rays at network-input resolution produced by the
                                  caller's camera model (infer(camera=<Camera object>): camera.crop / resize /
                                  get_rays, unidepthv2.py:299-303,361-362; decoder.py:400); overrides camera_k */
-  const float* ray_scales;    /* optional [hidden/2] frequency table (positional_embedding.py:231-233);
+  int32_t camera_model;       /* UDB_CAM_* of camera_params; 0 (UDB_CAM_NONE) = no camera model.  With a model the engine
+                                 generates the rays itself (udb_camera_rays into its workspace) from the camera in
+                                 input-image pixels; setting it together with camera_k or camera_rays is an error */
+  const float* camera_params; /* [B, UDB_CAM_STRIDE] packed camera rows (see udb_camera_rays), with camera_model */
+  const float* ray_scales;   /* optional [hidden/2] frequency table (positional_embedding.py:231-233);
                                  NULL = the engine's own table */
   void* workspace;
   size_t workspace_bytes;

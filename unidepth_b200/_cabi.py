@@ -14,6 +14,8 @@ ACT_NONE, ACT_GELU, ACT_LEAKY = 0, 1, 2
 STORE_ROWS, STORE_CONVT, STORE_CONVTILE, STORE_HEAD = 0, 1, 2, 3
 INTERP_BILINEAR, INTERP_BICUBIC = 0, 1
 INTERP_MODES = {"bilinear": INTERP_BILINEAR, "bicubic": INTERP_BICUBIC}
+CAM_NONE, CAM_PINHOLE, CAM_EUCM, CAM_SPHERICAL, CAM_OPENCV, CAM_FISHEYE624, CAM_MEI = range(7)
+CAM_STRIDE = 20      # floats per packed camera row (udb.h UDB_CAM_STRIDE)
 
 vp, i32, i64, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_float
 
@@ -122,7 +124,8 @@ class V1Geometry(C.Structure):
 class InferArgs(C.Structure):
     _fields_ = [
         ("rgb", vp), ("rgb_is_u8", i32), ("normalize", i32), ("B", i32), ("H", i32), ("W", i32),
-        ("resolution_level", i32), ("interpolation", i32), ("camera_k", vp), ("camera_rays", vp), ("ray_scales", vp), ("workspace", vp),
+        ("resolution_level", i32), ("interpolation", i32), ("camera_k", vp), ("camera_rays", vp),
+        ("camera_model", i32), ("camera_params", vp), ("ray_scales", vp), ("workspace", vp),
         ("workspace_bytes", C.c_size_t),
         ("confidence", vp), ("intrinsics", vp), ("radius", vp), ("depth", vp), ("points", vp), ("rays", vp),
         ("depth_features", vp),
@@ -205,6 +208,7 @@ EXPORTS = {
     "udb_reflect_border_fill_nhwc_f16": (i32, [vp, i32, i32, i32, i32, vp]),
     "udb_postprocess": (i32, [C.POINTER(Postprocess), vp]),
     "udb_camera_adjust_k": (i32, [vp, i32, f32, i32, i32, vp, vp]),
+    "udb_camera_rays": (i32, [i32, vp, i32, i32, i32, i32, i32, i32, i32, f32, vp, vp]),
     "udb_create": (i32, [C.POINTER(Config), C.POINTER(vp)]),
     "udb_destroy": (None, [vp]),
     "udb_set_weight": (i32, [vp, C.c_char_p, vp, C.POINTER(i64), i32, i32]),

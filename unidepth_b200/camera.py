@@ -14,9 +14,12 @@ that the README's second usage (`model.infer(rgb, Pinhole(K=K))`, README.md:140-
     MEI               :977-1142      MEI            fx fy cx cy k1 k2 p1 p2 xi
     BatchCamera       :1145-1308     BatchCamera    a batch of the above, params padded to 16
 
-This is plumbing for the optional GT-camera branch, not the hot path: the rays a camera object produces enter the
-CUDA path as a [B, H*W, 3] tensor (`unidepthv2.py::_camera_rays`); every op below is a small torch op on the
-device the parameters live on.  The closed-form models (Pinhole, EUCM, Spherical, every `project`) are pinned to
+The GT-camera branch of `infer` does not run the torch code below: `pack_camera` turns an object of these classes
+(or a BatchCamera of one of them) into a model id and rows of parameters, and the `udb_camera_rays` kernel evaluates
+the same crop / resize / unproject / get_rays arithmetic on the GPU.  Any other object (the reference's own classes,
+duck-typed cameras, mixed-model batches, the 15-parameter layout, non-fp32 parameters) still goes through its own
+methods on the host (`unidepthv2.py::_camera_rays`); every op below is a small torch op on the device the parameters
+live on.  The closed-form models (Pinhole, EUCM, Spherical, every `project`) are pinned to
 the reference's outputs (tests/golden/cameras.npz, made by oracle/make_golden_cameras.py).  The three models whose
 `unproject` has no closed form (OPENCV, Fisheye624, MEI) invert the SAME forward distortion, but with one shared
 damped-Newton solver run to convergence instead of the reference's per-class trust-region loops, which stop at a
@@ -33,7 +36,7 @@ import torch
 import torch.nn.functional as F
 
 __all__ = ["Camera", "Pinhole", "EUCM", "Spherical", "OPENCV", "Fisheye624", "MEI", "BatchCamera", "pixel_grid",
-           "invert_pinhole"]
+           "invert_pinhole", "pack_camera"]
 
 _PAD = 16          # parameter vector length inside a BatchCamera (camera.py:156-167)
 
@@ -658,3 +661,54 @@ class BatchCamera(Camera):
     @property
     def max_fov(self):
         return [cam.max_fov for cam in self.cameras]
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# Packing for the GPU ray generator (udb_camera_rays, include/udb.h)
+_CAM_STRIDE = 20                          # udb.h UDB_CAM_STRIDE: 16 parameters + use_radial, use_tangential, use_thin_prism, 0
+_MODEL_IDS = {"Pinhole": 1, "EUCM": 2, "Spherical": 3, "OPENCV": 4, "Fisheye624": 5, "MEI": 6}   # UDB_CAM_*
+_MIN_PARAMS = {"EUCM": 6, "Spherical": 8, "OPENCV": 16, "Fisheye624": 16, "MEI": 9}
+
+
+def _pack_one(cam) -> Optional[Tuple[int, torch.Tensor]]:
+    name = type(cam).__name__
+    if name not in _MODEL_IDS or type(cam) is not globals()[name]:      # exact classes only: a subclass may differ
+        return None
+    if name == "Pinhole":
+        K = cam.K
+        if not isinstance(K, torch.Tensor) or K.dtype != torch.float32 or K.shape[-2:] != (3, 3):
+            return None
+        vals = K.reshape(-1, 9)
+        flags = (0.0, 0.0, 0.0)
+    else:
+        p = cam.params
+        if p.dtype != torch.float32 or p.ndim != 2:
+            return None
+        n = p.shape[1]
+        if n < _MIN_PARAMS[name] or (name in ("OPENCV", "Fisheye624") and n != 16) or n > 16:
+            return None                       # the 15-parameter single-focal layout stays on the host
+        vals = p
+        flags = (float(getattr(cam, "use_radial", False)), float(getattr(cam, "use_tangential", False)),
+                 float(getattr(cam, "use_thin_prism", False)))
+    rows = vals.new_zeros(vals.shape[0], _CAM_STRIDE)
+    rows[:, :vals.shape[1]] = vals
+    rows[:, 16:19] = torch.tensor(flags, dtype=torch.float32)
+    return _MODEL_IDS[name], rows
+
+
+def pack_camera(camera) -> Optional[Tuple[int, torch.Tensor]]:
+    """(UDB_CAM_* model id, [rows, 20] float32 params in input-image pixels) for a Pinhole / EUCM / Spherical /
+    16-parameter OPENCV or Fisheye624 / MEI object, or a BatchCamera whose members are all one such model (one row per
+    member row); None for anything else, which keeps the host path.  The rows carry the object's own use_radial /
+    use_tangential / use_thin_prism decisions.  The caller's object is not modified."""
+    members = camera.cameras if type(camera) is BatchCamera else [camera]
+    model, rows = None, []
+    for cam in members:
+        packed = _pack_one(cam)
+        if packed is None or (model is not None and packed[0] != model):
+            return None
+        model = packed[0]
+        rows.append(packed[1])
+    if model is None:
+        return None
+    return model, torch.cat([r.to(rows[0].device) for r in rows])

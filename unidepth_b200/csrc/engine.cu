@@ -184,8 +184,16 @@ static int run(udb_engine* e, const udb_infer_args_t& a, const udb_geometry_t& g
 
   stage.next("udb:ray_embedding+prompt_blocks");
   // ---- a11/a12: rays (predicted K, or the caller's pinhole K) -> Fourier embedding on the patch grid
+  //      or the caller's camera model, whose rays udb_camera_rays writes into the workspace once per call
   const float* ray_intr = intr4;
-  if (a.camera_k && !a.camera_rays) {
+  const float* rays_in = a.camera_rays;
+  if (a.camera_model != UDB_CAM_NONE) {
+    float* gen = ar.f(static_cast<size_t>(B) * nh * nw * 3);
+    if (!c.dry && !c.rc)
+      c.done(udb_camera_rays(a.camera_model, a.camera_params, B, nh, nw, g.pad_l, g.pad_r, g.pad_t, g.pad_b,
+                             static_cast<float>(g.factor), gen, st));
+    rays_in = gen;
+  } else if (a.camera_k && !a.camera_rays) {
     float* gt4 = ar.f(static_cast<size_t>(B) * 4);
     if (!c.dry && !c.rc) c.done(udb_camera_adjust_k(a.camera_k, B, static_cast<float>(g.factor), g.pad_l, g.pad_t, gt4, st));
     ray_intr = gt4;
@@ -194,7 +202,7 @@ static int run(udb_engine* e, const udb_infer_args_t& a, const udb_geometry_t& g
   if (!c.dry && !c.rc) {
     udb_ray_embed_t p;
     memset(&p, 0, sizeof(p));
-    p.intr4 = ray_intr; p.rays_in = a.camera_rays; p.scales = a.ray_scales ? a.ray_scales : tb.scales;
+    p.intr4 = ray_intr; p.rays_in = rays_in; p.scales = a.ray_scales ? a.ray_scales : tb.scales;
     p.B = B; p.net_h = nh; p.net_w = nw; p.gh = gh; p.gw = gw; p.bands = hid / 2; p.out = remb; p.out_f32 = 1;
     c.done(udb_ray_embed(&p, st));
   }
@@ -312,7 +320,7 @@ static int run(udb_engine* e, const udb_infer_args_t& a, const udb_geometry_t& g
   if (!c.dry && !c.rc) {
     udb_postprocess_t p;
     memset(&p, 0, sizeof(p));
-    p.radius = planes[0]; p.confidence = planes[1]; p.intr4 = ray_intr; p.rays_in = a.camera_rays;
+    p.radius = planes[0]; p.confidence = planes[1]; p.intr4 = ray_intr; p.rays_in = rays_in;
     p.B = B; p.net_h = nh; p.net_w = nw; p.padded_h = g.padded_h; p.padded_w = g.padded_w; p.pad_l = g.pad_l; p.pad_t = g.pad_t;
     p.H = a.H; p.W = a.W;
     p.out_confidence = a.confidence; p.out_radius = a.radius; p.out_depth = a.depth; p.out_points = a.points; p.out_rays = a.rays;
@@ -440,7 +448,8 @@ size_t udb_schedule_bytes(udb_engine* e, int32_t B, int32_t H, int32_t W, int32_
   udb_infer_args_t a;
   memset(&a, 0, sizeof(a));
   a.B = B; a.H = H; a.W = W; a.resolution_level = level;
-  a.camera_k = reinterpret_cast<const float*>(16);   // the larger (GT-camera) variant, as udb_workspace_bytes sizes it
+  a.camera_model = UDB_CAM_PINHOLE;                  // the largest (camera-model) variant, as udb_workspace_bytes sizes it:
+  a.camera_params = reinterpret_cast<const float*>(16);   // its ray buffer sits where camera_k's (smaller) table would
   const ShapeTables none;                            // a dry run only hands the table pointers on
   Arena ar(nullptr, 0);
   if (run(e, a, g, none, ar, nullptr)) return 0;
@@ -455,7 +464,8 @@ size_t udb_workspace_bytes(udb_engine* e, int32_t B, int32_t H, int32_t W, int32
   udb_infer_args_t a;
   memset(&a, 0, sizeof(a));
   a.B = B; a.H = H; a.W = W; a.resolution_level = level;
-  a.camera_k = reinterpret_cast<const float*>(16);   // sized for the larger (GT-camera) variant
+  a.camera_model = UDB_CAM_PINHOLE;                  // sized for the largest (camera-model) variant, which also covers
+  a.camera_params = reinterpret_cast<const float*>(16);   // the camera_k and camera_rays ones
   Arena ar(nullptr, 0);
   if (run(e, a, g, *tb, ar, nullptr)) return 0;
   char key[96];
@@ -473,6 +483,22 @@ int udb_infer_v2(udb_engine* e, const udb_infer_args_t* a, void* stream) {
   if (a->interpolation != UDB_INTERP_BILINEAR && a->interpolation != UDB_INTERP_BICUBIC) {
     set_error("udb_infer_v2: `interpolation` %d is neither UDB_INTERP_BILINEAR (0) nor UDB_INTERP_BICUBIC (1)", a->interpolation);
     return 1;
+  }
+  if (a->camera_model < UDB_CAM_NONE || a->camera_model > UDB_CAM_MEI) {
+    set_error("udb_infer_v2: `camera_model` %d is not a UDB_CAM_* camera model (0..6)", a->camera_model);
+    return 1;
+  }
+  if (a->camera_model != UDB_CAM_NONE) {
+    if (a->camera_k || a->camera_rays) {
+      set_error("udb_infer_v2: `camera_model` cannot be combined with `%s`: give one camera source",
+                a->camera_k ? "camera_k" : "camera_rays");
+      return 1;
+    }
+    if (!a->camera_params) { set_error("udb_infer_v2: `camera_model` %d needs `camera_params` (null)", a->camera_model); return 1; }
+    if (reinterpret_cast<uintptr_t>(a->camera_params) & 15) {
+      set_error("udb_infer_v2: `camera_params` must be 16-byte aligned");
+      return 1;
+    }
   }
   udb_geometry_t g;
   if (udb_geometry(e, a->H, a->W, a->resolution_level, &g)) return 1;

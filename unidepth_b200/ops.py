@@ -296,6 +296,19 @@ def camera_intrinsics(x, B, net_hw, factor, pad_l, pad_t):
     return intr4, k_net, k_out
 
 
+def camera_rays(model, params, B, net_hw, paddings, factor):
+    """GT-camera rays [B, net_h*net_w, 3] of a packed camera (udb_camera_rays; camera.pack_camera): params [B, CAM_STRIDE]
+    f32 in input-image pixels, cropped by the paddings (l, r, t, b) and resized by `factor` in the kernel."""
+    assert params.dtype == f32 and params.is_contiguous() and tuple(params.shape) == (B, cabi.CAM_STRIDE), params.shape
+    nh, nw = net_hw
+    out = torch.empty((B, nh * nw, 3), device=params.device, dtype=f32)
+    pl, pr, pt, pb = paddings
+    cabi.check(_launch("camera_rays_kernel", 0.0,
+                       lambda: cabi.lib().udb_camera_rays(int(model), _ptr(params), B, nh, nw, pl, pr, pt, pb, float(factor),
+                                                          _ptr(out), _stream()), _nb(out)), "udb_camera_rays")
+    return out
+
+
 def ray_embed(intr4, scales, B, net_hw, grid_hw, out_dtype=f32, rays_in=None):
     bands = scales.numel()
     out = torch.empty((B * grid_hw[0] * grid_hw[1], 2 * bands), device=scales.device, dtype=out_dtype)

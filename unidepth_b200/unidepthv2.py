@@ -30,6 +30,7 @@ import torch.nn as nn
 
 from . import _cabi as cabi
 from . import ops
+from .camera import pack_camera
 from .spec import ModelSpec, PATCH, get_paddings, get_resize_factor, param_shapes, pixel_bounds
 
 try:  # same mixin as the reference (unidepthv2.py:111-117)
@@ -464,7 +465,8 @@ class UniDepthV2(nn.Module, PyTorchModelHubMixin,
         self._engine_tensors = tensors          # the engine borrows these pointers
         return handle
 
-    def _forward_engine(self, rgb: torch.Tensor, geom: dict, normalize: bool, level, camera_k=None, rays_in=None):
+    def _forward_engine(self, rgb: torch.Tensor, geom: dict, normalize: bool, level, camera_k=None, rays_in=None,
+                        camera_model=0, camera_params=None):
         """The whole path as ONE C call (udb_infer_v2): torch only allocates outputs / workspace."""
         eng = self._get_engine()
         lib = cabi.lib()
@@ -499,6 +501,8 @@ class UniDepthV2(nn.Module, PyTorchModelHubMixin,
         a.interpolation = cabi.INTERP_MODES[geom.get("interpolation", "bilinear")]
         a.camera_k = camera_k.data_ptr() if camera_k is not None else None
         a.camera_rays = rays_in.data_ptr() if rays_in is not None else None
+        a.camera_model = int(camera_model)
+        a.camera_params = camera_params.data_ptr() if camera_params is not None else None
         a.ray_scales = geom["scales"].data_ptr()
         a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
         for k, v in out.items():
@@ -709,15 +713,42 @@ class UniDepthV2(nn.Module, PyTorchModelHubMixin,
             K = K.expand(B, 3, 3)
         if float(K[:, 0, 1].abs().max()) != 0.0:
             raise NotImplementedError("pinhole K with skew is not supported")
+        return UniDepthV2._adjust_k(K, paddings, factor)
+
+    @staticmethod
+    def _adjust_k(K, paddings, factor):
+        """[B,3,3] K in input-image pixels -> [B,4] (fx, fy, cx, cy) in network-input pixels: the arithmetic of
+        udb_camera_adjust_k, as torch ops that a CUDA graph can capture (no host synchronisation)."""
         pl, _, pt, _ = paddings
         return torch.stack([K[:, 0, 0] * factor, K[:, 1, 1] * factor, (K[:, 0, 2] + pl) * factor,
                             (K[:, 1, 2] + pt) * factor], dim=1).contiguous()
 
+    @staticmethod
+    def _camera_source(camera, rays_in, B, geom, dev):
+        """The call's camera as (source, device tensors): source None (predicted rays), "K" ({"K": [B,3,3]}),
+        ("model", UDB_CAM_*) ({"params": [B, CAM_STRIDE]}: a camera object whose rays the udb_camera_rays kernel
+        generates) or "rays" ({"rays": [B, net_h*net_w, 3]}: network_forward's rays, or the host path of any other
+        camera object).  Everything is validated here, before a graph is captured or replayed."""
+        if camera is None:
+            return (None, {}) if rays_in is None else ("rays", {"rays": rays_in})
+        if isinstance(camera, torch.Tensor):
+            UniDepthV2._gt_intrinsics(camera, B, geom["paddings"], geom["factor"], dev)     # validates the argument
+            K = camera.to(dev, f32).reshape(-1, 3, 3)
+            return "K", {"K": K.expand(B, 3, 3).contiguous()}
+        packed = pack_camera(camera)
+        if packed is None:
+            nh, nw = geom["net_hw"]
+            return "rays", {"rays": UniDepthV2._camera_rays(camera, B, geom["paddings"], geom["factor"], (nh, nw), dev)}
+        model, rows = packed
+        if rows.shape[0] not in (1, B):
+            raise ValueError(f"camera holds {rows.shape[0]} cameras for a batch of {B} images (need 1 or {B})")
+        return ("model", model), {"params": rows.to(dev).expand(B, cabi.CAM_STRIDE).contiguous()}
+
     # ------------------------------------------------------------------ infer
     @staticmethod
     def _camera_rays(camera, B, paddings, factor, net_hw, dev):
-        """`camera=` given as a camera OBJECT (the reference's `Camera` / `BatchCamera` family,
-        utils/camera.py, or anything with the same three methods): the reference crops it by the
+        """`camera=` given as a camera OBJECT that `pack_camera` does not cover (the reference's `Camera` / `BatchCamera`
+        family, utils/camera.py, or anything with the same three methods): the reference crops it by the
         paddings, resizes it by the factor and asks it for unit rays at network-input resolution
         (unidepthv2.py:299-303, :361-362); those rays replace the predicted ones (decoder.py:400).
         The object's own host/torch code generates the rays; they enter the kernels as a
@@ -850,46 +881,48 @@ class UniDepthV2(nn.Module, PyTorchModelHubMixin,
             self._scales_cache[skey] = (2.0 ** torch.linspace(0.0, math.log2(max(gh, gw) // 2), steps=bands)).to(dev)
         geom["scales"] = self._scales_cache[skey]
 
-        gt_intr4, camera_k = None, None
-        if camera is not None and not isinstance(camera, torch.Tensor):
-            rays_in = self._camera_rays(camera, B, geom["paddings"], geom["factor"], (nh, nw), dev)
-        elif camera is not None:
-            gt_intr4 = self._gt_intrinsics(camera, B, geom["paddings"], geom["factor"], dev)     # validates the argument
-            camera_k = camera.to(dev, f32).reshape(-1, 3, 3)
-            if camera_k.shape[0] == 1 and B > 1:
-                camera_k = camera_k.expand(B, 3, 3)
-            camera_k = camera_k.contiguous()
+        source, cam = self._camera_source(camera, rays_in, B, geom, dev)
+        model = source[1] if isinstance(source, tuple) else 0
 
         self._weights()
         if len(self._engine_shapes) > self.max_engine_shapes:
             self._drop_engine()       # too many distinct grids seen: rebuild (frees the engine's per-shape tables)
 
-        def run(inp):
+        def run(inp, cam):
             if not self.use_engine and self.precision != "f16":
                 raise NotImplementedError("precision='split' runs through the C engine only (use_engine=True)")
             if self.use_engine:
-                return self._forward_engine(inp, geom, normalize, level, camera_k=camera_k, rays_in=rays_in)
+                return self._forward_engine(inp, geom, normalize, level, camera_k=cam.get("K"), rays_in=cam.get("rays"),
+                                            camera_model=model, camera_params=cam.get("params"))
             self._pos_embed(gh, gw)
-            return self._forward(inp, geom, normalize, gt_intr4=gt_intr4, rays_in=rays_in)
+            gt_intr4 = self._adjust_k(cam["K"], geom["paddings"], geom["factor"]) if "K" in cam else None
+            rays = cam.get("rays")
+            if "params" in cam:
+                rays = ops.camera_rays(model, cam["params"], B, (nh, nw), geom["paddings"], geom["factor"])
+            return self._forward(inp, geom, normalize, gt_intr4=gt_intr4, rays_in=rays)
 
-        if not self.use_cuda_graph or camera is not None or rays_in is not None:
-            return run(rgb)
+        if not self.use_cuda_graph:
+            return run(rgb, cam)
 
-        key = (B, H, W, rgb.dtype, bool(normalize), bool(self.use_engine)) + tuple(key_extra)
+        # The camera source is part of the key (a graph captured for one source reads other buffers); its values are not:
+        # the entry owns static copies of the camera tensors, refreshed before every replay like the image.
+        key = (B, H, W, rgb.dtype, bool(normalize), bool(self.use_engine)) + tuple(key_extra) + (source,)
         entry = self._graphs.get(key)
         if entry is None:
             static_in = rgb.clone()
+            static_cam = {k: v.clone() for k, v in cam.items()}
             # warm-up on a side stream (allocator, per-shape tables, workspace), then capture
             side = torch.cuda.Stream()
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
-                run(static_in)
+                run(static_in, static_cam)
             torch.cuda.current_stream().wait_stream(side)
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
-                static_out = run(static_in)
+                static_out = run(static_in, static_cam)
             # the entry owns everything whose address the captured kernels read
-            entry = dict(graph=graph, inp=static_in, out=static_out, ws=getattr(self, "_last_ws", None), scales=geom["scales"])
+            entry = dict(graph=graph, inp=static_in, cam=static_cam, out=static_out, ws=getattr(self, "_last_ws", None),
+                         scales=geom["scales"])
             self._graphs[key] = entry
             while len(self._graphs) > self.max_cached_graphs:
                 self._graphs.popitem(last=False)
@@ -897,6 +930,8 @@ class UniDepthV2(nn.Module, PyTorchModelHubMixin,
             self._graphs.move_to_end(key)
         if os.environ.get("UDB_SKIP_INPUT_COPY") != "1":      # (experiment switch: isolates copy-engine contention)
             entry["inp"].copy_(rgb, non_blocking=True)
+        for k, v in cam.items():
+            entry["cam"][k].copy_(v, non_blocking=True)
         entry["graph"].replay()
         bufs = self.output_buffers
         if bufs is not None:       # caller-provided destinations (e.g. the send slot of parallel.PeerGather): one copy, no clone
