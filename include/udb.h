@@ -674,6 +674,87 @@ int udb_p2p_barrier(void* const* peer_flags_dev, void* my_flags, int32_t rank, i
                     int32_t* timeout_flag_dev, void* stream);
 int udb_p2p_copy(void* dst, const void* src, size_t bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Evaluation metrics (reference unidepth/utils/evaluation_depth.py, chamfer_distance.py:59-158, ops/knn with K = 1,
+ * norm = 2).  Distances, ratios and rescaled values use the reference's fp32 op order with no FMA contraction; counts
+ * are integers and every floating-point sum is an f64 per-CTA partial reduced in a fixed order, so results are
+ * deterministic.  Inputs must be finite.  Checked before launch, udb_last_error() naming the argument.  No host sync.
+ * ------------------------------------------------------------------------------------------- */
+
+/* Nearest neighbour: for every valid point of x, the squared L2 distance ((dx*dx) + dy*dy) + dz*dz (dx = x - y, each op
+ * rounded, as knn_cpu.cpp forms it) to its nearest valid y point and that point's index, ties to the lowest index.
+ * x [N, P1, 3], y [N, P2, 3] f32 contiguous; lengths1 / lengths2: [N] int64 on the device or NULL (= P1 / P2), clamped
+ * to [0, P] in the kernel.  Rows past lengths1, or of a cloud with lengths2 == 0, get dist = 0 and idx = 0.  With
+ * dist_y / idx_y set, the y -> x direction comes from the same pass (both or neither).  idx_x / idx_y double as the
+ * packed (dist, idx) accumulators while the kernel runs. */
+typedef struct udb_nn_t {
+  const float* x;
+  const float* y;
+  const int64_t* lengths1;
+  const int64_t* lengths2;
+  int32_t N, P1, P2, pad0;
+  float* dist_x;   /* [N, P1] */
+  int64_t* idx_x;  /* [N, P1] */
+  float* dist_y;   /* [N, P2] or NULL */
+  int64_t* idx_y;  /* [N, P2] or NULL */
+} udb_nn_t;
+int udb_nearest_neighbor(const udb_nn_t* p, void* stream);
+
+/* Most CTAs per image (per cloud) of the metric reductions; partials hold [B, UDB_METRIC_MAX_BLOCKS, nacc] doubles. */
+#define UDB_METRIC_MAX_BLOCKS 64
+
+/* Depth metrics of eval_depth over the pixels with mask != 0 and (use_max_depth ? gt <= max_depth : true).
+ * gt, pred [B, HW] f32 (pred already resized to gt), mask [B, HW] uint8.  thr_*: the fp32 delta / tau thresholds;
+ * auc_thresholds: the UDB_DM_AUC_BINS d_auc thresholds, ascending; medians [B, 2]: median(gt), median(pred) of the
+ * valid pixels (si).  out [B, UDB_DM_NACC] f64 (layout below; counts are exact integers), ssi [B, 2] f32: the ssi
+ * (scale, shift) solved in f64 from the normal-equation sums with the reference's 1e-9 I stabiliser.  Two passes. */
+#define UDB_DM_AUC_BINS 100
+enum {
+  UDB_DM_N = 0, UDB_DM_D1, UDB_DM_D2, UDB_DM_D3, UDB_DM_TAU,                /* counts of ratio < threshold */
+  UDB_DM_SQ, UDB_DM_SQLOG, UDB_DM_AREL, UDB_DM_SQREL, UDB_DM_LOG10,          /* sums of the per-pixel terms */
+  UDB_DM_LG, UDB_DM_LG2,                                                     /* sum of log p - log g and of its square */
+  UDB_DM_D1_SI, UDB_DM_TAU_SI, UDB_DM_AREL_SI,                               /* si-rescaled counts / sum */
+  UDB_DM_PP, UDB_DM_P, UDB_DM_PG, UDB_DM_G,                                  /* ssi normal equations */
+  UDB_DM_AUC,                                        /* UDB_DM_AUC_BINS bins: pixels whose first threshold > ratio is k */
+  UDB_DM_AREL_SSI = UDB_DM_AUC + UDB_DM_AUC_BINS, UDB_DM_D1_SSI, UDB_DM_TAU_SSI,   /* ssi-rescaled sum / counts */
+  UDB_DM_NACC
+};
+typedef struct udb_depth_metrics_t {
+  const float* gt;
+  const float* pred;
+  const uint8_t* mask;
+  int32_t B, pad0;
+  int64_t HW;
+  float max_depth;
+  int32_t use_max_depth;
+  float thr_d1, thr_d2, thr_d3, thr_tau;
+  const float* auc_thresholds;
+  const float* medians;
+  double* partials;  /* workspace: [B, UDB_METRIC_MAX_BLOCKS, UDB_DM_NACC] */
+  double* out;
+  float* ssi;
+} udb_depth_metrics_t;
+int udb_depth_metrics(const udb_depth_metrics_t* p, void* stream);
+
+/* Point metrics of eval_3d on compacted clouds gt, pred [N, P, 3] f32 with lengths [N] int64 (device, or NULL = P)
+ * and the NN distances dist_x (gt -> pred), dist_y (pred -> gt) [N, P].  thresholds: n_thresholds f32, ascending.
+ * out [N, 2 + 2 * n_thresholds] f64: [0] sum of |gt - pred|_2, [1] sum of (sqrt(dist_x) + sqrt(dist_y)) / 2, then the
+ * histograms of dist_x and of dist_y, bin k counting the points whose first threshold above the distance is k (the
+ * count below threshold i is the sum of bins 0..i). */
+#define UDB_PM_MAX_THRESHOLDS 1024
+typedef struct udb_point_metrics_t {
+  const float* gt;
+  const float* pred;
+  const int64_t* lengths;
+  const float* dist_x;
+  const float* dist_y;
+  const float* thresholds;
+  int32_t N, P, n_thresholds, pad0;
+  double* partials;  /* workspace: [N, UDB_METRIC_MAX_BLOCKS, 2 + 2 * n_thresholds] */
+  double* out;
+} udb_point_metrics_t;
+int udb_point_metrics(const udb_point_metrics_t* p, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -177,6 +177,38 @@ class InferV1Args(C.Structure):
     ]
 
 
+class NearestNeighbor(C.Structure):
+    _fields_ = [
+        ("x", vp), ("y", vp), ("lengths1", vp), ("lengths2", vp), ("N", i32), ("P1", i32), ("P2", i32), ("pad0", i32),
+        ("dist_x", vp), ("idx_x", vp), ("dist_y", vp), ("idx_y", vp),
+    ]
+
+
+class DepthMetrics(C.Structure):
+    _fields_ = [
+        ("gt", vp), ("pred", vp), ("mask", vp), ("B", i32), ("pad0", i32), ("HW", i64),
+        ("max_depth", f32), ("use_max_depth", i32), ("thr_d1", f32), ("thr_d2", f32), ("thr_d3", f32), ("thr_tau", f32),
+        ("auc_thresholds", vp), ("medians", vp), ("partials", vp), ("out", vp), ("ssi", vp),
+    ]
+
+
+class PointMetrics(C.Structure):
+    _fields_ = [
+        ("gt", vp), ("pred", vp), ("lengths", vp), ("dist_x", vp), ("dist_y", vp), ("thresholds", vp),
+        ("N", i32), ("P", i32), ("n_thresholds", i32), ("pad0", i32), ("partials", vp), ("out", vp),
+    ]
+
+
+# udb.h evaluation-metric layouts
+METRIC_MAX_BLOCKS = 64
+DM_AUC_BINS = 100
+(DM_N, DM_D1, DM_D2, DM_D3, DM_TAU, DM_SQ, DM_SQLOG, DM_AREL, DM_SQREL, DM_LOG10, DM_LG, DM_LG2, DM_D1_SI, DM_TAU_SI,
+ DM_AREL_SI, DM_PP, DM_P, DM_PG, DM_G, DM_AUC) = range(20)
+DM_AREL_SSI, DM_D1_SSI, DM_TAU_SSI = DM_AUC + DM_AUC_BINS, DM_AUC + DM_AUC_BINS + 1, DM_AUC + DM_AUC_BINS + 2
+DM_NACC = DM_TAU_SSI + 1
+PM_MAX_THRESHOLDS = 1024
+
+
 class ProfileEntry(C.Structure):
     _fields_ = [("name", C.c_char * 48), ("ms", f32), ("flops", C.c_double), ("bytes", C.c_double)]
 
@@ -244,6 +276,10 @@ EXPORTS = {
     "udb_v1_geometry": (i32, [i32, i32, i32, i32, C.POINTER(V1Geometry)]),
     "udb_v1_workspace_bytes": (C.c_size_t, [vp, i32, i32, i32]),
     "udb_infer_v1": (i32, [vp, C.POINTER(InferV1Args), vp]),
+    # evaluation metrics
+    "udb_nearest_neighbor": (i32, [C.POINTER(NearestNeighbor), vp]),
+    "udb_depth_metrics": (i32, [C.POINTER(DepthMetrics), vp]),
+    "udb_point_metrics": (i32, [C.POINTER(PointMetrics), vp]),
     # peer-memory plumbing (multi-GPU gather)
     "udb_p2p_alloc": (i32, [C.c_size_t, C.POINTER(vp), vp]),
     "udb_p2p_open": (i32, [vp, C.POINTER(vp)]),

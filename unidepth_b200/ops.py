@@ -379,3 +379,83 @@ def postprocess(radius, confidence, intr4, B, net_hw, padded_hw, pad_l, pad_t, o
     cabi.check(_launch(kernel, 0.0, lambda: cabi.lib().udb_postprocess(C.byref(p), _stream()),
                        _nb(radius, confidence, rays_in, *outs.values())), "udb_postprocess")
     return outs
+
+
+def _metric_operand(name, t, dtype):
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != dtype or not t.is_contiguous():
+        raise ValueError(f"{name} must be a contiguous {dtype} CUDA tensor, got "
+                         f"{t.dtype if isinstance(t, torch.Tensor) else type(t).__name__}"
+                         f"{'' if not isinstance(t, torch.Tensor) else (' on ' + str(t.device))}")
+
+
+def nearest_neighbor(x, y, lengths1=None, lengths2=None, both=True):
+    """K = 1 squared-L2 nearest neighbours (udb_nearest_neighbor): x [N, P1, 3], y [N, P2, 3] f32 contiguous CUDA,
+    lengths int64 [N] on the same device or None.  Returns (dist_x, idx_x, dist_y, idx_y); the y -> x pair is None
+    unless `both`.  Lengths are assumed in [0, P] (the callers in validation.py check them)."""
+    _metric_operand("x", x, f32)
+    _metric_operand("y", y, f32)
+    N, P1, _ = x.shape
+    P2 = y.shape[1]
+    for n, l in (("lengths1", lengths1), ("lengths2", lengths2)):
+        if l is not None:
+            _metric_operand(n, l, torch.int64)
+    dev = x.device
+    dist_x, idx_x = torch.empty((N, P1), device=dev, dtype=f32), torch.empty((N, P1), device=dev, dtype=torch.int64)
+    dist_y = torch.empty((N, P2), device=dev, dtype=f32) if both else None
+    idx_y = torch.empty((N, P2), device=dev, dtype=torch.int64) if both else None
+    p = cabi.NearestNeighbor()
+    p.x, p.y, p.lengths1, p.lengths2 = _ptr(x), _ptr(y), _ptr(lengths1), _ptr(lengths2)
+    p.N, p.P1, p.P2 = N, P1, P2
+    p.dist_x, p.idx_x, p.dist_y, p.idx_y = _ptr(dist_x), _ptr(idx_x), _ptr(dist_y), _ptr(idx_y)
+    cabi.check(_launch("nn_kernel", 8.0 * N * P1 * P2, lambda: cabi.lib().udb_nearest_neighbor(C.byref(p), _stream())),
+               "udb_nearest_neighbor")
+    return dist_x, idx_x, dist_y, idx_y
+
+
+def depth_metrics(gt, pred, mask, max_depth, thresholds, auc_thresholds, medians):
+    """Per-image sums and counts of eval_depth (udb_depth_metrics): gt, pred [B, H, W] f32, mask [B, H, W] uint8,
+    thresholds = (d1, d2, d3, tau) fp32 values, auc_thresholds [100] f32 ascending, medians [B, 2] f32 (median gt,
+    median pred of the valid pixels).  Returns (out [B, DM_NACC] f64, ssi [B, 2] f32)."""
+    _metric_operand("gt", gt, f32)
+    _metric_operand("pred", pred, f32)
+    _metric_operand("mask", mask, torch.uint8)
+    _metric_operand("auc_thresholds", auc_thresholds, f32)
+    _metric_operand("medians", medians, f32)
+    B = gt.shape[0]
+    HW = gt[0].numel()
+    dev = gt.device
+    partials = torch.empty((B, cabi.METRIC_MAX_BLOCKS, cabi.DM_NACC), device=dev, dtype=torch.float64)
+    out = torch.empty((B, cabi.DM_NACC), device=dev, dtype=torch.float64)
+    ssi = torch.empty((B, 2), device=dev, dtype=f32)
+    p = cabi.DepthMetrics()
+    p.gt, p.pred, p.mask, p.B, p.HW = _ptr(gt), _ptr(pred), _ptr(mask), B, HW
+    p.use_max_depth = int(max_depth is not None)
+    p.max_depth = float(max_depth) if max_depth is not None else 0.0
+    p.thr_d1, p.thr_d2, p.thr_d3, p.thr_tau = thresholds
+    p.auc_thresholds, p.medians = _ptr(auc_thresholds), _ptr(medians)
+    p.partials, p.out, p.ssi = _ptr(partials), _ptr(out), _ptr(ssi)
+    cabi.check(_launch("depth_metrics_kernel", 0.0, lambda: cabi.lib().udb_depth_metrics(C.byref(p), _stream()),
+                       _nb(gt, pred, mask) * 2), "udb_depth_metrics")
+    return out, ssi
+
+
+def point_metrics(gt, pred, lengths, dist_x, dist_y, thresholds):
+    """Per-cloud sums and F1 histograms of eval_3d (udb_point_metrics): gt, pred [N, P, 3] f32, lengths int64 [N] or
+    None, dist_x, dist_y [N, P] f32, thresholds [T] f32 ascending.  Returns out [N, 2 + 2T] f64."""
+    for n, t in (("gt", gt), ("pred", pred), ("dist_x", dist_x), ("dist_y", dist_y), ("thresholds", thresholds)):
+        _metric_operand(n, t, f32)
+    if lengths is not None:
+        _metric_operand("lengths", lengths, torch.int64)
+    N, P, _ = gt.shape
+    T = thresholds.numel()
+    dev = gt.device
+    partials = torch.empty((N, cabi.METRIC_MAX_BLOCKS, 2 + 2 * T), device=dev, dtype=torch.float64)
+    out = torch.empty((N, 2 + 2 * T), device=dev, dtype=torch.float64)
+    p = cabi.PointMetrics()
+    p.gt, p.pred, p.lengths, p.dist_x, p.dist_y, p.thresholds = (_ptr(gt), _ptr(pred), _ptr(lengths), _ptr(dist_x),
+                                                                 _ptr(dist_y), _ptr(thresholds))
+    p.N, p.P, p.n_thresholds = N, P, T
+    p.partials, p.out = _ptr(partials), _ptr(out)
+    cabi.check(_launch("point_metrics_kernel", 0.0, lambda: cabi.lib().udb_point_metrics(C.byref(p), _stream()),
+                       _nb(gt, pred, dist_x, dist_y)), "udb_point_metrics")
+    return out
