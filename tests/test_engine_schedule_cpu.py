@@ -35,15 +35,15 @@ def _v2(cfg_name, depth=None, **attrs):
 
 
 def _v2_engine(m, drop=(), reshape=None):
-    P = m._pack_tensors(CPU)
-    tensors, scalars = m._flatten_packed(P)
+    tensors, scalars = m._pack_tensors(CPU)
+    cfg = m._engine_config(tensors)
     for name in drop:
         del tensors[name]
     if reshape:
         name, fn = reshape
         tensors[name] = fn(tensors[name]).contiguous()
     h = C.c_void_p()
-    _cabi.check(_cabi.lib().udb_create(C.byref(m._engine_config(P)), C.byref(h)), "udb_create")
+    _cabi.check(_cabi.lib().udb_create(C.byref(cfg), C.byref(h)), "udb_create")
     m._register(h, tensors, scalars)
     return h, tensors          # the caller keeps `tensors` alive while the engine holds their pointers
 
@@ -80,8 +80,7 @@ def test_v2_packer_and_schedule_agree(cfg_name, depth, attrs):
 def test_v2_schedule_names_the_missing_or_misshapen_operand():
     lib = _cabi.lib()
     m = _v2("config_v2_vits14.json")
-    P = m._pack_tensors(CPU)
-    names = list(m._flatten_packed(P)[0])
+    names = list(m._pack_tensors(CPU)[0])
     # every registered tensor is needed: dropping any one of a spread of them is reported by name
     for name in names[:: max(1, len(names) // 12)]:
         h, keep = _v2_engine(m, drop=(name,))

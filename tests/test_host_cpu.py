@@ -116,6 +116,20 @@ def test_state_dict_round_trip_and_no_cpu_fallback():
         m.infer(torch.zeros(3, 64, 64, dtype=torch.uint8))
     with pytest.raises(NotImplementedError):
         m(torch.zeros(1))
+    # UniDepthV1 (a small ConvNeXt) through the same hub-mixin round trip
+    from unidepth_b200 import UniDepthV1
+    cfg1 = _cfg("config_v1_cnvnxtl.json")
+    cfg1["model"]["pixel_encoder"]["arch"] = {"depths": [1, 1, 2, 1], "dims": [64, 128, 192, 256]}
+    m1 = UniDepthV1(cfg1)
+    info = m1.load_state_dict(fixture.make_v1_state_dict(cfg1, 3), strict=True)
+    assert not info.missing_keys and not info.unexpected_keys
+    with tempfile.TemporaryDirectory() as d:
+        m1.save_pretrained(d)
+        assert os.path.exists(os.path.join(d, "config.json")) and os.path.exists(os.path.join(d, "model.safetensors"))
+        m3 = UniDepthV1.from_pretrained(d)
+    assert isinstance(m3, UniDepthV1) and m3.spec.dims == (64, 128, 192, 256)
+    for k, v in m1.state_dict().items():
+        assert torch.equal(v, m3.state_dict()[k]), k
 
 
 def test_unknown_encoder_is_rejected():

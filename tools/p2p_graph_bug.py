@@ -24,7 +24,7 @@ lo, hi = shard_bounds(4, rank, world)
 
 def wsum():
     torch.cuda.synchronize()
-    T, _ = m._flatten_packed(m._weights())
+    T, _ = m._weights()
     return {k: float(v.double().abs().sum()) for k, v in T.items()}
 
 def diff(a, b, tag):

@@ -1,6 +1,6 @@
-"""Stage-by-stage parity report: CUDA path (unidepth_b200) vs the CPU oracle on the same seeded
-weights / input.  Test infrastructure (imports oracle/).  Usage on the GPU box:
-    python tools/parity_report.py [--depth N] [--batch B] [--hw H W] [--seed S] [--no-graph]
+"""Output parity report: CUDA path (unidepth_b200.UniDepthV2.infer, eager and CUDA graph) vs the CPU oracle on the
+same seeded weights / input.  Test infrastructure (imports oracle/).  Usage on a GPU machine:
+    python tools/parity_report.py [--depth N] [--batch B] [--hw H W] [--seed S] [--config NAME]
 --depth N builds a shallow ViT-L-shaped encoder (arch_override) so the oracle runs in a second."""
 import argparse
 import copy
@@ -46,36 +46,15 @@ def main():
     rgb = torch.randint(0, 256, (args.batch, 3, args.hw[0], args.hw[1]), dtype=torch.uint8, generator=g)
     torch.set_num_threads(os.cpu_count())
     t0 = time.time()
-    otaps = {}
-    ref = O.infer_v2(sd, copy.deepcopy(cfg), rgb, taps_out=otaps)
+    ref = O.infer_v2(sd, copy.deepcopy(cfg), rgb)
     print(f"oracle: {time.time()-t0:.1f}s on {os.cpu_count()} cores", flush=True)
 
     model = UniDepthV2(copy.deepcopy(cfg))
     model.load_state_dict(sd, strict=True)
     model = model.to("cuda").eval()
     model.use_cuda_graph = False
-    # tap run
-    from unidepth_b200.spec import get_paddings, get_resize_factor, pixel_bounds
-    import math
-    H, W = args.hw
-    paddings, (ph, pw) = get_paddings((H, W), model.shape_constraints["ratio_bounds"])
-    factor, (nh, nw) = get_resize_factor((ph, pw), pixel_bounds(model.shape_constraints, None))
-    gh, gw = nh // 14, nw // 14
-    geom = dict(paddings=paddings, padded_hw=(ph, pw), factor=factor, net_hw=(nh, nw), out_hw=(H, W),
-                scales=(2.0 ** torch.linspace(0.0, math.log2(max(gh, gw) // 2), steps=model.spec.hidden // 2)).cuda())
-    taps = {}
-    with torch.no_grad():
-        out = model._forward(rgb.cuda(), geom, True, taps=taps)
-    torch.cuda.synchronize()
-    print("---- stage taps (max rel, mean rel; floor = 10% of mean |ref|)")
-    for k in ["tokens0", "block0", "feat3", "cls3", "intrinsics4", "ray_embedding", "cond0", "ups0", "ups1", "ups2"]:
-        if k in taps and k in otaps:
-            a, b = taps[k], otaps[k]
-            if k.startswith("ups"):
-                a = a.permute(0, 3, 1, 2)
-            mx, mn = rel(a.reshape(b.shape), b)
-            print(f"{k:14s} max {mx:.3e} mean {mn:.3e}", flush=True)
-    print("---- outputs")
+    out = model.infer(rgb)
+    print("---- outputs (max rel, mean rel; floor = 10% of mean |ref|)")
     for k in ["intrinsics", "depth", "radius", "points", "rays", "confidence", "depth_features"]:
         mx, mn = rel(out[k], ref[k])
         print(f"{k:14s} max {mx:.3e} mean {mn:.3e}")
@@ -84,7 +63,7 @@ def main():
     K, Kr = out["intrinsics"].cpu(), ref["intrinsics"]
     for nm, (i, j) in dict(fx=(0, 0), fy=(1, 1), cx=(0, 2), cy=(1, 2)).items():
         print(f"{nm}: rel err {((K[:, i, j]-Kr[:, i, j]).abs()/Kr[:, i, j].abs()).max().item():.3e}")
-    # public API (+ CUDA graph) must equal the eager tap run
+    # CUDA graph capture and replay must equal the eager call
     model.use_cuda_graph = True
     o2 = model.infer(rgb)
     o3 = model.infer(rgb)

@@ -1,0 +1,216 @@
+"""Host runtime shared by UniDepthV1 and UniDepthV2: parameters under the reference's state-dict names, checkpoint
+loading, weight packing per weight version, the C engine's lifetime, and the workspace and CUDA-graph caches.
+
+A model class supplies its packer (`_pack_tensors` -> ({engine tensor name: tensor}, {scalar name: float})), its engine
+(`_get_engine`, `_forward_engine`) and the names of its engine's C entry points (`_ENGINE_FNS`)."""
+from __future__ import annotations
+
+import ctypes as C
+import json
+import os
+from collections import OrderedDict
+
+import torch
+import torch.nn as nn
+
+from . import _cabi as cabi
+
+try:  # same mixin as the reference (unidepthv2.py:111-117)
+    from huggingface_hub import PyTorchModelHubMixin
+    _HAS_HF = True
+except Exception:  # pragma: no cover
+    _HAS_HF = False
+
+    class PyTorchModelHubMixin:  # minimal stand-in: local directories only
+        def __init_subclass__(cls, **kwargs):
+            super().__init_subclass__()
+
+# Class keywords of the hub mixin.  Each public model class lists the mixin and these itself: the mixin records the
+# __init__ of the class it is declared on.
+HUB_KWARGS = dict(library_name="UniDepth", repo_url="https://github.com/lpiccinelli-eth/UniDepth",
+                  tags=["monocular-metric-depth-estimation"]) if _HAS_HF else {}
+
+f16, f32 = torch.float16, torch.float32
+
+
+class _Node(nn.Module):
+    """Anonymous container used to reproduce the reference's dotted parameter names."""
+
+
+class EngineModel(nn.Module):
+    # include/udb.h entry points of the model's engine: (create, destroy, set_weight, set_scalar)
+    _ENGINE_FNS: tuple
+
+    def __init__(self, config: dict, eps: float, max_cached_workspaces: int):
+        super().__init__()
+        self.config = config
+        self.eps = eps
+        self.use_cuda_graph = True
+        # optional dict of preallocated output tensors (same keys / shapes as infer's result): graph-mode infer copies its
+        # static outputs there instead of cloning them (parallel.PeerGather.views(): the multi-GPU send slot)
+        self.output_buffers = None
+        # Bounded caches (LRU): the reference handles arbitrary shapes in constant memory, so a stream of
+        # differently-sized images must not grow device memory without limit.  A captured graph keeps its own
+        # reference to the workspace it was captured with, so evicting a workspace never frees memory a live
+        # graph still replays into.
+        self.max_cached_graphs = 8
+        self.max_cached_workspaces = max_cached_workspaces
+        self._graphs: "OrderedDict[tuple, dict]" = OrderedDict()
+        self._workspaces: "OrderedDict[tuple, torch.Tensor]" = OrderedDict()
+        self._last_ws = None
+        self._packed = None          # (tensors, scalars) of the weight version `_packed_key`
+        self._packed_key = None
+        self._engine = self._engine_key = self._engine_device = None
+
+    def _add_params(self, shapes: dict):
+        """Zero f32 parameters under the reference's dotted state-dict names."""
+        for dotted, shape in shapes.items():
+            *path, leaf = dotted.split(".")
+            mod = self
+            for p in path:
+                if p not in mod._modules:
+                    mod.add_module(p, _Node())
+                mod = mod._modules[p]
+            mod.register_parameter(leaf, nn.Parameter(torch.zeros(shape, dtype=f32), requires_grad=False))
+
+    # ------------------------------------------------------------------ reference-compatible API
+    @property
+    def device(self):
+        return next(self.parameters()).device
+
+    def load_pretrained(self, model_file: str):
+        """unidepthv2.py:381-394 / unidepthv1.py:375-392: torch checkpoint, optional 'model' key, strip 'module.'."""
+        sd = torch.load(model_file, map_location="cpu", weights_only=False)
+        if "model" in sd:
+            sd = sd["model"]
+        sd = {k.replace("module.", ""): v for k, v in sd.items()}
+        info = self.load_state_dict(sd, strict=False)
+        print(f"Loaded from {model_file} for {self.__class__.__name__} results in:", info)
+
+    if not _HAS_HF:
+        @classmethod
+        def from_pretrained(cls, path: str, **kwargs):
+            config = json.load(open(os.path.join(path, "config.json")))
+            model = cls(config=config.get("config", config))
+            st = os.path.join(path, "model.safetensors")
+            if os.path.exists(st):
+                from safetensors.torch import load_file
+                model.load_state_dict(load_file(st), strict=False)
+            else:
+                model.load_state_dict(torch.load(os.path.join(path, "pytorch_model.bin"), map_location="cpu"),
+                                      strict=False)
+            return model
+
+    # ------------------------------------------------------------------ weight packing
+    def _fingerprint(self):
+        return tuple((p.data_ptr(), p._version) for p in self.parameters())
+
+    def _weights(self):
+        """The packed (tensors, scalars), repacked once per weight version; a repack drops the engine and its caches."""
+        if self._packed is None or self._packed_key != self._fingerprint():
+            dev = self.device
+            if dev.type != "cuda":
+                raise RuntimeError(f"unidepth_b200.{type(self).__name__}.infer needs the model on a CUDA device "
+                                   "(model.to('cuda')); there is no CPU fallback")
+            torch.cuda.set_device(dev)      # callers hold `with torch.cuda.device(self.device)`
+            self._drop_engine()             # it borrows the pointers of the tensors about to be replaced
+            self._packed = self._pack_tensors(dev)
+            self._packed_key = self._fingerprint()
+        return self._packed
+
+    # ------------------------------------------------------------------ C engine
+    def _register(self, handle, tensors: dict, scalars: dict):
+        """set_weight / set_scalar for every packed operand (the engine borrows the pointers)."""
+        _, _, set_weight, set_scalar = self._ENGINE_FNS
+        lib = cabi.lib()
+        for name, t in tensors.items():
+            assert t.is_contiguous() and t.dtype in (f16, f32), name
+            shape = (C.c_int64 * max(t.ndim, 1))(*t.shape)
+            cabi.check(getattr(lib, set_weight)(handle, name.encode(), C.c_void_p(t.data_ptr()), shape, t.ndim,
+                                                cabi.DT_F32 if t.dtype == f32 else cabi.DT_F16), f"{set_weight}({name})")
+        for name, v in scalars.items():
+            cabi.check(getattr(lib, set_scalar)(handle, name.encode(), float(v)), f"{set_scalar}({name})")
+
+    def _create_engine(self, cfg, key=None):
+        """A new engine for the config struct `cfg`, with the current packed weights registered; `key` is what the
+        caller compares to decide when to rebuild it."""
+        tensors, scalars = self._weights()
+        create = self._ENGINE_FNS[0]
+        handle = C.c_void_p()
+        cabi.check(getattr(cabi.lib(), create)(C.byref(cfg), C.byref(handle)), create)
+        for name, t in tensors.items():
+            assert t.is_cuda, name
+        self._register(handle, tensors, scalars)
+        self._engine, self._engine_key, self._engine_device = handle, key, self.device
+        return handle
+
+    def _drop_engine(self):
+        """Destroy the engine AND everything that holds raw pointers into it: captured graphs replay kernels whose
+        arguments point at the engine's tables and at the workspaces, so they go first."""
+        self._graphs.clear()
+        if self._engine is not None:
+            torch.cuda.synchronize(self._engine_device)       # nothing may still be running out of the tables we free
+            getattr(cabi.lib(), self._ENGINE_FNS[1])(self._engine)
+        self._engine = self._engine_key = None
+        self._workspaces.clear()
+
+    def __del__(self):
+        try:
+            self._drop_engine()
+        except Exception:
+            pass
+
+    def _workspace(self, key: tuple, nbytes) -> torch.Tensor:
+        """The cached workspace for `key`, or a new one of `nbytes()` bytes (0: the engine refused the shape)."""
+        ws = self._workspaces.get(key)
+        if ws is None:
+            n = nbytes()
+            if n == 0:
+                raise RuntimeError(f"engine workspace sizing failed: {cabi.lib().udb_last_error().decode()}")
+            ws = torch.empty(n, device=self.device, dtype=torch.uint8)
+            self._workspaces[key] = ws
+            while len(self._workspaces) > self.max_cached_workspaces:
+                self._workspaces.popitem(last=False)
+        else:
+            self._workspaces.move_to_end(key)
+        self._last_ws = ws
+        return ws
+
+    # ------------------------------------------------------------------ CUDA graphs
+    def _run_graphed(self, run, rgb: torch.Tensor, inputs: dict, key: tuple, keep=None) -> dict:
+        """`run(rgb, inputs)` -> outputs, eagerly or by replaying a CUDA graph cached under `key`.  The caller packs the
+        weights (`_weights()`) before this: a repack drops every graph, so none replays stale weights.  The graph reads
+        static copies of `rgb` and of the tensors in `inputs`, refreshed before every replay; `keep` is anything else a
+        captured kernel reads, which the cache entry must own."""
+        if not self.use_cuda_graph:
+            return run(rgb, inputs)
+        entry = self._graphs.get(key)
+        if entry is None:
+            static_in = rgb.clone()
+            static_inputs = {k: v.clone() for k, v in inputs.items()}
+            # warm-up on a side stream (allocator, per-shape tables, workspace), then capture
+            side = torch.cuda.Stream()
+            side.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(side):
+                run(static_in, static_inputs)
+            torch.cuda.current_stream().wait_stream(side)
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                static_out = run(static_in, static_inputs)
+            # the entry owns everything whose address the captured kernels read
+            entry = dict(graph=graph, inp=static_in, inputs=static_inputs, out=static_out, ws=self._last_ws, keep=keep)
+            self._graphs[key] = entry
+            while len(self._graphs) > self.max_cached_graphs:
+                self._graphs.popitem(last=False)
+        else:
+            self._graphs.move_to_end(key)
+        entry["inp"].copy_(rgb, non_blocking=True)
+        for k, v in inputs.items():
+            entry["inputs"][k].copy_(v, non_blocking=True)
+        entry["graph"].replay()
+        bufs = self.output_buffers
+        if bufs is not None:       # caller-provided destinations (e.g. the send slot of parallel.PeerGather): one copy, no clone
+            for k, v in entry["out"].items():
+                bufs[k].copy_(v)
+            return {k: bufs[k] for k in entry["out"]}
+        return {k: v.clone() for k, v in entry["out"].items()}

@@ -259,10 +259,6 @@ def posembed_bicubic(grid, m, dim, gh, gw):
     return out
 
 
-def set_cls_rows(x, cls_token, pos0, B, T, D):
-    cabi.check(cabi.lib().udb_set_cls_rows(_ptr(x), _ptr(cls_token), _ptr(pos0), B, T, D, _stream()), "udb_set_cls_rows")
-
-
 def small_linear(x, w, bias=None, act=ACT_NONE, gamma=None, resid=None, out=None):
     """fp32 y = resid + gamma * act(x @ w.T + bias); x / out / resid may be row-strided 2-D views."""
     M, K = x.shape

@@ -19,22 +19,17 @@ function is unpinned (see DESIGN.md).
 from __future__ import annotations
 
 import ctypes as C
-import json
 import math
-import os
-from collections import OrderedDict
 from typing import Dict, Optional
 
 import torch
-import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _cabi as cabi
 from .spec_v1 import (ENCODER_CONVNEXT, ENCODER_DINOV2, V1_INTERPOLATE_OFFSET, V1Spec, param_shapes, v1_paddings,
                       v1_shapes)
-from .unidepthv2 import PyTorchModelHubMixin, _HAS_HF, _register, pack_vit_encoder
-
-f16, f32 = torch.float16, torch.float32
+from ._engine_model import HUB_KWARGS, EngineModel, PyTorchModelHubMixin, f16, f32
+from .unidepthv2 import pack_vit_encoder
 
 
 def _offset_pos_embed(pos: torch.Tensor, gh: int, gw: int, offset: float) -> torch.Tensor:
@@ -66,70 +61,18 @@ def _sine_position_embedding(h: int, w: int, num_pos_feats: int, device) -> torc
     return torch.cat((py, px), dim=2).reshape(h * w, 2 * num_pos_feats)
 
 
-class UniDepthV1(nn.Module, PyTorchModelHubMixin,
-                 **(dict(library_name="UniDepth", repo_url="https://github.com/lpiccinelli-eth/UniDepth",
-                         tags=["monocular-metric-depth-estimation"]) if _HAS_HF else {})):
+class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
+    _ENGINE_FNS = ("udb_v1_create", "udb_v1_destroy", "udb_v1_set_weight", "udb_v1_set_scalar")
+
     def __init__(self, config: dict, eps: float = 1e-6, **kwargs):
-        super().__init__()
-        self.config = config
-        self.eps = eps
+        super().__init__(config, eps, max_cached_workspaces=4)
         self.spec = V1Spec(config)
-        for key, shape in param_shapes(config).items():
-            _register(self, key, torch.zeros(shape, dtype=f32))
+        self._add_params(param_shapes(config))
         self.image_shape = list(self.spec.image_shape)        # unidepthv1.py:447
-        self.use_cuda_graph = True
-        self.max_cached_graphs = 8
-        self.output_buffers = None      # see UniDepthV2.output_buffers
-        self._engine = None
-        self._packed: Optional[dict] = None
-        self._packed_key = None
-        self._graphs: "OrderedDict[tuple, dict]" = OrderedDict()
-        self._workspaces: "OrderedDict[tuple, torch.Tensor]" = OrderedDict()
-
-    # ------------------------------------------------------------------ reference-compatible API
-    @property
-    def device(self):
-        return next(self.parameters()).device
-
-    def load_pretrained(self, model_file: str):
-        """unidepthv1.py:375-392."""
-        sd = torch.load(model_file, map_location="cpu", weights_only=False)
-        if "model" in sd:
-            sd = sd["model"]
-        sd = {k.replace("module.", ""): v for k, v in sd.items()}
-        info = self.load_state_dict(sd, strict=False)
-        print(f"Loaded from {model_file} for {self.__class__.__name__} results in:", info)
-
-    if not _HAS_HF:
-        @classmethod
-        def from_pretrained(cls, path: str, **kwargs):
-            config = json.load(open(os.path.join(path, "config.json")))
-            model = cls(config=config.get("config", config))
-            st = os.path.join(path, "model.safetensors")
-            if os.path.exists(st):
-                from safetensors.torch import load_file
-                model.load_state_dict(load_file(st), strict=False)
-            else:
-                model.load_state_dict(torch.load(os.path.join(path, "pytorch_model.bin"), map_location="cpu"), strict=False)
-            return model
 
     # ------------------------------------------------------------------ weight packing
-    def _fingerprint(self):
-        return tuple((p.data_ptr(), p._version) for p in self.parameters())
-
-    def _pack(self):
-        dev = self.device
-        if dev.type != "cuda":
-            raise RuntimeError("unidepth_b200.UniDepthV1.infer needs the model on a CUDA device (model.to('cuda')); "
-                               "there is no CPU fallback")
-        torch.cuda.set_device(dev)
-        T, S = self._pack_tensors(dev)
-        self._packed = dict(T=T, S=S)
-        self._packed_key = self._fingerprint()
-        self._drop_engine()
-
     def _pack_tensors(self, dev):
-        """({engine tensor name: tensor on `dev`}, {scalar name: float}): plain torch layout work.  `_pack` is the only
+        """({engine tensor name: tensor on `dev`}, {scalar name: float}): plain torch layout work.  `_weights` is the only
         product caller (CUDA device); tests/test_engine_schedule_cpu.py runs it on the CPU to check, through the engine's
         dry run, that the packer registers exactly the operands the C schedule asks for."""
         s = self.spec
@@ -167,12 +110,8 @@ class UniDepthV1(nn.Module, PyTorchModelHubMixin,
         if s.encoder == ENCODER_DINOV2:
             # default f16 packing of the V2 encoder; the final norm, mask token and register tokens are never read
             # (use_norm=False, dinov2.py:173-178)
-            E = pack_vit_encoder(sd, s.embed_dim, s.enc_depth, dev)
-            T["patch_w"], T["patch_b"], T["cls"] = E["patch_w"], E["patch_b"], E["cls"]
-            for i, blk in enumerate(E["blocks"]):
-                for k, v in blk.items():
-                    T[f"blocks.{i}.{k}"] = v
-            T["pos"] = c32(_offset_pos_embed(E["pos"], hc, wc, V1_INTERPOLATE_OFFSET))
+            T.update(pack_vit_encoder(sd, s.embed_dim, s.enc_depth, dev))
+            T["pos"] = c32(_offset_pos_embed(T["pos"], hc, wc, V1_INTERPOLATE_OFFSET))
         for i, depth in enumerate(s.depths if s.encoder == ENCODER_CONVNEXT else ()):
             if i == 0:
                 T["stem_w"] = h16(zpad(sd[pe + "stem.0.weight"].reshape(s.dims[0], 48), s.dims[0], 64))
@@ -278,26 +217,7 @@ class UniDepthV1(nn.Module, PyTorchModelHubMixin,
             S[f"{name}.b"] = float(sd[f"{dl}{name}.bias"].item())
         return T, S
 
-    def _weights(self):
-        if self._packed is None or self._packed_key != self._fingerprint():
-            self._pack()
-        return self._packed
-
     # ------------------------------------------------------------------ engine
-    def _drop_engine(self):
-        self._graphs.clear()
-        if self._engine is not None:
-            torch.cuda.synchronize(self._engine_device)
-            cabi.lib().udb_v1_destroy(self._engine)
-        self._engine = None
-        self._workspaces.clear()
-
-    def __del__(self):
-        try:
-            self._drop_engine()
-        except Exception:
-            pass
-
     def _engine_config(self) -> "cabi.V1Config":
         """udb_v1_config_t of this model (include/udb.h)."""
         s = self.spec
@@ -311,46 +231,18 @@ class UniDepthV1(nn.Module, PyTorchModelHubMixin,
         cfg.encoder = s.encoder
         return cfg
 
-    @staticmethod
-    def _register(handle, tensors: dict, scalars: dict):
-        """udb_v1_set_weight / udb_v1_set_scalar for every packed operand (the engine borrows the pointers)."""
-        lib = cabi.lib()
-        for name, t in tensors.items():
-            assert t.is_contiguous() and t.dtype in (f16, f32), name
-            shape = (C.c_int64 * max(t.ndim, 1))(*t.shape)
-            cabi.check(lib.udb_v1_set_weight(handle, name.encode(), C.c_void_p(t.data_ptr()), shape, t.ndim,
-                                             cabi.DT_F32 if t.dtype == f32 else cabi.DT_F16), f"udb_v1_set_weight({name})")
-        for name, v in scalars.items():
-            cabi.check(lib.udb_v1_set_scalar(handle, name.encode(), float(v)), f"udb_v1_set_scalar({name})")
-
     def _get_engine(self):
-        P = self._weights()
+        self._weights()
         if self._engine is not None:
             return self._engine
-        handle = C.c_void_p()
-        cabi.check(cabi.lib().udb_v1_create(C.byref(self._engine_config()), C.byref(handle)), "udb_v1_create")
-        for name, t in P["T"].items():
-            assert t.is_cuda, name
-        self._register(handle, P["T"], P["S"])
-        self._engine, self._engine_device = handle, self.device
-        return handle
+        return self._create_engine(self._engine_config())
 
     def _forward_engine(self, rgb: torch.Tensor, K: Optional[torch.Tensor], skip_camera: bool, scale255: bool, normalize: bool):
         eng = self._get_engine()
         lib = cabi.lib()
         dev = rgb.device
         B, _, H, W = rgb.shape
-        wkey = (B, H, W)
-        ws = self._workspaces.get(wkey)
-        if ws is None:
-            nbytes = lib.udb_v1_workspace_bytes(eng, B, H, W)
-            if nbytes == 0:
-                raise RuntimeError(f"udb_v1_workspace_bytes failed: {lib.udb_last_error().decode()}")
-            ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
-            self._workspaces[wkey] = ws
-            while len(self._workspaces) > 4:
-                self._workspaces.popitem(last=False)
-        self._last_ws = ws
+        ws = self._workspace((B, H, W), lambda: lib.udb_v1_workspace_bytes(eng, B, H, W))
         out = {"intrinsics": torch.empty((B, 3, 3), device=dev, dtype=f32),
                "points": torch.empty((B, 3, H, W), device=dev, dtype=f32),
                "depth": torch.empty((B, 1, H, W), device=dev, dtype=f32)}
@@ -396,38 +288,9 @@ class UniDepthV1(nn.Module, PyTorchModelHubMixin,
                     raise ValueError(f"intrinsics holds {K.shape[0]} matrices for a batch of {B} images")
                 K = K.contiguous()
             self._weights()
-            run = lambda x, k: self._forward_engine(x, k, skip_camera, scale255, normalize)
-            if not self.use_cuda_graph:
-                return run(rgbs, K)
+            run = lambda x, inputs: self._forward_engine(x, inputs.get("K"), skip_camera, scale255, normalize)
             key = (tuple(rgbs.shape), rgbs.dtype, scale255, normalize, K is not None, bool(skip_camera))
-            entry = self._graphs.get(key)
-            if entry is None:
-                static_in = rgbs.clone()
-                static_k = K.clone() if K is not None else None
-                side = torch.cuda.Stream()
-                side.wait_stream(torch.cuda.current_stream())
-                with torch.cuda.stream(side):
-                    run(static_in, static_k)
-                torch.cuda.current_stream().wait_stream(side)
-                graph = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(graph):
-                    static_out = run(static_in, static_k)
-                entry = dict(graph=graph, inp=static_in, k=static_k, out=static_out, ws=self._last_ws)
-                self._graphs[key] = entry
-                while len(self._graphs) > self.max_cached_graphs:
-                    self._graphs.popitem(last=False)
-            else:
-                self._graphs.move_to_end(key)
-            entry["inp"].copy_(rgbs, non_blocking=True)
-            if K is not None:
-                entry["k"].copy_(K, non_blocking=True)
-            entry["graph"].replay()
-            bufs = self.output_buffers
-            if bufs is not None:
-                for k, v in entry["out"].items():
-                    bufs[k].copy_(v)
-                return {k: bufs[k] for k in entry["out"]}
-            return {k: v.clone() for k, v in entry["out"].items()}
+            return self._run_graphed(run, rgbs, {} if K is None else {"K": K}, key)
 
     def forward(self, *args, **kwargs):
         raise NotImplementedError("training / validation forward of UniDepthV1 is out of scope; use .infer()")
