@@ -124,12 +124,12 @@ def test_v1_packer_and_schedule_agree(arch):
         assert lib.udb_v1_workspace_bytes(h, 0, 480, 640) == 0
     finally:
         lib.udb_v1_destroy(h)
-    # one operand short: reported by name
-    for name in list(T)[:: max(1, len(T) // 10)]:
+    # one operand or scalar short (the output heads' biases included): reported by name
+    for name in list(T)[:: max(1, len(T) // 10)] + list(S):
         h = C.c_void_p()
         _cabi.check(lib.udb_v1_create(C.byref(m._engine_config()), C.byref(h)), "udb_v1_create")
         try:
-            m._register(h, {k: v for k, v in T.items() if k != name}, S)
+            m._register(h, {k: v for k, v in T.items() if k != name}, {k: v for k, v in S.items() if k != name})
             assert lib.udb_v1_workspace_bytes(h, 1, 480, 640) == 0
             assert name in lib.udb_last_error().decode(), (name, lib.udb_last_error().decode())
         finally:

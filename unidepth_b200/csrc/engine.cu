@@ -26,15 +26,12 @@ constexpr int PATCH = 14;
 struct udb_engine : udb::EngineBase {
   udb_config_t cfg;
   std::unordered_map<long long, udb::ShapeTables> tables;
-  std::unordered_map<std::string, size_t> ws_need;   // "B,H,W,level" -> bytes (filled by udb_workspace_bytes)
 };
 
 namespace udb {
 
 // ------------------------------------------------------------------------------------------ geometry
 // unidepthv2.py:36-58 (Python float == C double; int() truncates toward zero)
-static inline int floordiv2(int v) { return v >= 0 ? v / 2 : -((-v + 1) / 2); }   // Python's v // 2
-
 static void paddings(int H, int W, double lo, double hi, udb_geometry_t* g) {
   const double ratio = static_cast<double>(W) / H;
   const double target = fmin(hi, fmax(lo, ratio));
@@ -102,13 +99,13 @@ static int run(udb_engine* e, const udb_infer_args_t& a, const udb_geometry_t& g
   __half* x16 = fuse ? ar.h(BT * D) : nullptr;
   float* stats = fuse ? ar.f(BT * ln_parts * 2) : nullptr;
   __half* patches = ar.h(BN * 640 * sx);
-  if (!c.dry) {
+  {
     udb_preprocess_t p;
     memset(&p, 0, sizeof(p));
     p.rgb = a.rgb; p.rgb_is_u8 = a.rgb_is_u8; p.normalize = a.normalize; p.B = B; p.H = a.H; p.W = a.W;
     p.pad_l = g.pad_l; p.pad_r = g.pad_r; p.pad_t = g.pad_t; p.pad_b = g.pad_b; p.net_h = nh; p.net_w = nw;
     p.patches = patches; p.ldp = 640 * sx; p.split = sp ? 1 : 0;
-    c.done(udb_preprocess_patchify(&p, st));
+    c.launch([&] { return udb_preprocess_patchify(&p, st); });
   }
   float* x = ar.f(BT * D);           // fp32 residual stream
   {
@@ -119,9 +116,11 @@ static int run(udb_engine* e, const udb_infer_args_t& a, const udb_geometry_t& g
     c.expect2("patch_w", D, sp ? 3 * 640 : 640);
     if (fuse) { q.out2 = x16; q.out2_leaky = 0; q.ln_stats_out = stats; q.ln_parts = ln_parts; q.ln_part_cols = ln_pc; }
     c.gemm(q);
-    if (!c.dry && !c.rc)
-      c.done(fuse ? udb_set_cls_rows_ln(x, x16, stats, c.F("cls"), tb.pos, B, T, D, ln_parts, ln_pc, st)
-                  : udb_set_cls_rows(x, c.F("cls"), tb.pos, B, T, D, st));
+    const float* cls = c.F("cls");
+    c.launch([&] {
+      return fuse ? udb_set_cls_rows_ln(x, x16, stats, cls, tb.pos, B, T, D, ln_parts, ln_pc, st)
+                  : udb_set_cls_rows(x, cls, tb.pos, B, T, D, st);
+    });
   }
 
   // ---- a5-a8: transformer blocks, taps through the final norm
@@ -171,7 +170,8 @@ static int run(udb_engine* e, const udb_infer_args_t& a, const udb_geometry_t& g
     c.small_linear(xn, R4, hid, c.F(ag + ".q"), hid, nullptr, UDB_ACT_NONE, nullptr, nullptr, q);
     c.small_linear(cn, R4, hid, c.F(ag + ".kv"), 2 * hid, nullptr, UDB_ACT_NONE, nullptr, nullptr, kv);
     float* a4 = ar.f(static_cast<size_t>(R4) * hid);
-    if (!c.dry && !c.rc) c.done(udb_camera_attn4_f32(q, kv, c.F("cam.pos"), a4, B, hid, cf.dec_heads, st));
+    const float* cam_pos = c.F("cam.pos");
+    c.launch([&] { return udb_camera_attn4_f32(q, kv, cam_pos, a4, B, hid, cf.dec_heads, st); });
     float* t2 = ar.f(static_cast<size_t>(R4) * hid);
     c.small_linear(a4, R4, hid, c.F(ag + ".out"), hid, nullptr, UDB_ACT_NONE, c.F(ag + ".ls1"), t, t2);
     t = cam_mlp(c, ag + ".mlp", t2, R4, hid, cf.expansion * hid, hid, t2, c.F(ag + ".ls2"));
@@ -179,8 +179,9 @@ static int run(udb_engine* e, const udb_infer_args_t& a, const udb_geometry_t& g
   float* x4 = cam_mlp(c, "cam.pinhole", t, R4, hid, hid, 1, nullptr, nullptr);   // [B*4,1] == [B,4]
   float* intr4 = ar.f(static_cast<size_t>(B) * 4);
   float* k_net = ar.f(static_cast<size_t>(B) * 9);
-  if (!c.dry && !c.rc)
-    c.done(udb_camera_intrinsics(x4, B, nh, nw, static_cast<float>(g.factor), g.pad_l, g.pad_t, intr4, k_net, a.intrinsics, st));
+  c.launch([&] {
+    return udb_camera_intrinsics(x4, B, nh, nw, static_cast<float>(g.factor), g.pad_l, g.pad_t, intr4, k_net, a.intrinsics, st);
+  });
 
   stage.next("udb:ray_embedding+prompt_blocks");
   // ---- a11/a12: rays (predicted K, or the caller's pinhole K) -> Fourier embedding on the patch grid
@@ -189,22 +190,23 @@ static int run(udb_engine* e, const udb_infer_args_t& a, const udb_geometry_t& g
   const float* rays_in = a.camera_rays;
   if (a.camera_model != UDB_CAM_NONE) {
     float* gen = ar.f(static_cast<size_t>(B) * nh * nw * 3);
-    if (!c.dry && !c.rc)
-      c.done(udb_camera_rays(a.camera_model, a.camera_params, B, nh, nw, g.pad_l, g.pad_r, g.pad_t, g.pad_b,
-                             static_cast<float>(g.factor), gen, st));
+    c.launch([&] {
+      return udb_camera_rays(a.camera_model, a.camera_params, B, nh, nw, g.pad_l, g.pad_r, g.pad_t, g.pad_b,
+                             static_cast<float>(g.factor), gen, st);
+    });
     rays_in = gen;
   } else if (a.camera_k && !a.camera_rays) {
     float* gt4 = ar.f(static_cast<size_t>(B) * 4);
-    if (!c.dry && !c.rc) c.done(udb_camera_adjust_k(a.camera_k, B, static_cast<float>(g.factor), g.pad_l, g.pad_t, gt4, st));
+    c.launch([&] { return udb_camera_adjust_k(a.camera_k, B, static_cast<float>(g.factor), g.pad_l, g.pad_t, gt4, st); });
     ray_intr = gt4;
   }
   float* remb = ar.f(BN * hid);
-  if (!c.dry && !c.rc) {
+  {
     udb_ray_embed_t p;
     memset(&p, 0, sizeof(p));
     p.intr4 = ray_intr; p.rays_in = rays_in; p.scales = a.ray_scales ? a.ray_scales : tb.scales;
     p.B = B; p.net_h = nh; p.net_w = nw; p.gh = gh; p.gw = gw; p.bands = hid / 2; p.out = remb; p.out_f32 = 1;
-    c.done(udb_ray_embed(&p, st));
+    c.launch([&] { return udb_ray_embed(&p, st); });
   }
 
   // ---- a13: prompt blocks (cross attention to the ray embedding + MLP), fp16 residual out
@@ -273,7 +275,7 @@ static int run(udb_engine* e, const udb_infer_args_t& a, const udb_geometry_t& g
     }
     __half* u = ar.h(px * up_c);
     { Ctx::G q{act, c.H(s + "up_w"), static_cast<int>(px), up_c, cout}; q.bias = c.F(s + "up_b"); q.out = u; c.gemm(q); }
-    if (!c.dry && !c.rc) c.done(udb_upsample2x_nhwc_f16(u, nxt, B, oh, ow, up_c, st));
+    c.launch([&] { return udb_upsample2x_nhwc_f16(u, nxt, B, oh, ow, up_c, st); });
     ar.release(m);
     prev = nxt;
     prev_f32 = 0;
@@ -298,7 +300,7 @@ static int run(udb_engine* e, const udb_infer_args_t& a, const udb_geometry_t& g
   __half* mp = ar.h(static_cast<size_t>(B) * (hh + 2) * (hw + 2) * n_mlp);
   c.conv_transpose(xhat, static_cast<int>(hpx), c_hr, c.H("head_mlp_w"), 1, n_mlp, hh, hw, c.F("head_mlp_b"), nullptr, 0, mp,
                    0, nullptr, 1, 1);
-  if (!c.dry && !c.rc) c.done(udb_reflect_border_fill_nhwc_f16(mp, B, hh, hw, n_mlp, st));
+  c.launch([&] { return udb_reflect_border_fill_nhwc_f16(mp, B, hh, hw, n_mlp, st); });
   float* planes[2];
   for (int i = 0; i < 2; ++i) {
     const std::string hn = idx("heads.%d.", i);
@@ -309,7 +311,7 @@ static int run(udb_engine* e, const udb_infer_args_t& a, const udb_geometry_t& g
     c.conv_halo(mp, B, hh, hw, n_mlp / 2, n_mlp, i * (n_mlp / 2), c.H(hn + "lr_w"), lr_c, c.F(hn + "lr_b"), UDB_ACT_NONE, lr,
                 nullptr, 0.f, 0.f, nullptr);
     __half* up = ar.h(static_cast<size_t>(B) * (nh + 2) * (nw + 2) * lr_c);
-    if (!c.dry && !c.rc) c.done(udb_resize_ac_pad_nhwc_f16(lr, up, B, hh, hw, lr_c, nh, nw, 1, st));
+    c.launch([&] { return udb_resize_ac_pad_nhwc_f16(lr, up, B, hh, hw, lr_c, nh, nw, 1, st); });
     c.conv_halo(up, B, nh, nw, lr_c, lr_c, 0, c.H(hn + "hr_w"), 32, c.F(hn + "hr_b"), UDB_ACT_LEAKY, nullptr,
                 c.F(hn + "head_w"), static_cast<float>(c.S(hn + "head_b")), static_cast<float>(c.S(hn + "add")), planes[i]);
     ar.release(m);
@@ -317,7 +319,7 @@ static int run(udb_engine* e, const udb_infer_args_t& a, const udb_geometry_t& g
 
   stage.next("udb:postprocess");
   // ---- a18: output assembly at the original resolution
-  if (!c.dry && !c.rc) {
+  {
     udb_postprocess_t p;
     memset(&p, 0, sizeof(p));
     p.radius = planes[0]; p.confidence = planes[1]; p.intr4 = ray_intr; p.rays_in = rays_in;
@@ -325,7 +327,7 @@ static int run(udb_engine* e, const udb_infer_args_t& a, const udb_geometry_t& g
     p.H = a.H; p.W = a.W;
     p.out_confidence = a.confidence; p.out_radius = a.radius; p.out_depth = a.depth; p.out_points = a.points; p.out_rays = a.rays;
     p.mode = a.interpolation;
-    c.done(udb_postprocess(&p, st));
+    c.launch([&] { return udb_postprocess(&p, st); });
   }
   if (!c.rc && ar.overflow) { set_error("engine: workspace too small (%zu bytes needed)", ar.peak); return 1; }
   return c.rc;
@@ -344,8 +346,10 @@ static void ray_scale_table(int gh, int gw, int bands, std::vector<float>& out) 
   }
 }
 
+static long long table_key(const udb_geometry_t& g) { return (static_cast<long long>(g.gh) << 32) | static_cast<unsigned>(g.gw); }
+
 static const ShapeTables* prepare(udb_engine* e, const udb_geometry_t& g) {
-  const long long key = (static_cast<long long>(g.gh) << 32) | static_cast<unsigned>(g.gw);
+  const long long key = table_key(g);
   auto it = e->tables.find(key);
   if (it != e->tables.end()) return &it->second;
   auto pw = e->w.find("pos");
@@ -353,7 +357,7 @@ static const ShapeTables* prepare(udb_engine* e, const udb_geometry_t& g) {
   const int D = e->cfg.embed_dim, m = e->cfg.pos_grid, N = g.gh * g.gw;
   ShapeTables tb;
   auto fail = [&tb](const char* why) -> const ShapeTables* {      // nothing half-built stays allocated
-    if (why) set_error("%s", why);
+    if (why) set_error("%s", why);                                 // (null: the failed call has set the error text)
     cudaFree(tb.pos);
     cudaFree(tb.scales);
     return nullptr;
@@ -362,17 +366,34 @@ static const ShapeTables* prepare(udb_engine* e, const udb_geometry_t& g) {
       cudaMalloc(&tb.scales, static_cast<size_t>(e->cfg.hidden / 2) * 4) != cudaSuccess)
     return fail("engine: cudaMalloc of the per-shape tables failed");
   const float* pos = static_cast<const float*>(pw->second.p);
-  cudaMemcpy(tb.pos, pos, static_cast<size_t>(D) * 4, cudaMemcpyDeviceToDevice);   // cls position
+  if (cuda_rc(cudaMemcpy(tb.pos, pos, static_cast<size_t>(D) * 4, cudaMemcpyDeviceToDevice), "engine: copying the cls position"))
+    return fail(nullptr);
   if (g.gh == m && g.gw == m) {
-    cudaMemcpy(tb.pos + D, pos + D, static_cast<size_t>(N) * D * 4, cudaMemcpyDeviceToDevice);
+    if (cuda_rc(cudaMemcpy(tb.pos + D, pos + D, static_cast<size_t>(N) * D * 4, cudaMemcpyDeviceToDevice),
+                "engine: copying the position grid"))
+      return fail(nullptr);
   } else if (udb_posembed_bicubic(pos + D, m, D, tb.pos + D, g.gh, g.gw, nullptr)) {
-    return fail(nullptr);                                          // the operator has set the error text
+    return fail(nullptr);
   }
   std::vector<float> sc;
   ray_scale_table(g.gh, g.gw, e->cfg.hidden / 2, sc);
-  cudaMemcpy(tb.scales, sc.data(), sc.size() * 4, cudaMemcpyHostToDevice);
+  if (cuda_rc(cudaMemcpy(tb.scales, sc.data(), sc.size() * 4, cudaMemcpyHostToDevice), "engine: copying the ray frequencies"))
+    return fail(nullptr);
   if (cudaDeviceSynchronize() != cudaSuccess) return fail("engine: preparing the per-shape tables failed");
   return &(e->tables[key] = tb);
+}
+
+// Workspace bytes of the schedule at this shape, from a dry run of its largest variant (a camera model: its ray buffer sits
+// where camera_k's smaller table would, and it also covers camera_rays); 0 with the error set if the schedule fails.
+static size_t dry_run_bytes(udb_engine* e, int B, int H, int W, int level, const udb_geometry_t& g, const ShapeTables& tb) {
+  udb_infer_args_t a;
+  memset(&a, 0, sizeof(a));
+  a.B = B; a.H = H; a.W = W; a.resolution_level = level;
+  a.camera_model = UDB_CAM_PINHOLE;
+  a.camera_params = reinterpret_cast<const float*>(16);
+  Arena ar(nullptr, 0);
+  if (run(e, a, g, tb, ar, nullptr)) return 0;
+  return ar.peak + 256;
 }
 
 }  // namespace udb
@@ -406,21 +427,11 @@ void udb_destroy(udb_engine* e) {
 }
 
 int udb_set_weight(udb_engine* e, const char* name, const void* dev_ptr, const int64_t* shape, int32_t ndim, int32_t dtype) {
-  if (!e || !name || !dev_ptr || ndim < 0 || ndim > 4) { set_error("udb_set_weight: bad argument"); return 1; }
-  if (reinterpret_cast<uintptr_t>(dev_ptr) & 15) { set_error("udb_set_weight(%s): pointer must be 16-byte aligned", name); return 1; }
-  Weight w;
-  w.p = dev_ptr;
-  w.dtype = dtype;
-  w.ndim = ndim;
-  for (int i = 0; i < ndim; ++i) w.shape[i] = shape[i];
-  e->w[name] = w;
-  return 0;
+  return EngineBase::set_weight(e, "udb_set_weight", name, dev_ptr, shape, ndim, dtype);
 }
 
 int udb_set_scalar(udb_engine* e, const char* name, double value) {
-  if (!e || !name) { set_error("udb_set_scalar: bad argument"); return 1; }
-  e->scalars[name] = value;
-  return 0;
+  return EngineBase::set_scalar(e, "udb_set_scalar", name, value);
 }
 
 int udb_geometry(const udb_engine* e, int32_t H, int32_t W, int32_t level, udb_geometry_t* out) {
@@ -445,15 +456,8 @@ size_t udb_schedule_bytes(udb_engine* e, int32_t B, int32_t H, int32_t W, int32_
   if (!e || B <= 0) { set_error("udb_schedule_bytes: bad argument"); return 0; }
   udb_geometry_t g;
   if (udb_geometry(e, H, W, level, &g)) return 0;
-  udb_infer_args_t a;
-  memset(&a, 0, sizeof(a));
-  a.B = B; a.H = H; a.W = W; a.resolution_level = level;
-  a.camera_model = UDB_CAM_PINHOLE;                  // the largest (camera-model) variant, as udb_workspace_bytes sizes it:
-  a.camera_params = reinterpret_cast<const float*>(16);   // its ray buffer sits where camera_k's (smaller) table would
   const ShapeTables none;                            // a dry run only hands the table pointers on
-  Arena ar(nullptr, 0);
-  if (run(e, a, g, none, ar, nullptr)) return 0;
-  return ar.peak + 256;
+  return dry_run_bytes(e, B, H, W, level, g, none);
 }
 
 size_t udb_workspace_bytes(udb_engine* e, int32_t B, int32_t H, int32_t W, int32_t level) {
@@ -461,17 +465,8 @@ size_t udb_workspace_bytes(udb_engine* e, int32_t B, int32_t H, int32_t W, int32
   if (udb_geometry(e, H, W, level, &g)) return 0;
   const ShapeTables* tb = prepare(e, g);
   if (!tb) return 0;
-  udb_infer_args_t a;
-  memset(&a, 0, sizeof(a));
-  a.B = B; a.H = H; a.W = W; a.resolution_level = level;
-  a.camera_model = UDB_CAM_PINHOLE;                  // sized for the largest (camera-model) variant, which also covers
-  a.camera_params = reinterpret_cast<const float*>(16);   // the camera_k and camera_rays ones
-  Arena ar(nullptr, 0);
-  if (run(e, a, g, *tb, ar, nullptr)) return 0;
-  char key[96];
-  snprintf(key, sizeof(key), "%d,%d,%d,%d", B, H, W, level);
-  e->ws_need[key] = ar.peak + 256;
-  return ar.peak + 256;
+  const size_t n = dry_run_bytes(e, B, H, W, level, g, *tb);
+  return n ? e->prepared(shape_name(B, H, W) + idx(" (level %d)", level), n) : 0;
 }
 
 int udb_infer_v2(udb_engine* e, const udb_infer_args_t* a, void* stream) {
@@ -502,23 +497,15 @@ int udb_infer_v2(udb_engine* e, const udb_infer_args_t* a, void* stream) {
   }
   udb_geometry_t g;
   if (udb_geometry(e, a->H, a->W, a->resolution_level, &g)) return 1;
-  const long long key = (static_cast<long long>(g.gh) << 32) | static_cast<unsigned>(g.gw);
-  auto it = e->tables.find(key);
-  char wkey[96];
-  snprintf(wkey, sizeof(wkey), "%d,%d,%d,%d", a->B, a->H, a->W, a->resolution_level);
-  auto need = e->ws_need.find(wkey);
-  if (it == e->tables.end() || need == e->ws_need.end()) {
-    set_error("udb_infer_v2: shape %dx%dx%d (level %d) not prepared; call udb_workspace_bytes first", a->B, a->H, a->W,
-              a->resolution_level);
-    return 1;
-  }
-  if (a->workspace_bytes < need->second) {   // checked BEFORE anything is launched
-    set_error("udb_infer_v2: workspace too small (%zu bytes given, %zu needed)", a->workspace_bytes, need->second);
+  const std::string shape = shape_name(a->B, a->H, a->W) + idx(" (level %d)", a->resolution_level);
+  if (e->check_workspace("udb_infer_v2", "udb_workspace_bytes", shape, a->workspace, a->workspace_bytes)) return 1;
+  auto tb = e->tables.find(table_key(g));
+  if (tb == e->tables.end()) {
+    set_error("udb_infer_v2: shape %s has no per-shape tables; call udb_workspace_bytes first", shape.c_str());
     return 1;
   }
   Arena ar(a->workspace, a->workspace_bytes);
-  if (reinterpret_cast<uintptr_t>(a->workspace) & 255) { set_error("udb_infer_v2: workspace must be 256-byte aligned"); return 1; }
-  return run(e, *a, g, it->second, ar, stream);
+  return run(e, *a, g, tb->second, ar, stream);
 }
 
 }  // extern "C"

@@ -1,5 +1,6 @@
-// Shared by the whole-path engines (engine.cu: UniDepthV2, engine_v1.cu: UniDepthV1): registered weights, the bump
-// allocator over the caller's workspace, NVTX stage ranges and thin wrappers that fill the operator argument structs.
+// Shared by the whole-path engines (engine.cu: UniDepthV2, engine_v1.cu: UniDepthV1): registered weights and prepared
+// shapes, the bump allocator over the caller's workspace, NVTX stage ranges, the launch gate and thin wrappers that fill
+// the operator argument structs.
 #pragma once
 #include <cuda_fp16.h>
 #include <math.h>
@@ -33,11 +34,53 @@ struct Weight {
   int64_t shape[4] = {0, 0, 0, 0};
 };
 
-// registered operands / scalars: the part of an engine the schedule helpers (Ctx) need
+// Registered operands / scalars (what the schedule helpers, Ctx, read) and the prepared shapes of an engine.  `fn` is the
+// calling entry point's name, the prefix of every error message.
 struct EngineBase {
   std::unordered_map<std::string, Weight> w;
   std::unordered_map<std::string, double> scalars;
+  std::unordered_map<std::string, size_t> ws_need;   // prepared shape (as the messages print it) -> workspace bytes
+
+  static int set_weight(EngineBase* e, const char* fn, const char* name, const void* dev_ptr, const int64_t* shape,
+                        int32_t ndim, int32_t dtype) {
+    if (!e || !name || !dev_ptr || ndim < 0 || ndim > 4) { set_error("%s: bad argument", fn); return 1; }
+    if (reinterpret_cast<uintptr_t>(dev_ptr) & 15) { set_error("%s(%s): pointer must be 16-byte aligned", fn, name); return 1; }
+    Weight x;
+    x.p = dev_ptr; x.dtype = dtype; x.ndim = ndim;
+    for (int i = 0; i < ndim; ++i) x.shape[i] = shape[i];
+    e->w[name] = x;
+    return 0;
+  }
+  static int set_scalar(EngineBase* e, const char* fn, const char* name, double value) {
+    if (!e || !name) { set_error("%s: bad argument", fn); return 1; }
+    e->scalars[name] = value;
+    return 0;
+  }
+  // the sizing entry point records the workspace a shape needs; only a recorded shape may be launched, and the size and
+  // alignment of the caller's workspace are checked before anything is enqueued
+  size_t prepared(const std::string& shape, size_t bytes) { return ws_need[shape] = bytes; }
+  int check_workspace(const char* fn, const char* sizing_fn, const std::string& shape, const void* ws, size_t bytes) const {
+    auto need = ws_need.find(shape);
+    if (need == ws_need.end()) { set_error("%s: shape %s not prepared; call %s first", fn, shape.c_str(), sizing_fn); return 1; }
+    if (bytes < need->second) {
+      set_error("%s: workspace too small (%zu bytes given, %zu needed)", fn, bytes, need->second);
+      return 1;
+    }
+    if (reinterpret_cast<uintptr_t>(ws) & 255) { set_error("%s: workspace must be 256-byte aligned", fn); return 1; }
+    return 0;
+  }
 };
+
+// Python's v // 2 (the reference's padding arithmetic)
+static inline int floordiv2(int v) { return v >= 0 ? v / 2 : -((-v + 1) / 2); }
+
+// result of a CUDA runtime call the engine makes itself (not through an operator) as the engine's return code; the error
+// text is `what` + `name` + the CUDA error
+static inline int cuda_rc(cudaError_t err, const char* what, const std::string& name = "") {
+  if (err == cudaSuccess) return 0;
+  set_error("%s%s: %s", what, name.c_str(), cudaGetErrorString(err));
+  return 1;
+}
 
 // ------------------------------------------------------------------------------------------ arena
 struct Arena {
@@ -89,7 +132,14 @@ struct Ctx {
     }
     return it->second;
   }
-  void done(int r) { if (r && !rc) rc = r; }
+  // The one launch gate: every operator or CUDA call of a schedule is enqueued through here.  A dry run (which only sizes
+  // the workspace) and a run that has already failed enqueue nothing; otherwise a non-zero result of the call (an error
+  // whose text it has set) is kept.  Operands are looked up before the gate, so that a dry run names a missing one.
+  template <class Call>
+  void launch(Call&& call) {
+    if (dry || rc) return;
+    if (const int r = call()) rc = r;
+  }
   // registered 2-D operand must have exactly this shape (a mis-packed weight would otherwise be read with the
   // wrong leading dimension and silently produce garbage)
   void expect2(const std::string& name, int64_t rows, int64_t cols) {
@@ -113,7 +163,6 @@ struct Ctx {
     int ln_parts = 0, ln_part_cols = 0; float ln_eps = 0.f;
   };
   void gemm(const G& q) {
-    if (dry || rc) return;
     udb_gemm_t g;
     memset(&g, 0, sizeof(g));
     g.a = q.a; g.w = q.w; g.M = q.M; g.N = q.N; g.K = q.K;
@@ -129,12 +178,11 @@ struct Ctx {
     g.a_split_k = q.a_split_k; g.out_split = q.out_split;
     g.ln_stats_out = q.ln_stats_out; g.ln_stats_in = q.ln_stats_in; g.ln_c1 = q.ln_c1;
     g.ln_parts = q.ln_parts; g.ln_part_cols = q.ln_part_cols; g.ln_eps = q.ln_eps;
-    done(udb_gemm_f16(&g, st));
+    launch([&] { return udb_gemm_f16(&g, st); });
   }
   // ConvTranspose2d with kernel == stride == k as a GEMM with a pixel-shuffle store (ops.conv_transpose_ks)
   void conv_transpose(const void* x, int M, int K, const void* w, int k, int cout, int h, int ww, const float* bias,
                       const void* resid, int resid_f32, void* out, int out_f32, void* out2, int out2_leaky, int pad) {
-    if (dry || rc) return;
     udb_gemm_t g;
     memset(&g, 0, sizeof(g));
     g.a = x; g.w = w; g.M = M; g.N = k * k * cout; g.K = K; g.lda = K; g.ldw = K;
@@ -143,12 +191,11 @@ struct Ctx {
     g.out = out; g.out_f32 = out_f32; g.ldc = cout; g.out2 = out2; g.out2_leaky = out2_leaky;
     g.store_mode = UDB_STORE_CONVT;
     g.ct_k = k; g.ct_cout = cout; g.ct_h = h; g.ct_w = ww; g.ct_pad = pad;
-    done(udb_gemm_f16(&g, st));
+    launch([&] { return udb_gemm_f16(&g, st); });
   }
   // 3x3 zero-padded convolution over NHWC f16 (ops.conv3x3, tile 8x16)
   void conv3x3(const void* x, int B, int H, int Wd, int C, const void* w, int N, const float* bias, int act,
                const float* gamma, const void* resid, int resid_f32, void* out, int out_f32, void* out2, int out2_leaky) {
-    if (dry || rc) return;
     udb_gemm_t g;
     memset(&g, 0, sizeof(g));
     g.a = x; g.w = w; g.M = B * H * Wd; g.N = N; g.K = 9 * C; g.lda = C; g.ldw = 9 * C;
@@ -159,33 +206,30 @@ struct Ctx {
     g.out = out; g.out_f32 = out_f32; g.ldc = N;
     g.resid = resid; g.resid_f32 = resid_f32; g.ldr = resid ? N : 0;
     g.out2 = out2; g.out2_leaky = out2_leaky;
-    done(udb_gemm_f16(&g, st));
+    launch([&] { return udb_gemm_f16(&g, st); });
   }
   void conv_halo(const void* x, int B, int H, int Wd, int C, int cstride, int coff, const void* w, int cout,
                  const float* bias, int act, void* out, const float* head_w, float head_b, float head_add, float* head_out) {
-    if (dry || rc) return;
     udb_conv_halo_t c;
     memset(&c, 0, sizeof(c));
     c.x = x; c.w = w; c.bias = bias; c.B = B; c.H = H; c.W = Wd; c.C = C; c.cstride = cstride; c.coff = coff;
     c.cout = cout; c.act = act; c.out = out; c.ldc = cout;
     c.head_w = head_w; c.head_b = head_b; c.head_add = head_add; c.head_out = head_out;
-    done(udb_conv3x3_halo_f16(&c, st));
+    launch([&] { return udb_conv3x3_halo_f16(&c, st); });
   }
   void attention(const void* q, const void* k, const void* v, void* out, int B, int heads, int sq, int sk, int ldq,
                  int ldk, int ldv, int ldo, int q0, int k0, int v0, float scale, int lo_in = 0, int lo_out = 0) {
-    if (dry || rc) return;
     udb_attn_t a;
     memset(&a, 0, sizeof(a));
     a.q = q; a.k = k; a.v = v; a.out = out; a.B = B; a.heads = heads; a.seq_q = sq; a.seq_k = sk; a.head_dim = 64;
     a.ldq = ldq; a.ldk = ldk; a.ldv = ldv; a.ldo = ldo; a.q_col0 = q0; a.k_col0 = k0; a.v_col0 = v0; a.o_col0 = 0;
     a.scale = scale;
     if (lo_in) { a.split = 1; a.lo_off_q = a.lo_off_k = a.lo_off_v = lo_in; a.lo_off_o = lo_out; }
-    done(udb_attention_f16(&a, st));
+    launch([&] { return udb_attention_f16(&a, st); });
   }
   void layernorm(const void* in, int in_f32, void* out, int out_f32, const float* w, const float* b, int rows, int dim,
                  float eps, int rows_per_group = 0, int group_stride = 0, int row_offset = 0, int dim_valid = 0,
                  int out_split = 0) {
-    if (dry || rc) return;
     udb_layernorm_t p;
     memset(&p, 0, sizeof(p));
     p.in = in; p.in_f32 = in_f32; p.out = out; p.out_f32 = out_f32; p.weight = w; p.bias = b;
@@ -193,16 +237,26 @@ struct Ctx {
     p.rows_per_group = rows_per_group; p.group_stride = group_stride; p.row_offset = row_offset; p.eps = eps;
     p.dim_valid = dim_valid;
     p.out_split = out_split;
-    done(udb_layernorm(&p, st));
+    launch([&] { return udb_layernorm(&p, st); });
+  }
+  // LayerNorm for any width that is a multiple of 64, with the optional added term and space-to-depth store (UniDepthV1)
+  void ln_any(const void* in, int in_f32, void* out, int out_f32, const float* w, const float* b, long long rows, int dim,
+              float eps, long long ld_out = 0, const float* add = nullptr, long long add_mod = 0, int s2d_h = 0,
+              int s2d_w = 0) {
+    udb_layernorm_any_t p;
+    memset(&p, 0, sizeof(p));
+    p.in = in; p.in_f32 = in_f32; p.out = out; p.out_f32 = out_f32; p.weight = w; p.bias = b;
+    p.rows = rows; p.dim = dim; p.ld_in = dim; p.ld_out = ld_out ? ld_out : dim; p.eps = eps;
+    p.add = add; p.add_mod = add_mod; p.s2d_h = s2d_h; p.s2d_w = s2d_w;
+    launch([&] { return udb_layernorm_any(&p, st); });
   }
   void small_linear(const float* x, int M, int K, const float* w, int N, const float* bias, int act, const float* gamma,
                     const float* resid, float* y, int ldx = 0, int ldy = 0, int ldr = 0) {
-    if (dry || rc) return;
     udb_small_linear_t p;
     memset(&p, 0, sizeof(p));
     p.x = x; p.w = w; p.bias = bias; p.gamma = gamma; p.resid = resid; p.y = y; p.M = M; p.N = N; p.K = K; p.act = act;
     p.ldx = ldx ? ldx : K; p.ldy = ldy ? ldy : N; p.ldr = resid ? (ldr ? ldr : N) : 0;
-    done(udb_small_linear_f32(&p, st));
+    launch([&] { return udb_small_linear_f32(&p, st); });
   }
 };
 
@@ -226,6 +280,12 @@ static inline std::string idx(const char* fmt, int i) {
 static inline std::string idx2(const char* fmt, int i, int j) {
   char b[64];
   snprintf(b, sizeof(b), fmt, i, j);
+  return b;
+}
+// a batch shape B x H x W as the prepared-shape table stores it and the error messages print it
+static inline std::string shape_name(int B, int H, int W) {
+  char b[64];
+  snprintf(b, sizeof(b), "%dx%dx%d", B, H, W);
   return b;
 }
 

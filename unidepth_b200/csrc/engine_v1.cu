@@ -7,13 +7,10 @@
 //     pixel_encoder = ConvNeXt       unidepth/models/backbones/convnext.py:459-471 (stem :371-383, stage :289-298, block :208-223)
 //     pixel_decoder = Decoder        unidepth/models/unidepthv1/decoder.py:364-463 (run_camera :311-343, CameraHead :85-106,
 //                                    DepthHead :195-300), layers/{attention,nystrom_attention,mlp,upsample,convnext}.py
-#include <stdlib.h>
-
 #include "engine_common.h"
 
 struct udb_engine_v1 : udb::EngineBase {
   udb_v1_config_t cfg;
-  std::unordered_map<std::string, size_t> ws_need;   // "B,H,W" -> bytes
 };
 
 namespace udb {
@@ -32,78 +29,70 @@ static V1Geom v1_geometry(int H, int W, int net_h, int net_w) {
   g.rh = static_cast<int>(ceil(H * g.ratio - 0.5));
   g.rw = static_cast<int>(ceil(W * g.ratio - 0.5));
   const int dh = net_h - g.rh, dw = net_w - g.rw;
-  const auto fdiv2 = [](int v) { return v >= 0 ? v / 2 : -((-v + 1) / 2); };
-  g.pad_t = fdiv2(dh); g.pad_b = dh - g.pad_t;
-  g.pad_l = fdiv2(dw); g.pad_r = dw - g.pad_l;
+  g.pad_t = floordiv2(dh); g.pad_b = dh - g.pad_t;
+  g.pad_l = floordiv2(dw); g.pad_r = dw - g.pad_l;
   return g;
 }
 
-struct V1Ctx : Ctx {
-  // Debug taps: with UDB_V1_DUMP=<dir> set (and the call NOT under stream capture) named intermediates are written as raw
-  // files <dir>/<name>.bin after a stream sync; tests/tools compare them with the oracle's taps.  Off in normal operation.
-  void tap(const char* name, const void* p, size_t bytes) {
-    static const char* dir = getenv("UDB_V1_DUMP");
-    if (!dir || dry || rc) return;
-    cudaStreamSynchronize(static_cast<cudaStream_t>(st));
-    std::vector<char> host(bytes);
-    if (cudaMemcpy(host.data(), p, bytes, cudaMemcpyDeviceToHost) != cudaSuccess) return;
-    const std::string path = std::string(dir) + "/" + name + ".bin";
-    if (FILE* f = fopen(path.c_str(), "wb")) { fwrite(host.data(), 1, bytes, f); fclose(f); }
-  }
-  void ln_any(const void* in, int in_f32, void* out, int out_f32, const float* w, const float* b, long long rows, int dim, float eps,
-              long long ld_out = 0, const float* add = nullptr, long long add_mod = 0, int s2d_h = 0, int s2d_w = 0) {
-    if (dry || rc) return;
-    udb_layernorm_any_t p;
-    memset(&p, 0, sizeof(p));
-    p.in = in; p.in_f32 = in_f32; p.out = out; p.out_f32 = out_f32; p.weight = w; p.bias = b;
-    p.rows = rows; p.dim = dim; p.ld_in = dim; p.ld_out = ld_out ? ld_out : dim; p.eps = eps;
-    p.add = add; p.add_mod = add_mod; p.s2d_h = s2d_h; p.s2d_w = s2d_w;
-    done(udb_layernorm_any(&p, st));
-  }
-  // LayerNorm to f16 for any decoder / encoder width: the V2 kernels where they apply (128-multiples up to 1024 from f32,
-  // 64/128/256 from f16), the generic one otherwise
-  void ln16(const void* in, int in_f32, void* out, const std::string& wn, const std::string& bn, long long rows, int dim, float eps) {
-    const bool v2_ok = in_f32 ? (dim % 128 == 0 && dim <= 1024) : (dim == 64 || dim == 128 || dim == 256 || (dim % 128 == 0 && dim <= 1024));
-    if (v2_ok) layernorm(in, in_f32, out, 0, F(wn), F(bn), static_cast<int>(rows), dim, eps);
-    else ln_any(in, in_f32, out, 0, F(wn), F(bn), rows, dim, eps);
-  }
-  // MLP tail on the f32 residual stream x [rows, C]:  x += gamma * (W2 gelu(W1 LN(x) + b1) + b2)        (layers/mlp.py:9-35)
-  void mlp_resid(const std::string& p, float* x, long long rows, int C, int mid, const float* gamma, __half* x16 = nullptr) {
-    const size_t m = ar->mark();
-    __half* hN = ar->h(rows * C);
-    __half* md = ar->h(rows * mid);
-    ln16(x, 1, hN, p + "nw", p + "nb", rows, C, 1e-5f);
-    { G q{hN, H(p + "w1"), static_cast<int>(rows), mid, C}; q.bias = F(p + "b1"); q.act = UDB_ACT_GELU; q.out = md; gemm(q); }
-    { G q{md, H(p + "w2"), static_cast<int>(rows), C, mid}; q.bias = F(p + "b2"); q.gamma = gamma; q.resid = x; q.resid_f32 = 1;
-      q.out = x; q.out_f32 = 1; q.out2 = x16; q.out2_leaky = 0; gemm(q); }
-    ar->release(m);
-  }
-  // ConvNeXt-style block on an NHWC map: x f32 (+ its f16 copy x16) [B,H,W,C] updated in place
-  // (convnext.py:208-223 with eps 1e-6; layers/convnext.py:34-44 with eps 1e-5)
-  void cvnxt_block(const std::string& p, float* x, __half* x16, int B, int Hh, int Ww, int C, float eps) {
-    const size_t m = ar->mark();
-    const long long rows = static_cast<long long>(B) * Hh * Ww;
-    __half* y = ar->h(rows * C);
-    __half* hN = ar->h(rows * C);
-    __half* md = ar->h(rows * 4 * C);
-    if (!dry && !rc) done(udb_dwconv7_nhwc_f16(x16, F(p + "dw_w"), F(p + "dw_b"), y, B, Hh, Ww, C, st));
-    ln16(y, 0, hN, p + "ln_w", p + "ln_b", rows, C, eps);
-    { G q{hN, H(p + "w1"), static_cast<int>(rows), 4 * C, C}; q.bias = F(p + "b1"); q.act = UDB_ACT_GELU; q.out = md; gemm(q); }
-    { G q{md, H(p + "w2"), static_cast<int>(rows), C, 4 * C}; q.bias = F(p + "b2"); q.gamma = F(p + "gamma"); q.resid = x; q.resid_f32 = 1;
-      q.out = x; q.out_f32 = 1; q.out2 = x16; q.out2_leaky = 0; gemm(q); }
-    ar->release(m);
-  }
-  void attention_sp(const void* q, const void* k, const void* v, void* out, int B, int heads, int sq, int sk, int ldq, int ldk, int ldv, int ldo,
-                    int q0, int k0, int v0) {
-    attention(q, k, v, out, B, heads, sq, sk, ldq, ldk, ldv, ldo, q0, k0, v0, 0.125f);
-  }
-};
+// LayerNorm to f16 for any decoder / encoder width: the V2 kernels where they apply (128-multiples up to 1024 from f32,
+// 64/128/256 from f16), the generic one otherwise
+static void ln16(Ctx& c, const void* in, int in_f32, void* out, const std::string& wn, const std::string& bn, long long rows,
+                 int dim, float eps) {
+  const bool v2_ok = in_f32 ? (dim % 128 == 0 && dim <= 1024) : (dim == 64 || dim == 128 || dim == 256 || (dim % 128 == 0 && dim <= 1024));
+  if (v2_ok) c.layernorm(in, in_f32, out, 0, c.F(wn), c.F(bn), static_cast<int>(rows), dim, eps);
+  else c.ln_any(in, in_f32, out, 0, c.F(wn), c.F(bn), rows, dim, eps);
+}
+
+// MLP tail on the f32 residual stream x [rows, C]:  x += gamma * (W2 gelu(W1 LN(x) + b1) + b2)        (layers/mlp.py:9-35)
+static void mlp_resid(Ctx& c, const std::string& p, float* x, long long rows, int C, int mid, const float* gamma,
+                      __half* x16 = nullptr) {
+  Arena& ar = *c.ar;
+  const size_t m = ar.mark();
+  __half* hN = ar.h(rows * C);
+  __half* md = ar.h(rows * mid);
+  ln16(c, x, 1, hN, p + "nw", p + "nb", rows, C, 1e-5f);
+  { Ctx::G q{hN, c.H(p + "w1"), static_cast<int>(rows), mid, C}; q.bias = c.F(p + "b1"); q.act = UDB_ACT_GELU; q.out = md; c.gemm(q); }
+  { Ctx::G q{md, c.H(p + "w2"), static_cast<int>(rows), C, mid}; q.bias = c.F(p + "b2"); q.gamma = gamma; q.resid = x; q.resid_f32 = 1;
+    q.out = x; q.out_f32 = 1; q.out2 = x16; q.out2_leaky = 0; c.gemm(q); }
+  ar.release(m);
+}
+
+// ConvNeXt-style block on an NHWC map: x f32 (+ its f16 copy x16) [B,H,W,C] updated in place
+// (convnext.py:208-223 with eps 1e-6; layers/convnext.py:34-44 with eps 1e-5)
+static void cvnxt_block(Ctx& c, const std::string& p, float* x, __half* x16, int B, int Hh, int Ww, int C, float eps) {
+  Arena& ar = *c.ar;
+  const size_t m = ar.mark();
+  const long long rows = static_cast<long long>(B) * Hh * Ww;
+  __half* y = ar.h(rows * C);
+  __half* hN = ar.h(rows * C);
+  __half* md = ar.h(rows * 4 * C);
+  const float* dw_w = c.F(p + "dw_w");
+  const float* dw_b = c.F(p + "dw_b");
+  c.launch([&] { return udb_dwconv7_nhwc_f16(x16, dw_w, dw_b, y, B, Hh, Ww, C, c.st); });
+  ln16(c, y, 0, hN, p + "ln_w", p + "ln_b", rows, C, eps);
+  { Ctx::G q{hN, c.H(p + "w1"), static_cast<int>(rows), 4 * C, C}; q.bias = c.F(p + "b1"); q.act = UDB_ACT_GELU; q.out = md; c.gemm(q); }
+  { Ctx::G q{md, c.H(p + "w2"), static_cast<int>(rows), C, 4 * C}; q.bias = c.F(p + "b2"); q.gamma = c.F(p + "gamma"); q.resid = x;
+    q.resid_f32 = 1; q.out = x; q.out_f32 = 1; q.out2 = x16; q.out2_leaky = 0; c.gemm(q); }
+  ar.release(m);
+}
+
+// pre-processing of the input batch into the encoder's patch rows (unidepthv1.py _preprocess): 4x4 im2col rows of the
+// ConvNeXt stem (`patch` 0) or 14x14 DINOv2 patch rows (`patch` 14)
+static void preprocess(Ctx& c, const udb_v1_config_t& cf, const udb_infer_v1_args_t& a, const V1Geom& g, __half* patches,
+                       int patch) {
+  udb_v1_preprocess_t p;
+  memset(&p, 0, sizeof(p));
+  p.rgb = a.rgb; p.rgb_is_u8 = a.rgb_is_u8; p.scale255 = a.scale255; p.normalize = a.normalize; p.B = a.B; p.H = a.H; p.W = a.W;
+  p.rh = g.rh; p.rw = g.rw; p.pad_l = g.pad_l; p.pad_t = g.pad_t; p.net_h = cf.net_h; p.net_w = cf.net_w; p.patches = patches;
+  p.patch = patch;
+  c.launch([&] { return udb_v1_preprocess(&p, c.st); });
+}
 
 static inline long long rup(long long v, long long m) { return (v + m - 1) / m * m; }
 
 // Single-head (head dim = D) attention block with a separate context (decoder.py:225-236 aggregate_16 / prompt_camera),
 // computed densely: S = q k^T (GEMM) -> row softmax -> P v (GEMM with v^T as the K-major operand).
-static void dense_attn_block(V1Ctx& c, const std::string& p, float* x, int B, int nq, int D, const void* ctx, int ctx_f32, int nk,
+static void dense_attn_block(Ctx& c, const std::string& p, float* x, int B, int nq, int D, const void* ctx, int ctx_f32, int nk,
                              const float* pos_ctx) {
   Arena& ar = *c.ar;
   const size_t m = ar.mark();
@@ -111,13 +100,19 @@ static void dense_attn_block(V1Ctx& c, const std::string& p, float* x, int B, in
   const int kp = static_cast<int>(rup(nk, 64));
   __half* xn = ar.h(Rq * D);
   __half* cn = ar.h((Rk + 64) * D);
-  c.ln16(x, 1, xn, p + "nxw", p + "nxb", Rq, D, 1e-5f);
-  c.ln16(ctx, ctx_f32, cn, p + "ncw", p + "ncb", Rk, D, 1e-5f);
-  if (!c.dry && !c.rc) cudaMemsetAsync(cn + Rk * D, 0, sizeof(__half) * 64 * D, static_cast<cudaStream_t>(c.st));
+  ln16(c, x, 1, xn, p + "nxw", p + "nxb", Rq, D, 1e-5f);
+  ln16(c, ctx, ctx_f32, cn, p + "ncw", p + "ncb", Rk, D, 1e-5f);
+  c.launch([&] {
+    return cuda_rc(cudaMemsetAsync(cn + Rk * D, 0, sizeof(__half) * 64 * D, static_cast<cudaStream_t>(c.st)),
+                   "engine_v1: zeroing the padding rows of the normalised context of ", p);
+  });
   __half* q = ar.h(Rq * D);
   { Ctx::G g{xn, c.H(p + "q_w"), static_cast<int>(Rq), D, D}; g.bias = c.F(p + "q_b"); g.out = q; c.gemm(g); }
   __half* k = ar.h(static_cast<long long>(B) * kp * D);
-  if (!c.dry && !c.rc) cudaMemsetAsync(k, 0, sizeof(__half) * B * kp * D, static_cast<cudaStream_t>(c.st));
+  c.launch([&] {
+    return cuda_rc(cudaMemsetAsync(k, 0, sizeof(__half) * B * kp * D, static_cast<cudaStream_t>(c.st)),
+                   "engine_v1: zeroing the padded keys of ", p);
+  });
   { Ctx::G g{cn, c.H(p + "k_w"), static_cast<int>(Rk), D, D}; g.bias = c.F(p + "k_b"); g.out = k;
     g.rows_per_group = nk; g.group_stride = kp; g.row_offset = 0;
     if (pos_ctx) { g.resid = pos_ctx; g.resid_f32 = 1; g.ldr = D; g.resid_mod = nk; g.resid_row_offset = 0; }
@@ -131,32 +126,32 @@ static void dense_attn_block(V1Ctx& c, const std::string& p, float* x, int B, in
     // v^T [D, kp] = W_v . ctx_b^T  (the value bias is added after P v: softmax rows sum to 1)
     { Ctx::G g{c.H(p + "v_w"), cn + static_cast<long long>(b) * nk * D, D, kp, D}; g.out = vt + static_cast<long long>(b) * D * kp; c.gemm(g); }
     { Ctx::G g{q + static_cast<long long>(b) * nq * D, k + static_cast<long long>(b) * kp * D, nq, kp, D}; g.out = S; g.out_f32 = 1; c.gemm(g); }
-    if (!c.dry && !c.rc) c.done(udb_softmax_rows(S, P, nq, nk, kp, kp, scale, c.st));
+    c.launch([&] { return udb_softmax_rows(S, P, nq, nk, kp, kp, scale, c.st); });
     { Ctx::G g{P, vt + static_cast<long long>(b) * D * kp, nq, D, kp}; g.bias = c.F(p + "v_b"); g.out = o + static_cast<long long>(b) * nq * D; c.gemm(g); }
   }
   { Ctx::G g{o, c.H(p + "out_w"), static_cast<int>(Rq), D, D}; g.bias = c.F(p + "out_b"); g.gamma = c.F(p + "ls1"); g.resid = x; g.resid_f32 = 1;
     g.out = x; g.out_f32 = 1; c.gemm(g); }
   ar.release(m);
-  c.mlp_resid(p + "m", x, Rq, D, 4 * D, c.F(p + "ls2"));
+  mlp_resid(c, p + "m", x, Rq, D, 4 * D, c.F(p + "ls2"));
 }
 
 // Multi-head self-attention block with 64-wide heads and a positional term added to q (decoder.py:239-241,256-258,271-273):
 // exact attention (AttentionBlock) or the Nystrom approximation with 128 landmarks (NystromBlock).
-static void mh_attn_block(V1Ctx& c, const std::string& p, float* x, int B, int n, int C, int heads, const float* pos, bool nystrom) {
+static void mh_attn_block(Ctx& c, const std::string& p, float* x, int B, int n, int C, int heads, const float* pos, bool nystrom) {
   Arena& ar = *c.ar;
   const size_t m = ar.mark();
   const long long R = static_cast<long long>(B) * n;
   __half* xn = ar.h(R * C);
   __half* cn = ar.h(R * C);
-  c.ln16(x, 1, xn, p + "nxw", p + "nxb", R, C, 1e-5f);
-  c.ln16(x, 1, cn, p + "ncw", p + "ncb", R, C, 1e-5f);
+  ln16(c, x, 1, xn, p + "nxw", p + "nxb", R, C, 1e-5f);
+  ln16(c, x, 1, cn, p + "ncw", p + "ncb", R, C, 1e-5f);
   __half* q = ar.h(R * C);
   { Ctx::G g{xn, c.H(p + "q_w"), static_cast<int>(R), C, C}; g.bias = c.F(p + "q_b"); g.resid = pos; g.resid_f32 = 1; g.out = q; c.gemm(g); }
   __half* kv = ar.h(R * 2 * C);
   { Ctx::G g{cn, c.H(p + "kv_w"), static_cast<int>(R), 2 * C, C}; g.bias = c.F(p + "kv_b"); g.out = kv; c.gemm(g); }
   __half* o = ar.h(R * C);
   if (!nystrom) {
-    c.attention_sp(q, kv, kv, o, B, heads, n, n, C, 2 * C, 2 * C, C, 0, 0, C);
+    c.attention(q, kv, kv, o, B, heads, n, n, C, 2 * C, 2 * C, C, 0, 0, C, 0.125f);
   } else {
     const long long L = static_cast<long long>(B) * 128, mm = static_cast<long long>(B) * heads * 128 * 128;
     __half* lm = ar.h(L * 2 * C);          // (q landmarks | k landmarks)
@@ -165,34 +160,34 @@ static void mh_attn_block(V1Ctx& c, const std::string& p, float* x, int B, int n
     float* tmp = ar.f(3 * mm);
     __half* k3 = ar.h(L * C);
     __half* w2 = ar.h(L * C);
-    if (!c.dry && !c.rc) c.done(udb_nystrom_landmarks(q, C, kv, 2 * C, lm, B, n, heads, c.st));
-    if (!c.dry && !c.rc) c.done(udb_nystrom_k2_pinv(lm, k2, z, tmp, B, heads, 6, c.st));
-    c.attention_sp(lm, kv, kv, k3, B, heads, 128, n, 2 * C, 2 * C, 2 * C, C, 0, 0, C);        // softmax(ql k^T) v
-    if (!c.dry && !c.rc) c.done(udb_nystrom_zk3(z, k3, C, w2, C, B, heads, c.st));             // pinv . kernel_3
-    c.attention_sp(q, lm, w2, o, B, heads, n, 128, C, 2 * C, C, C, 0, C, 0);                  // softmax(q kl^T) (pinv kernel_3)
+    c.launch([&] { return udb_nystrom_landmarks(q, C, kv, 2 * C, lm, B, n, heads, c.st); });
+    c.launch([&] { return udb_nystrom_k2_pinv(lm, k2, z, tmp, B, heads, 6, c.st); });
+    c.attention(lm, kv, kv, k3, B, heads, 128, n, 2 * C, 2 * C, 2 * C, C, 0, 0, C, 0.125f);        // softmax(ql k^T) v
+    c.launch([&] { return udb_nystrom_zk3(z, k3, C, w2, C, B, heads, c.st); });           // pinv . kernel_3
+    c.attention(q, lm, w2, o, B, heads, n, 128, C, 2 * C, C, C, 0, C, 0, 0.125f);                  // softmax(q kl^T) (pinv kernel_3)
   }
   { Ctx::G g{o, c.H(p + "out_w"), static_cast<int>(R), C, C}; g.bias = c.F(p + "out_b"); g.gamma = c.F(p + "ls1"); g.resid = x; g.resid_f32 = 1;
     g.out = x; g.out_f32 = 1; c.gemm(g); }
   ar.release(m);
-  c.mlp_resid(p + "m", x, R, C, 4 * C, c.F(p + "ls2"));
+  mlp_resid(c, p + "m", x, R, C, 4 * C, c.F(p + "ls2"));
 }
 
 // ConvUpsample (layers/upsample.py:13-45): (lat + emb) -> 2 CvnxtBlocks -> conv1x1 C->C/2 -> x2 bilinear (align_corners=True)
 // -> conv3x3 (zero pad).  Returns the next level's f32 tokens and their f16 copy (allocated before the scratch mark).
-static void conv_upsample(V1Ctx& c, const std::string& p, const float* lat, const float* emb, int B, int h, int w, int C, float* next,
+static void conv_upsample(Ctx& c, const std::string& p, const float* lat, const float* emb, int B, int h, int w, int C, float* next,
                           __half* next16) {
   Arena& ar = *c.ar;
   const size_t m = ar.mark();
   const long long R = static_cast<long long>(B) * h * w;
   float* xs = ar.f(R * C);
   __half* xs16 = ar.h(R * C);
-  if (!c.dry && !c.rc) c.done(udb_add_f32(lat, emb, xs, xs16, R * C, c.st));
-  for (int j = 0; j < 2; ++j) c.cvnxt_block(p + (j ? "c1." : "c0."), xs, xs16, B, h, w, C, 1e-5f);
+  c.launch([&] { return udb_add_f32(lat, emb, xs, xs16, R * C, c.st); });
+  for (int j = 0; j < 2; ++j) cvnxt_block(c, p + (j ? "c1." : "c0."), xs, xs16, B, h, w, C, 1e-5f);
   const int C2 = C / 2;
   __half* u = ar.h(R * C2);
   { Ctx::G g{xs16, c.H(p + "up_w"), static_cast<int>(R), C2, C}; g.bias = c.F(p + "up_b"); g.out = u; c.gemm(g); }
   __half* up = ar.h(R * 4 * C2);
-  if (!c.dry && !c.rc) c.done(udb_resize_ac_pad_nhwc_f16(u, up, B, h, w, C2, 2 * h, 2 * w, 0, c.st));
+  c.launch([&] { return udb_resize_ac_pad_nhwc_f16(u, up, B, h, w, C2, 2 * h, 2 * w, 0, c.st); });
   c.expect2(p + "conv_w", C2, 9 * C2);
   c.conv3x3(up, B, 2 * h, 2 * w, C2, c.H(p + "conv_w"), C2, c.F(p + "conv_b"), UDB_ACT_NONE, nullptr, nullptr, 0, next, 1, next16, 0);
   ar.release(m);
@@ -203,7 +198,7 @@ static void conv_upsample(V1Ctx& c, const std::string& p, const float* lat, cons
 // bicubic resize of the 37x37 grid) as row-mapped residual -> cls rows -> the shared block loop.  After every block the
 // tap kernel folds (patch tokens + cls token) into the running max of its slice (levels[s], decoder.py:371-379; slice s
 // holds cf.depths[s] blocks) and copies the raw cls rows of the last four blocks into clsbuf[k] (block last - k).
-static void dino_encoder(V1Ctx& c, const udb_v1_config_t& cf, const udb_infer_v1_args_t& a, const V1Geom& g, int gh, int gw,
+static void dino_encoder(Ctx& c, const udb_v1_config_t& cf, const udb_infer_v1_args_t& a, const V1Geom& g, int gh, int gw,
                          __half* const* levels, float* const* clsbuf) {
   Arena& ar = *c.ar;
   const int B = a.B, D = cf.dims[0], N = gh * gw, T = N + 1;
@@ -212,14 +207,7 @@ static void dino_encoder(V1Ctx& c, const udb_v1_config_t& cf, const udb_infer_v1
   for (int i = 0; i < 4; ++i) depth += cf.depths[i];
   const size_t m = ar.mark();
   __half* patches = ar.h(BN * 640);
-  if (!c.dry) {
-    udb_v1_preprocess_t p;
-    memset(&p, 0, sizeof(p));
-    p.rgb = a.rgb; p.rgb_is_u8 = a.rgb_is_u8; p.scale255 = a.scale255; p.normalize = a.normalize; p.B = B; p.H = a.H; p.W = a.W;
-    p.rh = g.rh; p.rw = g.rw; p.pad_l = g.pad_l; p.pad_t = g.pad_t; p.net_h = cf.net_h; p.net_w = cf.net_w; p.patches = patches;
-    p.patch = 14;
-    c.done(udb_v1_preprocess(&p, c.st));
-  }
+  preprocess(c, cf, a, g, patches, 14);
   float* x = ar.f(BT * D);           // fp32 residual stream [B, 1 + N, D]
   {
     c.expect2("patch_w", D, 640);
@@ -230,25 +218,21 @@ static void dino_encoder(V1Ctx& c, const udb_v1_config_t& cf, const udb_infer_v1
     q.bias = c.F("patch_b"); q.resid = pos; q.resid_f32 = 1; q.ldr = D; q.out = x; q.out_f32 = 1;
     q.rows_per_group = N; q.group_stride = T; q.row_offset = 1; q.resid_mod = N; q.resid_row_offset = 1;
     c.gemm(q);
-    if (!c.dry && !c.rc) c.done(udb_set_cls_rows(x, cls, pos, B, T, D, c.st));
+    c.launch([&] { return udb_set_cls_rows(x, cls, pos, B, T, D, c.st); });
   }
   VitBlocks v{B, T, D, D / 64, depth};
   int slice = 0, start = 0;
   vit_blocks(c, "blocks.", x, v, [&](int i) {
     if (i == start + cf.depths[slice]) { start = i; ++slice; }
     const int from_end = depth - 1 - i;
-    if (!c.dry && !c.rc)
-      c.done(udb_vit_tap(x, levels[slice], from_end < 4 ? clsbuf[from_end] : nullptr, B, N, D, i == start, c.st));
-    if (i == 0) c.tap("enc_block0", x, sizeof(float) * BT * D);
+    c.launch([&] { return udb_vit_tap(x, levels[slice], from_end < 4 ? clsbuf[from_end] : nullptr, B, N, D, i == start, c.st); });
   });
-  c.tap("enc_last", x, sizeof(float) * BT * D);
   ar.release(m);
 }
 
 static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, void* st) {
   const udb_v1_config_t& cf = e->cfg;
-  V1Ctx c;
-  c.e = e; c.ar = &ar; c.st = st; c.dry = ar.dry;
+  Ctx c{e, &ar, st, ar.dry};
   const int B = a.B, net_h = cf.net_h, net_w = cf.net_w, hid = cf.hidden;
   const V1Geom g = v1_geometry(a.H, a.W, net_h, net_w);
   const bool dino = cf.encoder == UDB_V1_ENCODER_DINOV2;
@@ -284,13 +268,7 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
     const size_t enc_mark = ar.mark();
     const long long n0 = static_cast<long long>(B) * sh[0] * sw[0];
     __half* patches = ar.h(n0 * 64);
-    if (!c.dry) {
-      udb_v1_preprocess_t p;
-      memset(&p, 0, sizeof(p));
-      p.rgb = a.rgb; p.rgb_is_u8 = a.rgb_is_u8; p.scale255 = a.scale255; p.normalize = a.normalize; p.B = B; p.H = a.H; p.W = a.W;
-      p.rh = g.rh; p.rw = g.rw; p.pad_l = g.pad_l; p.pad_t = g.pad_t; p.net_h = net_h; p.net_w = net_w; p.patches = patches;
-      c.done(udb_v1_preprocess(&p, st));
-    }
+    preprocess(c, cf, a, g, patches, 0);
     const int C0 = cf.dims[0];
     __half* y0 = ar.h(n0 * C0);
     { Ctx::G q{patches, c.H("stem_w"), static_cast<int>(n0), C0, 64}; q.bias = c.F("stem_b"); q.out = y0; c.gemm(q); }
@@ -320,14 +298,12 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
         x16 = xn16;
       }
       for (int j = 0; j < cf.depths[i]; ++j, ++blk) {
-        c.cvnxt_block(idx2("s%d.b%d.", i, j), x, x16, B, sh[i], sw[i], C, 1e-6f);
-        if (!c.dry && !c.rc) c.done(udb_max_accum_f16(x16, levels[i], n * C, j == 0, st));
+        cvnxt_block(c, idx2("s%d.b%d.", i, j), x, x16, B, sh[i], sw[i], C, 1e-6f);
+        c.launch([&] { return udb_max_accum_f16(x16, levels[i], n * C, j == 0, st); });
         const int from_end = total_blocks - 1 - blk;
-        if (from_end < 4 && !c.dry && !c.rc) c.done(udb_spatial_mean_f32(x, clsbuf[from_end], B, sh[i] * sw[i], C, st));
-        if (blk == 0) c.tap("enc_block0", x, sizeof(float) * n * C);
+        if (from_end < 4) c.launch([&] { return udb_spatial_mean_f32(x, clsbuf[from_end], B, sh[i] * sw[i], C, st); });
       }
     }
-    c.tap("enc_last", x, sizeof(float) * B * sh[3] * sw[3] * cf.dims[3]);
     ar.release(enc_mark);
   }
 
@@ -343,19 +319,18 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
     const __half* src = levels[l];
     if (sh[l] != hc || sw[l] != wc) {
       __half* r = ar.h(Rq * C);
-      if (!c.dry && !c.rc) c.done(udb_aa_resize_nhwc_f16(levels[l], r, B, sh[l], sw[l], C, hc, wc, st));
+      c.launch([&] { return udb_aa_resize_nhwc_f16(levels[l], r, B, sh[l], sw[l], C, hc, wc, st); });
       src = r;
     }
     __half* an = ar.h(Rq * C);
     const std::string ad = idx("adapt.%d.", l);
-    c.ln16(src, 0, an, ad + "ln_w", ad + "ln_b", Rq, C, 1e-5f);
+    ln16(c, src, 0, an, ad + "ln_w", ad + "ln_b", Rq, C, 1e-5f);
     { Ctx::G q{an, c.H(ad + "w"), static_cast<int>(Rq), hid, C}; q.bias = c.F(ad + "b"); q.act = UDB_ACT_GELU; q.out = tokens;
       q.rows_per_group = nq; q.group_stride = 4 * nq; q.row_offset = l * nq; c.gemm(q); }
     { Ctx::G q{an, c.H(ad + "w"), static_cast<int>(Rq), hid, C}; q.bias = c.F(ad + "b"); q.act = UDB_ACT_GELU; q.out = featcat + l * hid;
       q.ldc = 4 * hid; c.gemm(q); }
     ar.release(m);
   }
-  c.tap("tokens", tokens, sizeof(__half) * Rq * 4 * hid);
   const float* tokens_pos = c.F("tokens_pos");                     // [4*nq, hid]: sine position + level embedding (decoder.py:410-433)
   {
     const Weight* tp = c.W("tokens_pos");
@@ -392,7 +367,7 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
         q.rows_per_group = 4 * nq; q.group_stride = 4 * nq + 4; q.row_offset = 0; c.gemm(q); }
       ar.release(m2);
     }
-    if (!c.dry && !c.rc) c.done(udb_copy_rows_f32_to_f16(cl, ctx, B, 4, hid, 4LL * nq + 4, 4LL * nq, st));
+    c.launch([&] { return udb_copy_rows_f32_to_f16(cl, ctx, B, 4, hid, 4LL * nq + 4, 4LL * nq, st); });
     // aggregate: the 4 tokens attend to the context (single head of width hid, position term on q)
     float* t;
     {
@@ -400,15 +375,17 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
       float* xn = ar.f(static_cast<size_t>(R4) * hid);
       c.layernorm(cl, 1, xn, 1, c.F(ag + "nxw"), c.F(ag + "nxb"), R4, hid, 1e-5f);
       __half* cn = ar.h(Rc * hid);
-      c.ln16(ctx, 0, cn, ag + "ncw", ag + "ncb", Rc, hid, 1e-5f);
+      ln16(c, ctx, 0, cn, ag + "ncw", ag + "ncb", Rc, hid, 1e-5f);
       __half* kv = ar.h(Rc * 2 * hid);
       { Ctx::G q{cn, c.H(ag + "kv_w"), static_cast<int>(Rc), 2 * hid, hid}; q.bias = c.F(ag + "kv_b"); q.out = kv; c.gemm(q); }
       float* q = ar.f(static_cast<size_t>(R4) * hid);
       c.small_linear(xn, R4, hid, c.F(ag + "q_w"), hid, c.F(ag + "q_b"), UDB_ACT_NONE, nullptr, nullptr, q);
       float* at = ar.f(static_cast<size_t>(R4) * hid);
       float* scratch = ar.f(static_cast<size_t>(B) * 16 * 4 * (hid + 2));
-      if (!c.dry && !c.rc)
-        c.done(udb_cross_attn_small(q, c.F("cam.pos"), kv, at, scratch, B, 4, 4 * nq + 4, hid, 1.0f / sqrtf(static_cast<float>(hid)), st));
+      const float* cam_pos = c.F("cam.pos");
+      c.launch([&] {
+        return udb_cross_attn_small(q, cam_pos, kv, at, scratch, B, 4, 4 * nq + 4, hid, 1.0f / sqrtf(static_cast<float>(hid)), st);
+      });
       float* t2 = ar.f(static_cast<size_t>(R4) * hid);
       c.small_linear(at, R4, hid, c.F(ag + "out_w"), hid, c.F(ag + "out_b"), UDB_ACT_NONE, c.F(ag + "ls1"), cl, t2);
       t = cam_mlp(c, ag + "mlp", t2, R4, hid, cf.expansion * hid, hid, t2, c.F(ag + "ls2"));
@@ -424,7 +401,8 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
       c.small_linear(xn, R4, hid, c.F(ly + "q_w"), hid, c.F(ly + "q_b"), UDB_ACT_NONE, nullptr, nullptr, q);
       c.small_linear(cn, R4, hid, c.F(ly + "kv_w"), 2 * hid, c.F(ly + "kv_b"), UDB_ACT_NONE, nullptr, nullptr, kv);
       float* a4 = ar.f(static_cast<size_t>(R4) * hid);
-      if (!c.dry && !c.rc) c.done(udb_camera_attn4_f32(q, kv, c.F("cam.pos"), a4, B, hid, cf.heads, st));
+      const float* cam_pos = c.F("cam.pos");
+      c.launch([&] { return udb_camera_attn4_f32(q, kv, cam_pos, a4, B, hid, cf.heads, st); });
       float* t2 = ar.f(static_cast<size_t>(R4) * hid);
       c.small_linear(a4, R4, hid, c.F(ly + "out_w"), hid, c.F(ly + "out_b"), UDB_ACT_NONE, c.F(ly + "ls1"), t, t2);
       t = cam_mlp(c, ly + "mlp", t2, R4, hid, cf.expansion * hid, hid, t2, c.F(ly + "ls2"));
@@ -435,11 +413,11 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
     x4 = xo;
     (void)m;
   }
-  if (!c.dry && !c.rc)
-    c.done(udb_v1_camera_intrinsics(x4, a.intrinsics, B, net_h, net_w, static_cast<float>(g.ratio), g.pad_l, g.pad_t, a.skip_camera, intr4,
-                                    a.out_intrinsics, k4_points, st));
+  c.launch([&] {
+    return udb_v1_camera_intrinsics(x4, a.intrinsics, B, net_h, net_w, static_cast<float>(g.ratio), g.pad_l, g.pad_t, a.skip_camera,
+                                    intr4, a.out_intrinsics, k4_points, st);
+  });
 
-  c.tap("intr4", intr4, sizeof(float) * B * 4);
   // ---- ray embeddings at the three decoder levels (decoder.py:203-220)
   stage.next("udb_v1:ray_embeddings");
   float* emb[3];
@@ -463,13 +441,13 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
       const size_t m = ar.mark();
       __half* r = ar.h(R * 128);
       __half* m1 = ar.h(R * 384);
-      if (!c.dry && !c.rc) {
+      {
         udb_v1_rays_t p;
         memset(&p, 0, sizeof(p));
         p.intr4 = intr4; p.B = B; p.net_h = net_h; p.net_w = net_w; p.gh = gh; p.gw = gw;
         p.ln_w = c.F(std::string(names[s]) + "ln_w"); p.ln_b = c.F(std::string(names[s]) + "ln_b"); p.out = r;
         memcpy(p.sh_k, shk, sizeof(shk));
-        c.done(udb_v1_rays_sh81(&p, st));
+        c.launch([&] { return udb_v1_rays_sh81(&p, st); });
       }
       const std::string n = names[s];
       c.expect2(n + "w1", 384, 128);
@@ -488,19 +466,14 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
     { Ctx::G q{featcat, c.H("fcc_w"), static_cast<int>(Rq), hid, 4 * hid}; q.bias = c.F("fcc_b"); q.out = f16l; c.gemm(q); }
     __half* hN = ar.h(Rq * hid);
     __half* md = ar.h(Rq * 2 * hid);
-    c.ln16(f16l, 0, hN, "lat.nw", "lat.nb", Rq, hid, 1e-5f);
+    ln16(c, f16l, 0, hN, "lat.nw", "lat.nb", Rq, hid, 1e-5f);
     { Ctx::G q{hN, c.H("lat.w1"), static_cast<int>(Rq), 2 * hid, hid}; q.bias = c.F("lat.b1"); q.act = UDB_ACT_GELU; q.out = md; c.gemm(q); }
     { Ctx::G q{md, c.H("lat.w2"), static_cast<int>(Rq), hid, 2 * hid}; q.bias = c.F("lat.b2"); q.out = lat16; q.out_f32 = 1; c.gemm(q); }
     ar.release(m);
   }
-  c.tap("emb16", emb[0], sizeof(float) * Rq * hid);
-  c.tap("lat16_init", lat16, sizeof(float) * Rq * hid);
   dense_attn_block(c, "agg16.", lat16, B, nq, hid, tokens, 0, 4 * nq, tokens_pos);
-  c.tap("lat16_agg", lat16, sizeof(float) * Rq * hid);
   dense_attn_block(c, "prompt.", lat16, B, nq, hid, emb[0], 1, nq, nullptr);
-  c.tap("lat16_prompt", lat16, sizeof(float) * Rq * hid);
   for (int i = 0; i < cf.dec_depths[0]; ++i) mh_attn_block(c, idx("l16.%d.", i), lat16, B, nq, hid, cf.heads, emb[0], false);
-  c.tap("lat16", lat16, sizeof(float) * Rq * hid);
 
   float* outs[3];
   float* lat = lat16;
@@ -517,11 +490,9 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
     __half* nxt16 = ar.h(Rn * (C / 2));
     outs[s] = ar.f(Rn);
     conv_upsample(c, ups[s], lat, emb[s], B, ch, cw, C, nxt, nxt16);
-    if (!c.dry && !c.rc)
-      c.done(udb_conv3x3_c1_exp(nxt16, c.F(std::string(ons[s]) + ".w"), static_cast<float>(c.S(std::string(ons[s]) + ".b")), outs[s], B, 2 * ch, 2 * cw,
-                                C / 2, st));
-    c.tap(s == 0 ? "lat8" : (s == 1 ? "lat4" : "lat2"), nxt, sizeof(float) * Rn * (C / 2));
-    c.tap(ons[s], outs[s], sizeof(float) * Rn);
+    const float* head_w = c.F(std::string(ons[s]) + ".w");
+    const float head_b = static_cast<float>(c.S(std::string(ons[s]) + ".b"));
+    c.launch([&] { return udb_conv3x3_c1_exp(nxt16, head_w, head_b, outs[s], B, 2 * ch, 2 * cw, C / 2, st); });
     lat = nxt;
     ch *= 2; cw *= 2; C /= 2;
   }
@@ -529,14 +500,14 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
   // ---- post-processing (unidepthv1.py:66-94,352-366)
   stage.next("udb_v1:postprocess");
   float* mean = ar.f(static_cast<size_t>(B) * net_h * net_w);
-  if (!c.dry && !c.rc) c.done(udb_v1_mean_maps(outs[0], outs[1], outs[2], mean, B, hc, wc, net_h, net_w, st));
-  if (!c.dry && !c.rc) {
+  c.launch([&] { return udb_v1_mean_maps(outs[0], outs[1], outs[2], mean, B, hc, wc, net_h, net_w, st); });
+  {
     udb_v1_postprocess_t p;
     memset(&p, 0, sizeof(p));
     p.mean = mean; p.k4 = k4_points; p.B = B; p.net_h = net_h; p.net_w = net_w;
     p.pad_l = g.pad_l; p.pad_r = g.pad_r; p.pad_t = g.pad_t; p.pad_b = g.pad_b; p.H = a.H; p.W = a.W;
     p.out_depth = a.out_depth; p.out_points = a.out_points;
-    c.done(udb_v1_postprocess(&p, st));
+    c.launch([&] { return udb_v1_postprocess(&p, st); });
   }
   if (!c.rc && ar.overflow) { set_error("engine_v1: workspace too small (%zu bytes needed)", ar.peak); return 1; }
   return c.rc;
@@ -590,19 +561,11 @@ int udb_v1_geometry(int32_t H, int32_t W, int32_t net_h, int32_t net_w, udb_v1_g
 }
 
 int udb_v1_set_weight(udb_engine_v1* e, const char* name, const void* dev_ptr, const int64_t* shape, int32_t ndim, int32_t dtype) {
-  if (!e || !name || !dev_ptr || ndim < 0 || ndim > 4) { set_error("udb_v1_set_weight: bad argument"); return 1; }
-  if (reinterpret_cast<uintptr_t>(dev_ptr) & 15) { set_error("udb_v1_set_weight(%s): pointer must be 16-byte aligned", name); return 1; }
-  Weight w;
-  w.p = dev_ptr; w.dtype = dtype; w.ndim = ndim;
-  for (int i = 0; i < ndim; ++i) w.shape[i] = shape[i];
-  e->w[name] = w;
-  return 0;
+  return EngineBase::set_weight(e, "udb_v1_set_weight", name, dev_ptr, shape, ndim, dtype);
 }
 
 int udb_v1_set_scalar(udb_engine_v1* e, const char* name, double value) {
-  if (!e || !name) { set_error("udb_v1_set_scalar: bad argument"); return 1; }
-  e->scalars[name] = value;
-  return 0;
+  return EngineBase::set_scalar(e, "udb_v1_set_scalar", name, value);
 }
 
 size_t udb_v1_workspace_bytes(udb_engine_v1* e, int32_t B, int32_t H, int32_t W) {
@@ -612,25 +575,15 @@ size_t udb_v1_workspace_bytes(udb_engine_v1* e, int32_t B, int32_t H, int32_t W)
   a.B = B; a.H = H; a.W = W;
   Arena ar(nullptr, 0);
   if (run_v1(e, a, ar, nullptr)) return 0;
-  char key[96];
-  snprintf(key, sizeof(key), "%d,%d,%d", B, H, W);
-  e->ws_need[key] = ar.peak + 256;
-  return ar.peak + 256;
+  return e->prepared(shape_name(B, H, W), ar.peak + 256);
 }
 
 int udb_infer_v1(udb_engine_v1* e, const udb_infer_v1_args_t* a, void* stream) {
   if (!e || !a || !a->rgb || !a->workspace) { set_error("udb_infer_v1: null argument"); return 1; }
   if (!a->out_intrinsics || !a->out_points || !a->out_depth) { set_error("udb_infer_v1: all three output pointers are required"); return 1; }
   if (a->skip_camera && !a->intrinsics) { set_error("udb_infer_v1: skip_camera needs intrinsics"); return 1; }
-  char key[96];
-  snprintf(key, sizeof(key), "%d,%d,%d", a->B, a->H, a->W);
-  auto need = e->ws_need.find(key);
-  if (need == e->ws_need.end()) { set_error("udb_infer_v1: shape %dx%dx%d not prepared; call udb_v1_workspace_bytes first", a->B, a->H, a->W); return 1; }
-  if (a->workspace_bytes < need->second) {
-    set_error("udb_infer_v1: workspace too small (%zu bytes given, %zu needed)", a->workspace_bytes, need->second);
+  if (e->check_workspace("udb_infer_v1", "udb_v1_workspace_bytes", shape_name(a->B, a->H, a->W), a->workspace, a->workspace_bytes))
     return 1;
-  }
-  if (reinterpret_cast<uintptr_t>(a->workspace) & 255) { set_error("udb_infer_v1: workspace must be 256-byte aligned"); return 1; }
   Arena ar(a->workspace, a->workspace_bytes);
   return run_v1(e, *a, ar, stream);
 }
