@@ -129,6 +129,12 @@ typedef struct udb_gemm_t {
 } udb_gemm_t;
 
 int udb_gemm_f16(const udb_gemm_t* g, void* stream);
+/* The same GEMM on FP8 E4M3 operands (UniDepthV2 precision "fp8"): A [M,K] and W [N,K] of `g` are e4m3 bytes, both
+ * K-major (lda / ldw in bytes: >= K and multiples of 16), with f32 per-row scales a_scale[M] and per-column scales
+ * w_scale[N] (both 16-byte aligned): the epilogue starts from v = acc * a_scale[m] * w_scale[n], then adds bias, applies
+ * act / gamma / resid and stores as above.  The MMA partial sums are promoted into an f32 accumulator after every 128
+ * values of K.  a_mode MATRIX and the ROWS store only; no split operands, out_split or ln_stats_*. */
+int udb_gemm_e4m3(const udb_gemm_t* g, const float* a_scale, const float* w_scale, void* stream);
 /* Epilogue of the last udb_gemm_f16 call on the calling thread that got past its checks: 1 = the TMA-store epilogue
  * (plain ROWS store with an identity row map, no out2 / out_split / ln_stats_*, 16-byte aligned out and row pitch, and
  * a residual only as f32 with an f32 out), 0 = the general one.  Both give bit-identical outputs; setting the
@@ -206,6 +212,18 @@ typedef struct udb_layernorm_t {
 } udb_layernorm_t;
 
 int udb_layernorm(const udb_layernorm_t* p, void* stream);
+/* LayerNorm of f32 rows (in_f32 = 1, dim a multiple of 128 and <= 1024, no out_split / dim_valid; out_f32 is ignored) to
+ * FP8 E4M3 bytes -- the A operand and a_scale of udb_gemm_e4m3: with the row scale s = amax|y| / 448 (1 for an all-zero
+ * row) stored to out_scale[row], out[row, c] = e4m3(y * (448 / amax)), rounded to nearest even.  ld_out in bytes, a
+ * multiple of 4; out 4-byte aligned. */
+int udb_layernorm_e4m3(const udb_layernorm_t* p, float* out_scale, void* stream);
+
+/* Row quantiser f16 -> FP8 E4M3 for the A operand of udb_gemm_e4m3: out[r, c] = e4m3(in[r, c] * 448 / amax_r) with
+ * amax_r = max_c |in[r, c]|, round to nearest even, and the scale s[r] = amax_r / 448 (1 for an all-zero row) stored to
+ * scale[r].  cols % 8 == 0 and
+ * cols <= 4096; ld_in (elements) and ld_out (bytes) >= cols and multiples of 8; in / out 16-byte aligned. */
+int udb_quantize_rows_e4m3(const void* in, int64_t ld_in, void* out, int64_t ld_out, float* scale, int32_t rows, int32_t cols,
+                           void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Pre-processing + patch extraction (unidepthv2.py:288-297 + patch_embed.py:82's im2col):
@@ -519,7 +537,7 @@ int udb_postprocess(const udb_postprocess_t* p, void* stream);
  * ====================================================================================== */
 typedef struct udb_engine udb_engine;
 
-enum { UDB_DT_F16 = 0, UDB_DT_F32 = 1 };
+enum { UDB_DT_F16 = 0, UDB_DT_F32 = 1, UDB_DT_E4M3 = 2 };
 
 typedef struct udb_config_t {
   /* DINOv2 encoder (unidepth/models/backbones/dinov2.py:388-427, encoder.py:139-193) */
@@ -544,7 +562,10 @@ void udb_destroy(udb_engine* e);
  * reference's state_dict (SURVEY.md 8b).  dtype: UDB_DT_*. */
 int udb_set_weight(udb_engine* e, const char* name, const void* dev_ptr, const int64_t* shape, int32_t ndim,
                    int32_t dtype);
-/* Host scalars of the packed model (the two 1x1 head biases and their additive constants). */
+/* Host scalars of the packed model (the two 1x1 head biases and their additive constants), and the encoder mode:
+ * "precision" 0 = f16 operands, 1 = split-f16 (hi/lo) operands, 2 = FP8 E4M3 operands for the four linear layers of every
+ * encoder block (blocks.{i}.{qkv,proj,fc1,fc2}_w8 [N, K] UDB_DT_E4M3 with f32 per-output-channel scales *_w8s [N]; the
+ * activations are quantised per row on the fly); "fuse_ln" 1 = fused LayerNorm (precision 0 only). */
 int udb_set_scalar(udb_engine* e, const char* name, double value);
 
 /* Geometry of one call, same arithmetic as get_paddings / get_resize_factor (unidepthv2.py:36-77). */

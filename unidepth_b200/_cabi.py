@@ -213,7 +213,7 @@ class ProfileEntry(C.Structure):
     _fields_ = [("name", C.c_char * 48), ("ms", f32), ("flops", C.c_double), ("bytes", C.c_double)]
 
 
-DT_F16, DT_F32 = 0, 1
+DT_F16, DT_F32, DT_E4M3 = 0, 1, 2
 
 EXPORTS = {
     "udb_version": (i32, []),
@@ -222,10 +222,13 @@ EXPORTS = {
     "udb_profile_begin": (i32, [vp]),
     "udb_profile_end": (i32, [C.POINTER(ProfileEntry), i32]),
     "udb_gemm_f16": (i32, [C.POINTER(Gemm), vp]),
+    "udb_gemm_e4m3": (i32, [C.POINTER(Gemm), vp, vp, vp]),
     "udb_gemm_tma_epilogue_used": (i32, []),
     "udb_conv3x3_halo_f16": (i32, [C.POINTER(ConvHalo), vp]),
     "udb_attention_f16": (i32, [C.POINTER(Attn), vp]),
     "udb_layernorm": (i32, [C.POINTER(LayerNorm), vp]),
+    "udb_layernorm_e4m3": (i32, [C.POINTER(LayerNorm), vp, vp]),
+    "udb_quantize_rows_e4m3": (i32, [vp, i64, vp, i64, vp, i32, i32, vp]),
     "udb_preprocess_patchify": (i32, [C.POINTER(Preprocess), vp]),
     "udb_posembed_bicubic": (i32, [vp, i32, i32, vp, i32, i32, vp]),
     "udb_set_cls_rows": (i32, [vp, vp, vp, i32, i32, i32, vp]),

@@ -31,6 +31,7 @@ HUB_KWARGS = dict(library_name="UniDepth", repo_url="https://github.com/lpiccine
                   tags=["monocular-metric-depth-estimation"]) if _HAS_HF else {}
 
 f16, f32 = torch.float16, torch.float32
+_DTYPES = {f16: cabi.DT_F16, f32: cabi.DT_F32, torch.float8_e4m3fn: cabi.DT_E4M3}   # udb.h UDB_DT_*
 
 
 class _Node(nn.Module):
@@ -124,10 +125,10 @@ class EngineModel(nn.Module):
         _, _, set_weight, set_scalar = self._ENGINE_FNS
         lib = cabi.lib()
         for name, t in tensors.items():
-            assert t.is_contiguous() and t.dtype in (f16, f32), name
+            assert t.is_contiguous() and t.dtype in _DTYPES, name
             shape = (C.c_int64 * max(t.ndim, 1))(*t.shape)
             cabi.check(getattr(lib, set_weight)(handle, name.encode(), C.c_void_p(t.data_ptr()), shape, t.ndim,
-                                                cabi.DT_F32 if t.dtype == f32 else cabi.DT_F16), f"{set_weight}({name})")
+                                                _DTYPES[t.dtype]), f"{set_weight}({name})")
         for name, v in scalars.items():
             cabi.check(getattr(lib, set_scalar)(handle, name.encode(), float(v)), f"{set_scalar}({name})")
 

@@ -1,6 +1,8 @@
 // HBM-bound / latency-bound kernels of the UniDepthV2.infer() path: LayerNorm, preprocessing +
 // patch extraction, position-embedding resize, the fp32 camera head, ray embedding, bilinear
 // resamplers and the output assembly.  Reference call sites are cited in include/udb.h.
+#include <cuda_fp8.h>
+
 #include "common.h"
 #include "ptx.cuh"
 
@@ -17,12 +19,49 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
+// ------------------------------------------------------------------------------------ e4m3 quantisation
+// x rounded to nearest even at e4m3's precision, in f32 (|x| <= 464): 3 mantissa bits above 2^-6, multiples of 2^-9
+// below.  The e4m3x2 conversion that follows is then exact, so every byte is the round-to-nearest-even value of torch's
+// float8_e4m3fn cast by construction, whatever rounding the conversion instruction itself applies.
+__device__ __forceinline__ float round_e4m3(float x) {
+  const float a = fabsf(x);
+  float r;
+  if (a < 0.015625f) {
+    r = __fsub_rn(__fadd_rn(a, 24576.f), 24576.f);   // 24576 = 1.5 * 2^14: its ulp is 2^-9
+  } else {
+    const uint32_t u = __float_as_uint(a);
+    r = __uint_as_float((u + 0x7FFFFu + ((u >> 20) & 1u)) & 0xFFF00000u);
+  }
+  return copysignf(r, x);
+}
+
+// A row of e4m3 operands is q = e4m3(x * (448 / amax)) with the dequantisation scale s = amax / 448 (448 = the largest
+// finite e4m3 value); an all-zero row gets multiplier and scale 1.  Both are correctly rounded f32 divisions, so a host
+// model (torch: 448 / amax, x * inv, .to(float8_e4m3fn), amax / 448) reproduces every byte and scale.
+struct E4m3Row {
+  float inv, scale;
+  __device__ __forceinline__ explicit E4m3Row(float amax)
+      : inv(amax > 0.f ? 448.f / amax : 1.f), scale(amax > 0.f ? amax / 448.f : 1.f) {}
+  // four values, round to nearest even; |x * inv| exceeds 448 at most by the product's rounding, which round_e4m3
+  // brings back to 448 (torch's cast agrees there: it rounds everything below 464 to at most 448)
+  __device__ __forceinline__ uint32_t q4(float a, float b, float c, float d) const {
+    const auto q = [&](float x, float y) {
+      return (uint32_t)__nv_cvt_float2_to_fp8x2(make_float2(round_e4m3(__fmul_rn(x, inv)), round_e4m3(__fmul_rn(y, inv))),
+                                                __NV_SATFINITE, __NV_E4M3);
+    };
+    return q(a, b) | (q(c, d) << 16);
+  }
+};
+
 // ------------------------------------------------------------------------------------ LayerNorm
 // One warp per R rows (R = 1 by default; the R = 2 variant -- both rows' loads in flight before the first
 // reduction -- measured slower, see udb_layernorm); dim % 128 == 0, dim <= 1024; lane owns float4
 // #(lane + 32*i).
-template <bool IN_F32, bool OUT_F32, int R>
-__global__ void __launch_bounds__(256) layernorm_kernel(const udb_layernorm_t p) {
+// E4M3 (R = 1, f32 in): the normalised row stays in registers, is scaled by its amax and written as e4m3 bytes plus the
+// row scale to out_scale (udb_layernorm_e4m3).
+template <bool IN_F32, bool OUT_F32, int R, bool E4M3 = false>
+__global__ void __launch_bounds__(256) layernorm_kernel(const udb_layernorm_t p, float* out_scale) {
+  static_assert(!E4M3 || (IN_F32 && !OUT_F32 && R == 1), "e4m3 output: f32 rows, one per warp");
   const int row0 = (blockIdx.x * 8 + (threadIdx.x >> 5)) * R;
   const int lane = threadIdx.x & 31;
   pdl_launch_dependents();
@@ -72,30 +111,58 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const udb_layernorm_t p)
     }
     rstd[r] = rsqrtf(warp_sum(v) / (float)p.dim + p.eps);
   }
+  if constexpr (E4M3) {
+    float am = 0.f;
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    if (i < nvec) {
-      const int e = (lane + 32 * i) * 4;
-      const float4 w = __ldg(reinterpret_cast<const float4*>(p.weight + e));
-      const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + e));
+    for (int i = 0; i < 8; ++i) {
+      if (i < nvec) {
+        const int e = (lane + 32 * i) * 4;
+        const float4 w = __ldg(reinterpret_cast<const float4*>(p.weight + e));
+        const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + e));
+        const float y0 = (x[0][i].x - mean[0]) * rstd[0] * w.x + b.x;   // the same expression as the f16 / f32 outputs
+        const float y1 = (x[0][i].y - mean[0]) * rstd[0] * w.y + b.y;
+        const float y2 = (x[0][i].z - mean[0]) * rstd[0] * w.z + b.z;
+        const float y3 = (x[0][i].w - mean[0]) * rstd[0] * w.w + b.w;
+        x[0][i] = make_float4(y0, y1, y2, y3);
+        am = fmaxf(am, fmaxf(fmaxf(fabsf(y0), fabsf(y1)), fmaxf(fabsf(y2), fabsf(y3))));
+      }
+    }
+    const E4m3Row q(warp_max(am));
+    if (lane == 0) out_scale[row0] = q.scale;
+    uint8_t* op = reinterpret_cast<uint8_t*>(p.out) + (long long)row0 * p.ld_out;
 #pragma unroll
-      for (int r = 0; r < R; ++r) {
-        if (!live[r]) continue;
-        const float y0 = (x[r][i].x - mean[r]) * rstd[r] * w.x + b.x;
-        const float y1 = (x[r][i].y - mean[r]) * rstd[r] * w.y + b.y;
-        const float y2 = (x[r][i].z - mean[r]) * rstd[r] * w.z + b.z;
-        const float y3 = (x[r][i].w - mean[r]) * rstd[r] * w.w + b.w;
-        if (OUT_F32) {
-          *reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + (long long)(row0 + r) * p.ld_out + e) =
-              make_float4(y0, y1, y2, y3);
-        } else {
-          __half* op = reinterpret_cast<__half*>(p.out) + (long long)(row0 + r) * p.ld_out + e;
-          const uint2 hi = make_uint2(pack_half2(y0, y1), pack_half2(y2, y3));
-          *reinterpret_cast<uint2*>(op) = hi;
-          if (p.out_split > 0) {      // split-f16 precise mode: lo = f16(y - f32(hi)) at column + out_split
-            const float2 h01 = __half22float2(*reinterpret_cast<const __half2*>(&hi.x));
-            const float2 h23 = __half22float2(*reinterpret_cast<const __half2*>(&hi.y));
-            *reinterpret_cast<uint2*>(op + p.out_split) = make_uint2(pack_half2(y0 - h01.x, y1 - h01.y), pack_half2(y2 - h23.x, y3 - h23.y));
+    for (int i = 0; i < 8; ++i) {
+      if (i < nvec) {
+        const int e = (lane + 32 * i) * 4;
+        *reinterpret_cast<uint32_t*>(op + e) = q.q4(x[0][i].x, x[0][i].y, x[0][i].z, x[0][i].w);
+      }
+    }
+  } else {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      if (i < nvec) {
+        const int e = (lane + 32 * i) * 4;
+        const float4 w = __ldg(reinterpret_cast<const float4*>(p.weight + e));
+        const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + e));
+#pragma unroll
+        for (int r = 0; r < R; ++r) {
+          if (!live[r]) continue;
+          const float y0 = (x[r][i].x - mean[r]) * rstd[r] * w.x + b.x;
+          const float y1 = (x[r][i].y - mean[r]) * rstd[r] * w.y + b.y;
+          const float y2 = (x[r][i].z - mean[r]) * rstd[r] * w.z + b.z;
+          const float y3 = (x[r][i].w - mean[r]) * rstd[r] * w.w + b.w;
+          if (OUT_F32) {
+            *reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + (long long)(row0 + r) * p.ld_out + e) =
+                make_float4(y0, y1, y2, y3);
+          } else {
+            __half* op = reinterpret_cast<__half*>(p.out) + (long long)(row0 + r) * p.ld_out + e;
+            const uint2 hi = make_uint2(pack_half2(y0, y1), pack_half2(y2, y3));
+            *reinterpret_cast<uint2*>(op) = hi;
+            if (p.out_split > 0) {      // split-f16 precise mode: lo = f16(y - f32(hi)) at column + out_split
+              const float2 h01 = __half22float2(*reinterpret_cast<const __half2*>(&hi.x));
+              const float2 h23 = __half22float2(*reinterpret_cast<const __half2*>(&hi.y));
+              *reinterpret_cast<uint2*>(op + p.out_split) = make_uint2(pack_half2(y0 - h01.x, y1 - h01.y), pack_half2(y2 - h23.x, y3 - h23.y));
+            }
           }
         }
       }
@@ -636,6 +703,42 @@ __global__ void __launch_bounds__(256) postprocess_bicubic_kernel(const udb_post
   }
 }
 
+// f16 rows -> e4m3 rows + row scales (udb_quantize_rows_e4m3): one warp per row, lane holds 16-byte chunks
+// lane + 32 i (i < 16: up to 4096 columns) in registers between the amax reduction and the conversion
+__global__ void __launch_bounds__(256) quantize_rows_e4m3_kernel(const __half* __restrict__ in, long long ld_in,
+                                                                 uint8_t* __restrict__ out, long long ld_out,
+                                                                 float* __restrict__ scale, int rows, int cols) {
+  const int row = blockIdx.x * 8 + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (row >= rows) return;
+  const int nch = cols >> 3;
+  const uint4* ip = reinterpret_cast<const uint4*>(in + (long long)row * ld_in);
+  uint4 v[16];
+  __half2 am2 = __float2half2_rn(0.f);
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    const int c = lane + 32 * i;
+    if (c < nch) {
+      v[i] = ip[c];
+      const __half2* h = reinterpret_cast<const __half2*>(&v[i]);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) am2 = __hmax2(am2, __habs2(h[k]));
+    }
+  }
+  const E4m3Row q(warp_max(fmaxf(__low2float(am2), __high2float(am2))));
+  if (lane == 0) scale[row] = q.scale;
+  uint2* op = reinterpret_cast<uint2*>(out + (long long)row * ld_out);
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    const int c = lane + 32 * i;
+    if (c < nch) {
+      const __half2* h = reinterpret_cast<const __half2*>(&v[i]);
+      const float2 a = __half22float2(h[0]), b = __half22float2(h[1]), d = __half22float2(h[2]), f = __half22float2(h[3]);
+      op[c] = make_uint2(q.q4(a.x, a.y, b.x, b.y), q.q4(d.x, d.y, f.x, f.y));
+    }
+  }
+}
+
 static inline int grid_for(long long total, int block = 256) {
   long long g = (total + block - 1) / block;
   const long long cap = (long long)num_sms() * 16;
@@ -646,6 +749,24 @@ static inline int grid_for(long long total, int block = 256) {
 
 using namespace udb;
 #define ST(s) reinterpret_cast<cudaStream_t>(s)
+
+extern "C" int udb_layernorm_e4m3(const udb_layernorm_t* p, float* out_scale, void* stream) {
+  if (!p || !p->in_f32 || p->out_split || (p->dim_valid && p->dim_valid != p->dim) || !out_scale || (reinterpret_cast<uintptr_t>(out_scale) & 3)) {
+    set_error("udb_layernorm_e4m3: needs f32 input, no out_split / dim_valid and a 4-byte aligned out_scale");
+    return 1;
+  }
+  if (p->dim % 128 != 0 || p->dim > 1024) { set_error("udb_layernorm_e4m3: dim %d unsupported (multiple of 128, <= 1024)", p->dim); return 1; }
+  if (p->ld_out < p->dim || p->ld_out % 4 || (reinterpret_cast<uintptr_t>(p->out) & 3)) {
+    set_error("udb_layernorm_e4m3: `out` needs 4-byte alignment and ld_out >= dim, a multiple of 4 (ld_out %lld)", (long long)p->ld_out);
+    return 1;
+  }
+  note_work(0.0, (double)p->rows * p->dim * (4 + 1) + 4.0 * p->rows);
+  const int grid = (p->rows + 7) / 8;
+  if (grid == 0) return 0;
+  const cudaError_t e = launch_ex(layernorm_kernel<true, false, 1, true>, dim3(grid), dim3(256), 0, ST(stream), 1, *p, out_scale);
+  if (e != cudaSuccess) { set_error("layernorm_kernel launch: %s", cudaGetErrorString(e)); return 1; }
+  return check_launch("layernorm_e4m3_kernel");
+}
 
 extern "C" int udb_layernorm(const udb_layernorm_t* p, void* stream) {
   note_work(0.0, (double)p->rows * p->dim * ((p->in_f32 ? 4 : 2) + (p->out_f32 ? 4 : 2) + (p->out_split ? 2 : 0)));
@@ -676,18 +797,37 @@ extern "C" int udb_layernorm(const udb_layernorm_t* p, void* stream) {
   cudaError_t e;
   const dim3 g(grid), blk(256);
   if (R == 2) {
-    if (p->in_f32 && p->out_f32) e = launch_ex(layernorm_kernel<true, true, 2>, g, blk, 0, ST(stream), 1, *p);
-    else if (p->in_f32) e = launch_ex(layernorm_kernel<true, false, 2>, g, blk, 0, ST(stream), 1, *p);
-    else if (p->out_f32) e = launch_ex(layernorm_kernel<false, true, 2>, g, blk, 0, ST(stream), 1, *p);
-    else e = launch_ex(layernorm_kernel<false, false, 2>, g, blk, 0, ST(stream), 1, *p);
+    if (p->in_f32 && p->out_f32) e = launch_ex(layernorm_kernel<true, true, 2>, g, blk, 0, ST(stream), 1, *p, static_cast<float*>(nullptr));
+    else if (p->in_f32) e = launch_ex(layernorm_kernel<true, false, 2>, g, blk, 0, ST(stream), 1, *p, static_cast<float*>(nullptr));
+    else if (p->out_f32) e = launch_ex(layernorm_kernel<false, true, 2>, g, blk, 0, ST(stream), 1, *p, static_cast<float*>(nullptr));
+    else e = launch_ex(layernorm_kernel<false, false, 2>, g, blk, 0, ST(stream), 1, *p, static_cast<float*>(nullptr));
   } else {
-    if (p->in_f32 && p->out_f32) e = launch_ex(layernorm_kernel<true, true, 1>, g, blk, 0, ST(stream), 1, *p);
-    else if (p->in_f32) e = launch_ex(layernorm_kernel<true, false, 1>, g, blk, 0, ST(stream), 1, *p);
-    else if (p->out_f32) e = launch_ex(layernorm_kernel<false, true, 1>, g, blk, 0, ST(stream), 1, *p);
-    else e = launch_ex(layernorm_kernel<false, false, 1>, g, blk, 0, ST(stream), 1, *p);
+    if (p->in_f32 && p->out_f32) e = launch_ex(layernorm_kernel<true, true, 1>, g, blk, 0, ST(stream), 1, *p, static_cast<float*>(nullptr));
+    else if (p->in_f32) e = launch_ex(layernorm_kernel<true, false, 1>, g, blk, 0, ST(stream), 1, *p, static_cast<float*>(nullptr));
+    else if (p->out_f32) e = launch_ex(layernorm_kernel<false, true, 1>, g, blk, 0, ST(stream), 1, *p, static_cast<float*>(nullptr));
+    else e = launch_ex(layernorm_kernel<false, false, 1>, g, blk, 0, ST(stream), 1, *p, static_cast<float*>(nullptr));
   }
   if (e != cudaSuccess) { set_error("layernorm_kernel launch: %s", cudaGetErrorString(e)); return 1; }
   return check_launch("layernorm_kernel");
+}
+
+extern "C" int udb_quantize_rows_e4m3(const void* in, int64_t ld_in, void* out, int64_t ld_out, float* scale, int32_t rows,
+                                      int32_t cols, void* stream) {
+  if (!in || !out || !scale || rows < 0 || cols < 8 || cols > 4096 || cols % 8) {
+    set_error("udb_quantize_rows_e4m3: bad arguments (rows %d, cols %d: need a multiple of 8 in [8, 4096])", rows, cols);
+    return 1;
+  }
+  if (ld_in < cols || ld_in % 8 || ld_out < cols || ld_out % 8 || (reinterpret_cast<uintptr_t>(in) & 15) ||
+      (reinterpret_cast<uintptr_t>(out) & 15) || (reinterpret_cast<uintptr_t>(scale) & 3)) {
+    set_error("udb_quantize_rows_e4m3: ld_in %lld / ld_out %lld must be >= cols and multiples of 8, in / out 16-byte aligned",
+              (long long)ld_in, (long long)ld_out);
+    return 1;
+  }
+  note_work(0.0, (double)rows * cols * (2 + 1) + 4.0 * rows);
+  if (rows == 0) return 0;
+  quantize_rows_e4m3_kernel<<<(rows + 7) / 8, 256, 0, ST(stream)>>>(static_cast<const __half*>(in), ld_in, static_cast<uint8_t*>(out),
+                                                                    ld_out, scale, rows, cols);
+  return check_launch("quantize_rows_e4m3_kernel");
 }
 
 extern "C" int udb_preprocess_patchify(const udb_preprocess_t* p, void* stream) {

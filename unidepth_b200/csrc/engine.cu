@@ -90,10 +90,13 @@ static int run(udb_engine* e, const udb_infer_args_t& a, const udb_geometry_t& g
   // cls tokens / camera head are fp32 anyway, so the intrinsics then carry no f16 operand rounding at all.
   const bool sp = e->scalars.count("precision") && e->scalars["precision"] == 1.0;
   const int sx = sp ? 2 : 1;
+  // E4M3 mode (udb_set_scalar("precision", 2)): the four linear layers of every encoder block run on e4m3 operands
+  // (vit_block_e4m3); the patch embedding, attention and everything after the encoder stay as in the f16 mode.
+  const bool f8 = e->scalars.count("precision") && e->scalars["precision"] == 2.0;
   // Fused LayerNorm (udb_set_scalar("fuse_ln", 1), default f16 mode): norm1 / norm2 never run as their own pass.  The GEMM
   // that updates the residual stream (patch embed, attn.proj, mlp.fc2) also writes the f16 copy of its rows and their
   // per-part statistics; qkv / fc1 read that copy with LayerNorm-folded weights (udb_gemm_t.ln_*; block.py:84-109).
-  const bool fuse = !sp && e->scalars.count("fuse_ln") && e->scalars["fuse_ln"] == 1.0;
+  const bool fuse = !sp && !f8 && e->scalars.count("fuse_ln") && e->scalars["fuse_ln"] == 1.0;
   const int ln_bn = D % 256 == 0 ? 256 : (D % 192 == 0 ? 192 : (D % 128 == 0 ? 128 : 64));   // udb_gemm_f16's tile width for N = D
   const int ln_parts = D / ln_bn * 2, ln_pc = ln_bn / 2;
   __half* x16 = fuse ? ar.h(BT * D) : nullptr;
@@ -130,7 +133,7 @@ static int run(udb_engine* e, const udb_infer_args_t& a, const udb_geometry_t& g
   for (int l = 0; l < 4; ++l) { feats[l] = ar.h(BN * D); clss[l] = ar.f(static_cast<size_t>(B) * D); }
   {
     VitBlocks v{B, T, D, cf.enc_heads, cf.depth};
-    v.split = sp; v.fuse = fuse; v.x16 = x16; v.stats = stats; v.ln_parts = ln_parts; v.ln_pc = ln_pc;
+    v.split = sp; v.fuse = fuse; v.fp8 = f8; v.x16 = x16; v.stats = stats; v.ln_parts = ln_parts; v.ln_pc = ln_pc;
     int tap = 0;
     vit_blocks(c, "blocks.", x, v, [&](int i) {
       if (tap < 4 && i + 1 == cf.taps[tap]) {

@@ -161,6 +161,7 @@ struct Ctx {
     int a_split_k = 0, out_split = 0;    // split-f16 precise mode (udb_gemm_t)
     float* ln_stats_out = nullptr; const float* ln_stats_in = nullptr; const float* ln_c1 = nullptr;   // fused LayerNorm (udb_gemm_t.ln_*)
     int ln_parts = 0, ln_part_cols = 0; float ln_eps = 0.f;
+    const float* a_scale = nullptr; const float* w_scale = nullptr;   // set: e4m3 operands (udb_gemm_e4m3)
   };
   void gemm(const G& q) {
     udb_gemm_t g;
@@ -178,7 +179,7 @@ struct Ctx {
     g.a_split_k = q.a_split_k; g.out_split = q.out_split;
     g.ln_stats_out = q.ln_stats_out; g.ln_stats_in = q.ln_stats_in; g.ln_c1 = q.ln_c1;
     g.ln_parts = q.ln_parts; g.ln_part_cols = q.ln_part_cols; g.ln_eps = q.ln_eps;
-    launch([&] { return udb_gemm_f16(&g, st); });
+    launch([&] { return q.a_scale ? udb_gemm_e4m3(&g, q.a_scale, q.w_scale, st) : udb_gemm_f16(&g, st); });
   }
   // ConvTranspose2d with kernel == stride == k as a GEMM with a pixel-shuffle store (ops.conv_transpose_ks)
   void conv_transpose(const void* x, int M, int K, const void* w, int k, int cout, int h, int ww, const float* bias,
@@ -239,6 +240,18 @@ struct Ctx {
     p.out_split = out_split;
     launch([&] { return udb_layernorm(&p, st); });
   }
+  // LayerNorm of f32 rows straight to e4m3 bytes + row scales (the A operand of an e4m3 GEMM)
+  void layernorm_e4m3(const float* in, void* out, float* scale, const float* w, const float* b, int rows, int dim, float eps) {
+    udb_layernorm_t p;
+    memset(&p, 0, sizeof(p));
+    p.in = in; p.in_f32 = 1; p.out = out; p.weight = w; p.bias = b;
+    p.rows = rows; p.dim = dim; p.ld_in = dim; p.ld_out = dim; p.eps = eps;
+    launch([&] { return udb_layernorm_e4m3(&p, scale, st); });
+  }
+  // f16 rows -> dense e4m3 rows + row scales
+  void quantize_e4m3(const __half* in, long long ld_in, void* out, float* scale, int rows, int cols) {
+    launch([&] { return udb_quantize_rows_e4m3(in, ld_in, out, cols, scale, rows, cols, st); });
+  }
   // LayerNorm for any width that is a multiple of 64, with the optional added term and space-to-depth store (UniDepthV1)
   void ln_any(const void* in, int in_f32, void* out, int out_f32, const float* w, const float* b, long long rows, int dim,
               float eps, long long ld_out = 0, const float* add = nullptr, long long add_mod = 0, int s2d_h = 0,
@@ -295,10 +308,43 @@ struct VitBlocks {
   int B, T, D, heads, depth;
   bool split = false;          // split-f16 precise mode: operands are [hi | lo] pairs, weights [N, 3K] = [hi | hi | lo]
   bool fuse = false;           // fused LayerNorm: norm1 / norm2 folded into qkv / fc1 (udb_gemm_t.ln_*)
+  bool fp8 = false;            // e4m3 mode: qkv / proj / fc1 / fc2 on e4m3 operands with per-row / per-channel scales
   __half* x16 = nullptr;       // fused mode: f16 copy of x and its per-part LayerNorm statistics, kept up to date by the
   float* stats = nullptr;      // GEMMs that write x (the patch embedding included)
   int ln_parts = 0, ln_pc = 0;
 };
+
+// One block in e4m3 mode: each of the four linear layers reads an e4m3 copy of its input (LayerNorm or row quantiser,
+// one scale per row) and e4m3 weights with one scale per output channel; attention and the epilogues are those of the
+// f16 mode.  `q8` / `qs` hold the current GEMM's A operand and row scales; the stream orders their reuse.
+static inline void vit_block_e4m3(Ctx& c, const std::string& b, float* x, const VitBlocks& v, __half* qkv, __half* att,
+                                  __half* mid, void* q8, float* qs) {
+  const int D = v.D, BT = v.B * v.T;
+  c.expect2(b + "qkv_w8", 3 * D, D);
+  c.expect2(b + "proj_w8", D, D);
+  c.expect2(b + "fc1_w8", 4 * D, D);
+  c.expect2(b + "fc2_w8", D, 4 * D);
+  for (const char* n : {"qkv_w8", "proj_w8", "fc1_w8", "fc2_w8"}) {   // f16 bytes would be read as e4m3 pairs
+    const Weight* w = c.W(b + n);
+    if (!c.rc && w->dtype != UDB_DT_E4M3) {
+      set_error("engine: packed tensor '%s' has dtype %d, expected e4m3 (%d)", (b + n).c_str(), w->dtype, UDB_DT_E4M3);
+      c.rc = 1;
+    }
+  }
+  c.layernorm_e4m3(x, q8, qs, c.F(b + "n1w"), c.F(b + "n1b"), BT, D, 1e-6f);
+  { Ctx::G q{q8, c.W(b + "qkv_w8")->p, BT, 3 * D, D}; q.a_scale = qs; q.w_scale = c.F(b + "qkv_w8s");
+    q.bias = c.F(b + "qkv_b"); q.out = qkv; c.gemm(q); }
+  c.attention(qkv, qkv, qkv, att, v.B, v.heads, v.T, v.T, 3 * D, 3 * D, 3 * D, D, 0, D, 2 * D, 0.125f);
+  c.quantize_e4m3(att, D, q8, qs, BT, D);
+  { Ctx::G q{q8, c.W(b + "proj_w8")->p, BT, D, D}; q.a_scale = qs; q.w_scale = c.F(b + "proj_w8s");
+    q.bias = c.F(b + "proj_b"); q.gamma = c.F(b + "ls1"); q.resid = x; q.resid_f32 = 1; q.out = x; q.out_f32 = 1; c.gemm(q); }
+  c.layernorm_e4m3(x, q8, qs, c.F(b + "n2w"), c.F(b + "n2b"), BT, D, 1e-6f);
+  { Ctx::G q{q8, c.W(b + "fc1_w8")->p, BT, 4 * D, D}; q.a_scale = qs; q.w_scale = c.F(b + "fc1_w8s");
+    q.bias = c.F(b + "fc1_b"); q.act = UDB_ACT_GELU; q.out = mid; c.gemm(q); }
+  c.quantize_e4m3(mid, 4 * D, q8, qs, BT, 4 * D);
+  { Ctx::G q{q8, c.W(b + "fc2_w8")->p, BT, D, 4 * D}; q.a_scale = qs; q.w_scale = c.F(b + "fc2_w8s");
+    q.bias = c.F(b + "fc2_b"); q.gamma = c.F(b + "ls2"); q.resid = x; q.resid_f32 = 1; q.out = x; q.out_f32 = 1; c.gemm(q); }
+}
 
 // `depth` pre-norm transformer blocks (metadinov2/block.py:84-109, LayerNorm eps 1e-6) on the f32 residual stream
 // x [B*T, D], weights "<prefix><i>.<operand>" as unidepthv2.pack_vit_encoder packs them.  after_block(i) runs once block
@@ -314,13 +360,20 @@ static inline void vit_blocks(Ctx& c, const std::string& prefix, float* x, const
   float* stats = v.stats;
   const int ln_parts = v.ln_parts, ln_pc = v.ln_pc;
   const size_t m = ar.mark();
-  __half* h = fuse ? nullptr : ar.h(BT * D * sx);
+  __half* h = (fuse || v.fp8) ? nullptr : ar.h(BT * D * sx);
   __half* qkv = ar.h(BT * 3 * D * sx);
   __half* att = ar.h(BT * D * sx);
   __half* mid = ar.h(BT * 4 * D * sx);
+  void* q8 = v.fp8 ? ar.alloc(BT * 4 * D) : nullptr;   // e4m3 mode: A operand (up to 4D bytes per row) and row scales
+  float* qs = v.fp8 ? ar.f(BT) : nullptr;
   const int kx = sp ? 3 : 1;          // logical K multiplier of a split operand
   for (int i = 0; i < v.depth; ++i) {
     const std::string b = prefix + idx("%d.", i);
+    if (v.fp8) {
+      vit_block_e4m3(c, b, x, v, qkv, att, mid, q8, qs);
+      after_block(i);
+      continue;
+    }
     // a weight packed for another mode (or transposed) must be refused, not read with the wrong leading dimension
     c.expect2(b + (fuse ? "qkv_wf" : "qkv_w"), 3 * D, D * kx);
     c.expect2(b + (fuse ? "fc1_wf" : "fc1_w"), 4 * D, D * kx);

@@ -65,6 +65,9 @@ struct GemmArgs {
   const float* ln_c1;
   int ln_parts, ln_part_cols;
   float ln_eps;
+  // e4m3 operands (udb_gemm_e4m3): acc is dequantised as acc * a_scale[m] * w_scale[n] before the epilogue
+  const float* a_scale;
+  const float* w_scale;
 };
 
 // TMA epilogue staging box: one warpgroup's 64 rows x 32 columns, f32 (128 B rows, 128B swizzle) or f16 (64 B rows,
@@ -461,14 +464,40 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmArgs& p, const CUten
   }
 }
 
+// e4m3 mode: scale the finished accumulator tile in registers, acc = (acc * a_scale[m]) * w_scale[n], so that both
+// epilogues then run unchanged.  Fragment layout as in ptx.cuh (d[4j + 2h + e]: row 16 wq + lane / 4 + 8h, column
+// 8j + 2 (lane % 4) + e of the warpgroup's 64 x BN tile).  Rows past M and columns past N get scale 0.
+template <int BN>
+__device__ __forceinline__ void dequant_acc(const GemmArgs& p, float (&acc)[BN / 2], const int mt, const int nt, const int wg,
+                                            const int wq, const int lane) {
+  const int r0 = mt * BM + 64 * wg + 16 * wq + (lane >> 2);
+  const float s0 = r0 < p.M ? __ldg(p.a_scale + r0) : 0.f;
+  const float s1 = r0 + 8 < p.M ? __ldg(p.a_scale + r0 + 8) : 0.f;
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int n = nt * BN + 8 * j + 2 * (lane & 3);
+    const float2 ws = n < p.N ? __ldg(reinterpret_cast<const float2*>(p.w_scale + n)) : make_float2(0.f, 0.f);
+    acc[4 * j] = acc[4 * j] * s0 * ws.x;
+    acc[4 * j + 1] = acc[4 * j + 1] * s0 * ws.y;
+    acc[4 * j + 2] = acc[4 * j + 2] * s1 * ws.x;
+    acc[4 * j + 3] = acc[4 * j + 3] * s1 * ws.y;
+  }
+}
+
 // TMAE: TMA epilogue (tmC: `out`, box 32 x 64; tmR: f32 `resid`, box 32 x 128; both unused otherwise)
-template <int BN, bool LNF, bool TMAE>
+// FP8: A and W are e4m3 (udb_gemm_e4m3).  A k-block is still one 128-byte swizzled row per operand row (128 values), so
+// the stage layout, TMA boxes and barrier protocol are those of the f16 kernel; it runs as 4 x k32 e4m3 MMAs into a
+// partial accumulator that is added to the f32 accumulator once they complete (Hopper's e4m3 MMA accumulates with
+// fewer mantissa bits than f32, so sums are promoted every 128 products).
+template <int BN, bool LNF, bool TMAE, bool FP8 = false>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                 const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR, const GemmArgs p) {
   static_assert(!(TMAE && LNF), "the TMA epilogue carries no fused-LayerNorm code");
+  static_assert(!(FP8 && (LNF || BN > 128)), "e4m3 mode: no fused LayerNorm, tiles up to 128 columns (two accumulators)");
   using Cfg = GemmCfg<BN, TMAE>;
   constexpr int kStages = Cfg::kStages;
+  constexpr int kKB = FP8 ? 2 * BK : BK;   // elements per k-block (128 bytes per operand row either way)
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sA = smem;
   uint8_t* sB = smem + kStages * Cfg::kABytes;
@@ -557,11 +586,11 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             const int c0 = p.conv_coff + (kb % p.conv_cpb) * BK;
             tma_load_4d(sA + stage * Cfg::kABytes, &tmA, &full_bar[stage], c0, cx + tap % 3, cy + tap / 3, cb);
           } else {
-            int ka = kb * BK;
+            int ka = kb * kKB;
             if (p.a_wrap && ka >= p.a_wrap) ka -= p.a_wrap;
             tma_load_2d(sA + stage * Cfg::kABytes, &tmA, &full_bar[stage], ka, mt * BM);
           }
-          tma_load_2d(sB + stage * Cfg::kBBytes, &tmB, &full_bar[stage], kb * BK, nt * BN);
+          tma_load_2d(sB + stage * Cfg::kBBytes, &tmB, &full_bar[stage], kb * kKB, nt * BN);
         }
         __syncwarp();
         if (++stage == kStages) {
@@ -586,26 +615,53 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int mt = tile / p.tiles_n;
       const int nt = tile % p.tiles_n;
-      int prev = -1;
-      for (int kb = 0; kb < p.num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint64_t da = gmma_desc_sw128(smem_u32(sA + stage * Cfg::kABytes + wg * 64 * 128), 16, 1024);
-        const uint64_t db = gmma_desc_sw128(smem_u32(sB + stage * Cfg::kBBytes), 16, 1024);
-        wgmma_fence();
+      if constexpr (FP8) {
+        // no MMA overlap across k-blocks inside a warpgroup (the partial sum must be complete before it is promoted);
+        // the other consumer warpgroup keeps the tensor cores busy meanwhile
+        float part[BN / 2];
 #pragma unroll
-        for (int k = 0; k < BK / 16; ++k) WgmmaSS<BN>::run(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
-        wgmma_commit();
-        wgmma_wait<1>();   // the previous k-block's MMAs are done: release its stage
-        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
-        prev = stage;
-        if (++stage == kStages) {
-          stage = 0;
-          phase ^= 1;
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        for (int kb = 0; kb < p.num_kb; ++kb) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint64_t da = gmma_desc_sw128(smem_u32(sA + stage * Cfg::kABytes + wg * 64 * 128), 16, 1024);
+          const uint64_t db = gmma_desc_sw128(smem_u32(sB + stage * Cfg::kBBytes), 16, 1024);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < 4; ++k) WgmmaE4M3<BN>::run(part, da + 2 * k, db + 2 * k, k != 0 ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<0>();
+          wgmma_fence_regs(part);
+          if (lane == 0) mbar_arrive(&empty_bar[stage]);
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+          if (++stage == kStages) {
+            stage = 0;
+            phase ^= 1;
+          }
         }
+        dequant_acc<BN>(p, acc, mt, nt, wg, wq, lane);
+      } else {
+        int prev = -1;
+        for (int kb = 0; kb < p.num_kb; ++kb) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint64_t da = gmma_desc_sw128(smem_u32(sA + stage * Cfg::kABytes + wg * 64 * 128), 16, 1024);
+          const uint64_t db = gmma_desc_sw128(smem_u32(sB + stage * Cfg::kBBytes), 16, 1024);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < BK / 16; ++k) WgmmaSS<BN>::run(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<1>();   // the previous k-block's MMAs are done: release its stage
+          if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+          prev = stage;
+          if (++stage == kStages) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
       }
-      wgmma_wait<0>();
-      wgmma_fence_regs(acc);
-      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
       if constexpr (TMAE) epilogue_tile_tma<BN>(p, &tmC, etma, acc, mt, nt, wg, wq, lane);
       else epilogue_tile<BN, LNF>(p, ctx, acc, mt, nt);
     }
@@ -615,13 +671,13 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   }
 }
 
-template <int BN, bool LNF, bool TMAE>
+template <int BN, bool LNF, bool TMAE, bool FP8 = false>
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const CUtensorMap& tmR,
                        const GemmArgs& a, cudaStream_t st) {
   using Cfg = GemmCfg<BN, TMAE>;
   static std::atomic<uint64_t> attr_mask{0};
   if (first_on_device(attr_mask)) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_f16_kernel<BN, LNF, TMAE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(gemm_f16_kernel<BN, LNF, TMAE, FP8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          Cfg::kSmemBytes);
     if (e != cudaSuccess) {
       set_error("gemm: cudaFuncSetAttribute(%d B smem): %s", Cfg::kSmemBytes, cudaGetErrorString(e));
@@ -630,13 +686,13 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUt
   }
   const int tiles = a.tiles_m * a.tiles_n;
   const int grid = tiles < num_sms() ? tiles : num_sms();
-  cudaError_t e = launch_ex(gemm_f16_kernel<BN, LNF, TMAE>, dim3(grid), dim3(kThreads), Cfg::kSmemBytes, st, 1, tmA, tmB, tmC,
-                            tmR, a);
+  cudaError_t e = launch_ex(gemm_f16_kernel<BN, LNF, TMAE, FP8>, dim3(grid), dim3(kThreads), Cfg::kSmemBytes, st, 1, tmA, tmB,
+                            tmC, tmR, a);
   if (e != cudaSuccess) {
     set_error("gemm_f16_kernel launch: %s", cudaGetErrorString(e));
     return 1;
   }
-  return check_launch("gemm_f16_kernel");
+  return check_launch(FP8 ? "gemm_e4m3_kernel" : "gemm_f16_kernel");
 }
 
 static bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
@@ -750,8 +806,9 @@ static thread_local int g_last_tma_epilogue = 0;
 
 extern "C" int udb_gemm_tma_epilogue_used(void) { return udb::g_last_tma_epilogue; }
 
-extern "C" int udb_gemm_f16(const udb_gemm_t* g, void* stream) {
-  using namespace udb;
+namespace udb {
+// udb_gemm_f16 (a_scale == nullptr) and udb_gemm_e4m3
+static int gemm(const udb_gemm_t* g, const float* a_scale, const float* w_scale, void* stream) {
   if (!g || !g->a || !g->w) { set_error("udb_gemm_f16: null operand"); return 1; }
   if (g->N % 32 != 0) { set_error("udb_gemm_f16: N=%d must be a multiple of 32", g->N); return 1; }
   if (check_gemm_layout(g)) return 1;
@@ -789,12 +846,31 @@ extern "C" int udb_gemm_f16(const udb_gemm_t* g, void* stream) {
   if (g->out_split && (g->out_f32 || !g->out || g->store_mode != UDB_STORE_ROWS)) {
     set_error("udb_gemm_f16: out_split needs an f16 `out` with the ROWS store"); return 1;
   }
+  const bool fp8 = a_scale != nullptr;
+  if (fp8) {
+    if (g->a_mode != UDB_A_MATRIX || g->store_mode != UDB_STORE_ROWS) {
+      set_error("udb_gemm_e4m3: e4m3 operands need a_mode MATRIX and the ROWS store"); return 1;
+    }
+    if (g->a_split_k || g->out_split) { set_error("udb_gemm_e4m3: e4m3 operands exclude split-f16 operands and outputs"); return 1; }
+    if (g->ln_stats_out || g->ln_stats_in) { set_error("udb_gemm_e4m3: e4m3 operands exclude fused LayerNorm statistics"); return 1; }
+    if (!w_scale || !aligned(a_scale, 16) || !aligned(w_scale, 16)) {
+      set_error("udb_gemm_e4m3: `a_scale` [M] and `w_scale` [N] must be non-null and 16-byte aligned"); return 1;
+    }
+    if (g->lda < g->K || g->ldw < g->K || g->lda % 16 || g->ldw % 16) {
+      set_error("udb_gemm_e4m3: e4m3 rows need lda, ldw >= K and multiples of 16 (lda=%d ldw=%d K=%d)", g->lda, g->ldw, g->K);
+      return 1;
+    }
+    a.num_kb = (g->K + 2 * BK - 1) / (2 * BK);
+    a.a_scale = a_scale; a.w_scale = w_scale;
+  }
 
   // tile width: widest that divides the work sensibly
   int bn;
   if (g->store_mode == UDB_STORE_HEAD) {
     if (g->N != 32) { set_error("udb_gemm_f16: HEAD store needs N == 32"); return 1; }
     bn = 32;
+  } else if (fp8) {                        // two accumulators per thread (partial + promoted): at most 128 columns
+    bn = g->N % 128 == 0 ? 128 : (g->N % 64 == 0 ? 64 : 32);
   } else if (g->N % 256 == 0) bn = 256;
   else if (g->N % 192 == 0) bn = 192;      // ConvNeXt widths 192 / 384: 3 (or 6) times fewer passes over A than 64 / 128
   else if (g->N % 128 == 0) bn = 128;
@@ -844,15 +920,27 @@ extern "C" int udb_gemm_f16(const udb_gemm_t* g, void* stream) {
       set_error("udb_gemm_f16: tile store modes need a_mode == CONV3X3"); return 1;
     }
     const uint64_t dims[2] = {(uint64_t)(g->a_split_k > 0 ? 2 * g->a_split_k : g->K), (uint64_t)g->M};
-    const uint64_t str[1] = {(uint64_t)g->lda * 2};
-    const uint32_t box[2] = {(uint32_t)BK, (uint32_t)BM};
-    if (make_tmap_f16(&tmA, g->a, 2, dims, str, box, true)) return 1;
+    if (fp8) {   // one-byte elements: the same 128-byte swizzled box rows hold 128 values
+      const uint64_t str[1] = {(uint64_t)g->lda};
+      const uint32_t box[2] = {(uint32_t)(2 * BK), (uint32_t)BM};
+      if (make_tmap(&tmA, g->a, 2, dims, str, box, CU_TENSOR_MAP_DATA_TYPE_UINT8, CU_TENSOR_MAP_SWIZZLE_128B)) return 1;
+    } else {
+      const uint64_t str[1] = {(uint64_t)g->lda * 2};
+      const uint32_t box[2] = {(uint32_t)BK, (uint32_t)BM};
+      if (make_tmap_f16(&tmA, g->a, 2, dims, str, box, true)) return 1;
+    }
   }
   {
     const uint64_t dims[2] = {(uint64_t)g->K, (uint64_t)g->N};
-    const uint64_t str[1] = {(uint64_t)g->ldw * 2};
-    const uint32_t box[2] = {(uint32_t)BK, (uint32_t)bn};
-    if (make_tmap_f16(&tmB, g->w, 2, dims, str, box, true)) return 1;
+    if (fp8) {
+      const uint64_t str[1] = {(uint64_t)g->ldw};
+      const uint32_t box[2] = {(uint32_t)(2 * BK), (uint32_t)bn};
+      if (make_tmap(&tmB, g->w, 2, dims, str, box, CU_TENSOR_MAP_DATA_TYPE_UINT8, CU_TENSOR_MAP_SWIZZLE_128B)) return 1;
+    } else {
+      const uint64_t str[1] = {(uint64_t)g->ldw * 2};
+      const uint32_t box[2] = {(uint32_t)BK, (uint32_t)bn};
+      if (make_tmap_f16(&tmB, g->w, 2, dims, str, box, true)) return 1;
+    }
   }
   const bool tmae = tma_epilogue_ok(g);
   CUtensorMap tmC, tmR;
@@ -874,8 +962,16 @@ extern "C" int udb_gemm_f16(const udb_gemm_t* g, void* stream) {
   g_last_tma_epilogue = tmae ? 1 : 0;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   note_work(2.0 * a.M * (double)g->N * g->K,
-            2.0 * ((double)a.M * (g->a_mode == UDB_A_CONV3X3 ? g->conv_C : (g->a_split_k ? 2 * g->a_split_k : g->K)) + (double)g->N * g->K) +
+            (fp8 ? (double)a.M * g->K + (double)g->N * g->K + 4.0 * (a.M + g->N) :
+            2.0 * ((double)a.M * (g->a_mode == UDB_A_CONV3X3 ? g->conv_C : (g->a_split_k ? 2 * g->a_split_k : g->K)) + (double)g->N * g->K)) +
                 (double)a.M * g->N * ((g->out ? (g->out_f32 ? 4 : 2) : 0) + (g->out2 ? 2 : 0) + (g->resid ? (g->resid_f32 ? 4 : 2) : 0)));
+  if (fp8) {
+    switch (bn) {
+      case 128: return tmae ? launch_gemm<128, false, true, true>(tmA, tmB, tmC, tmR, a, st) : launch_gemm<128, false, false, true>(tmA, tmB, tmC, tmR, a, st);
+      case 64: return tmae ? launch_gemm<64, false, true, true>(tmA, tmB, tmC, tmR, a, st) : launch_gemm<64, false, false, true>(tmA, tmB, tmC, tmR, a, st);
+      default: return tmae ? launch_gemm<32, false, true, true>(tmA, tmB, tmC, tmR, a, st) : launch_gemm<32, false, false, true>(tmA, tmB, tmC, tmR, a, st);
+    }
+  }
   const bool lnf = g->ln_stats_out || g->ln_stats_in;
   if (lnf) {
     switch (bn) {
@@ -902,4 +998,12 @@ extern "C" int udb_gemm_f16(const udb_gemm_t* g, void* stream) {
     case 64: return launch_gemm<64, false, false>(tmA, tmB, tmC, tmR, a, st);
     default: return launch_gemm<32, false, false>(tmA, tmB, tmC, tmR, a, st);
   }
+}
+}  // namespace udb
+
+extern "C" int udb_gemm_f16(const udb_gemm_t* g, void* stream) { return udb::gemm(g, nullptr, nullptr, stream); }
+
+extern "C" int udb_gemm_e4m3(const udb_gemm_t* g, const float* a_scale, const float* w_scale, void* stream) {
+  if (!a_scale) { udb::set_error("udb_gemm_e4m3: `a_scale` [M] and `w_scale` [N] must be non-null and 16-byte aligned"); return 1; }
+  return udb::gemm(g, a_scale, w_scale, stream);
 }

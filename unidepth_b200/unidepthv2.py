@@ -30,13 +30,28 @@ from .camera import pack_camera
 from .spec import ModelSpec, PATCH, get_paddings, get_resize_factor, param_shapes, pixel_bounds
 
 
+def pack_e4m3(w: torch.Tensor):
+    """A GEMM weight [N, K] as FP8 E4M3 with one f32 scale per output channel: (w8, s) with s = amax / 448 (1 for an
+    all-zero row) and w8 = e4m3(w * (448 / amax)), rounded to nearest even; w ~= w8 * s.  The same arithmetic as the
+    engine's activation quantisers (include/udb.h udb_quantize_rows_e4m3)."""
+    w = w.to(f32)
+    amax = w.abs().amax(dim=1)
+    nz = amax > 0
+    one = torch.ones_like(amax)
+    # a tensor division (correctly rounded, as on the device): `448.0 / amax` would be computed as amax.reciprocal() * 448
+    inv = torch.where(nz, torch.full_like(amax, 448.0) / torch.where(nz, amax, one), one)
+    s = torch.where(nz, amax / 448.0, one)
+    return (w * inv[:, None]).to(torch.float8_e4m3fn).contiguous(), s.contiguous()
+
+
 def pack_vit_encoder(sd: dict, d: int, depth: int, dev, split: bool = False, fuse: bool = False,
-                     pe: str = "pixel_encoder.") -> Dict[str, torch.Tensor]:
+                     pe: str = "pixel_encoder.", fp8: bool = False) -> Dict[str, torch.Tensor]:
     """Operands of the DINOv2 encoder (patch embedding, cls token, position grid, `depth` blocks) from the reference
     state dict `sd`, under their engine names (`patch_w`, `cls`, `pos`, `blocks.{i}.qkv_w`, ...) and in the layouts the
     engines' shared block loop reads (engine_common.h `vit_blocks`).  UniDepthV2 packs every mode through it; UniDepthV1
     (ViT-L/14) uses the default f16 mode.  The position grid is returned as stored ([1 + 37*37, d]); how it is resized
-    to the patch grid differs between the two models."""
+    to the patch grid differs between the two models.  `fp8`: the blocks' four linear layers are packed as e4m3 weights
+    with per-output-channel scales (`blocks.{i}.qkv_w8`, `qkv_w8s`, ...; `pack_e4m3`)."""
     h16 = lambda t: t.to(f16).contiguous()
     c32 = lambda t: t.to(f32).contiguous()
 
@@ -71,6 +86,13 @@ def pack_vit_encoder(sd: dict, d: int, depth: int, dev, split: bool = False, fus
                 qkv_wf=qw, qkv_c1=qc1, qkv_c2=qc2, fc1_wf=fw, fc1_c1=fc1, fc1_c2=fc2,
                 proj_w=h16(sd[b + "attn.proj.weight"]), proj_b=c32(sd[b + "attn.proj.bias"]), ls1=c32(sd[b + "ls1.gamma"]),
                 fc2_w=h16(sd[b + "mlp.fc2.weight"]), fc2_b=c32(sd[b + "mlp.fc2.bias"]), ls2=c32(sd[b + "ls2.gamma"]))
+        elif fp8:
+            blk = dict(n1w=c32(sd[b + "norm1.weight"]), n1b=c32(sd[b + "norm1.bias"]), qkv_b=c32(sd[b + "attn.qkv.bias"]),
+                       proj_b=c32(sd[b + "attn.proj.bias"]), ls1=c32(sd[b + "ls1.gamma"]),
+                       n2w=c32(sd[b + "norm2.weight"]), n2b=c32(sd[b + "norm2.bias"]), fc1_b=c32(sd[b + "mlp.fc1.bias"]),
+                       fc2_b=c32(sd[b + "mlp.fc2.bias"]), ls2=c32(sd[b + "ls2.gamma"]))
+            for k, src in (("qkv", "attn.qkv"), ("proj", "attn.proj"), ("fc1", "mlp.fc1"), ("fc2", "mlp.fc2")):
+                blk[k + "_w8"], blk[k + "_w8s"] = pack_e4m3(sd[b + src + ".weight"])
         else:
             blk = dict(
                 n1w=c32(sd[b + "norm1.weight"]), n1b=c32(sd[b + "norm1.bias"]),
@@ -103,6 +125,10 @@ class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         # wgmma GEMM (three products hi.W_hi + lo.W_hi + hi.W_lo, include/udb.h udb_gemm_t.a_split_k) and attention
         # runs in fp32; ~4x slower.  It shows that the default mode's residual against the fp32 reference is operand
         # rounding: the intrinsics (fp32 camera head on the encoder's cls tokens) then meet north_star's 1e-4.
+        # "fp8": speed mode -- the four linear layers of every encoder block (qkv, proj, fc1, fc2) multiply FP8 E4M3
+        # operands on the e4m3 wgmma: weights with one scale per output channel, activations quantised per row on the
+        # fly (include/udb.h udb_gemm_e4m3).  The patch embedding, attention and the decoder are unchanged.  Its
+        # accuracy is only measured on seeded synthetic weights (tests/test_fp8_gpu.py), not on trained checkpoints.
         self.precision = "f16"
         # Fused LayerNorm (north_star: "fused LayerNorm + QKV projection"): norm1 / norm2 of the encoder blocks folded into
         # the qkv / fc1 GEMMs (include/udb.h udb_gemm_t.ln_*), no stand-alone LayerNorm pass.  f16 mode only.
@@ -133,9 +159,9 @@ class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         sd = {k: v.detach() for k, v in self.state_dict().items()}
         h16 = lambda t: t.to(f16).contiguous()
         c32 = lambda t: t.to(f32).contiguous()
-        if self.precision not in ("f16", "split"):
-            raise ValueError(f"precision must be 'f16' or 'split', not {self.precision!r}")
-        split = self.precision == "split"
+        if self.precision not in ("f16", "split", "fp8"):
+            raise ValueError(f"precision must be 'f16', 'split' or 'fp8', not {self.precision!r}")
+        split, fp8 = self.precision == "split", self.precision == "fp8"
         fuse = self._fuse()
 
         d, hid = s.embed_dim, s.hidden
@@ -157,8 +183,8 @@ class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         if c_hr_real % 8 or c_hr > 256:
             raise NotImplementedError(f"high-resolution feature width {c_hr_real} not supported")
         pe = "pixel_encoder."
-        T = pack_vit_encoder(sd, d, s.depth, dev, split, fuse)
-        S: Dict[str, float] = {"precision": 1.0 if split else 0.0, "fuse_ln": 1.0 if fuse else 0.0}
+        T = pack_vit_encoder(sd, d, s.depth, dev, split, fuse, fp8=fp8)
+        S: Dict[str, float] = {"precision": 1.0 if split else (2.0 if fp8 else 0.0), "fuse_ln": 1.0 if fuse else 0.0}
         T["norm_w"], T["norm_b"] = c32(sd[pe + "norm.weight"]), c32(sd[pe + "norm.bias"])
 
         pd = "pixel_decoder."
