@@ -221,7 +221,7 @@ int udb_layernorm_e4m3(const udb_layernorm_t* p, float* out_scale, void* stream)
 /* Row quantiser f16 -> FP8 E4M3 for the A operand of udb_gemm_e4m3: out[r, c] = e4m3(in[r, c] * 448 / amax_r) with
  * amax_r = max_c |in[r, c]|, round to nearest even, and the scale s[r] = amax_r / 448 (1 for an all-zero row) stored to
  * scale[r].  cols % 8 == 0 and
- * cols <= 4096; ld_in (elements) and ld_out (bytes) >= cols and multiples of 8; in / out 16-byte aligned. */
+ * cols <= 6144; ld_in (elements) and ld_out (bytes) >= cols and multiples of 8; in / out 16-byte aligned. */
 int udb_quantize_rows_e4m3(const void* in, int64_t ld_in, void* out, int64_t ld_out, float* scale, int32_t rows, int32_t cols,
                            void* stream);
 
@@ -411,6 +411,14 @@ int udb_layernorm_any(const udb_layernorm_any_t* p, void* stream);
  * w f32 [49, C] (tap-major), bias f32 [C] -> y f16 NHWC.  C % 64 == 0. */
 int udb_dwconv7_nhwc_f16(const void* x, const float* w, const float* bias, void* y, int32_t B, int32_t H, int32_t W,
                          int32_t C, void* stream);
+/* ConvNeXt block head of UniDepthV1 precision "fp8" (convnext.py:208-212: conv_dw -> norm), fused: the depthwise 7x7 of
+ * udb_dwconv7_nhwc_f16 (same x / w / bias, f32 accumulation, result rounded to f16 as that call stores it), then
+ * LayerNorm over the channels (eps 1e-6, f32 statistics; ln_w / ln_b f32 [C]) written straight as FP8 E4M3 bytes out
+ * [B*H*W, C] with the row scale s = amax|y| / 448 (1 for an all-zero row) in out_scale[B*H*W] and
+ * out = e4m3(y * (448 / amax)), rounded to nearest even -- the A operand and a_scale of udb_gemm_e4m3, with the
+ * arithmetic of udb_layernorm_e4m3.  C % 64 == 0 and C <= 1536; B, H, W >= 1; every pointer 16-byte aligned. */
+int udb_dwconv7_ln_e4m3(const void* x, const float* w, const float* bias, const float* ln_w, const float* ln_b, void* out,
+                        float* out_scale, int32_t B, int32_t H, int32_t W, int32_t C, void* stream);
 
 /* dst = first ? src : max(dst, src) element-wise over n f16 values (decoder.py:371-374 max_stack over a stage's blocks). */
 int udb_max_accum_f16(const void* src, void* dst, int64_t n, int32_t first, void* stream);
@@ -649,6 +657,13 @@ int udb_v1_create(const udb_v1_config_t* cfg, udb_engine_v1** out);
 void udb_v1_destroy(udb_engine_v1* e);
 int udb_v1_set_weight(udb_engine_v1* e, const char* name, const void* dev_ptr, const int64_t* shape, int32_t ndim,
                       int32_t dtype);
+/* Host scalars of the packed V1 model (the three output-head biases) and the encoder mode "precision": 0 (or absent) = f16
+ * operands, 2 = FP8 E4M3 operands for the two MLP linear layers of the ConvNeXt encoder blocks of the stages the schedule
+ * runs in e4m3 (engine_v1.cu kFp8Stage; none at present, as none is faster that way) (s{i}.b{j}.w1_8 [4C, C],
+ * w2_8 [C, 4C] UDB_DT_E4M3 with f32 per-output-channel scales w1_8s / w2_8s; udb_dwconv7_ln_e4m3 and
+ * udb_quantize_rows_e4m3 quantise the activations per row) or for the four linear layers of every DINOv2 block (the
+ * blocks.{i}.*_w8 operands of the V2 engine's fp8 mode).  The stem, downsample layers, attention and the decoder stay
+ * f16 in both. */
 int udb_v1_set_scalar(udb_engine_v1* e, const char* name, double value);
 /* Shape arithmetic of one V1 call, the engine's own copy of `_shapes` / `_paddings` (unidepthv1.py:30-46): the image is resized
  * by `ratio` to (resized_h, resized_w) -- the larger side-ratio that still fits the fixed network input -- and zero-padded

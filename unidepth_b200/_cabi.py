@@ -256,6 +256,7 @@ EXPORTS = {
     "udb_v1_preprocess": (i32, [C.POINTER(V1Preprocess), vp]),
     "udb_layernorm_any": (i32, [C.POINTER(LayerNormAny), vp]),
     "udb_dwconv7_nhwc_f16": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, vp]),
+    "udb_dwconv7_ln_e4m3": (i32, [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]),
     "udb_max_accum_f16": (i32, [vp, vp, i64, i32, vp]),
     "udb_spatial_mean_f32": (i32, [vp, vp, i32, i32, i32, vp]),
     "udb_vit_tap": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),

@@ -1,8 +1,6 @@
 // HBM-bound / latency-bound kernels of the UniDepthV2.infer() path: LayerNorm, preprocessing +
 // patch extraction, position-embedding resize, the fp32 camera head, ray embedding, bilinear
 // resamplers and the output assembly.  Reference call sites are cited in include/udb.h.
-#include <cuda_fp8.h>
-
 #include "common.h"
 #include "ptx.cuh"
 
@@ -18,40 +16,6 @@ __device__ __forceinline__ float warp_max(float v) {
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
-
-// ------------------------------------------------------------------------------------ e4m3 quantisation
-// x rounded to nearest even at e4m3's precision, in f32 (|x| <= 464): 3 mantissa bits above 2^-6, multiples of 2^-9
-// below.  The e4m3x2 conversion that follows is then exact, so every byte is the round-to-nearest-even value of torch's
-// float8_e4m3fn cast by construction, whatever rounding the conversion instruction itself applies.
-__device__ __forceinline__ float round_e4m3(float x) {
-  const float a = fabsf(x);
-  float r;
-  if (a < 0.015625f) {
-    r = __fsub_rn(__fadd_rn(a, 24576.f), 24576.f);   // 24576 = 1.5 * 2^14: its ulp is 2^-9
-  } else {
-    const uint32_t u = __float_as_uint(a);
-    r = __uint_as_float((u + 0x7FFFFu + ((u >> 20) & 1u)) & 0xFFF00000u);
-  }
-  return copysignf(r, x);
-}
-
-// A row of e4m3 operands is q = e4m3(x * (448 / amax)) with the dequantisation scale s = amax / 448 (448 = the largest
-// finite e4m3 value); an all-zero row gets multiplier and scale 1.  Both are correctly rounded f32 divisions, so a host
-// model (torch: 448 / amax, x * inv, .to(float8_e4m3fn), amax / 448) reproduces every byte and scale.
-struct E4m3Row {
-  float inv, scale;
-  __device__ __forceinline__ explicit E4m3Row(float amax)
-      : inv(amax > 0.f ? 448.f / amax : 1.f), scale(amax > 0.f ? amax / 448.f : 1.f) {}
-  // four values, round to nearest even; |x * inv| exceeds 448 at most by the product's rounding, which round_e4m3
-  // brings back to 448 (torch's cast agrees there: it rounds everything below 464 to at most 448)
-  __device__ __forceinline__ uint32_t q4(float a, float b, float c, float d) const {
-    const auto q = [&](float x, float y) {
-      return (uint32_t)__nv_cvt_float2_to_fp8x2(make_float2(round_e4m3(__fmul_rn(x, inv)), round_e4m3(__fmul_rn(y, inv))),
-                                                __NV_SATFINITE, __NV_E4M3);
-    };
-    return q(a, b) | (q(c, d) << 16);
-  }
-};
 
 // ------------------------------------------------------------------------------------ LayerNorm
 // One warp per R rows (R = 1 by default; the R = 2 variant -- both rows' loads in flight before the first
@@ -704,7 +668,10 @@ __global__ void __launch_bounds__(256) postprocess_bicubic_kernel(const udb_post
 }
 
 // f16 rows -> e4m3 rows + row scales (udb_quantize_rows_e4m3): one warp per row, lane holds 16-byte chunks
-// lane + 32 i (i < 16: up to 4096 columns) in registers between the amax reduction and the conversion
+// lane + 32 i (i < NCH: up to NCH * 256 columns) in registers between the amax reduction and the conversion.  NCH = 16
+// serves up to 4096 columns (the DINOv2 MLP), NCH = 24 up to 6144 (ConvNeXt-L stage 3's 4 x 1536); the amax is a max,
+// so both give the same bytes where both apply.
+template <int NCH>
 __global__ void __launch_bounds__(256) quantize_rows_e4m3_kernel(const __half* __restrict__ in, long long ld_in,
                                                                  uint8_t* __restrict__ out, long long ld_out,
                                                                  float* __restrict__ scale, int rows, int cols) {
@@ -713,10 +680,10 @@ __global__ void __launch_bounds__(256) quantize_rows_e4m3_kernel(const __half* _
   if (row >= rows) return;
   const int nch = cols >> 3;
   const uint4* ip = reinterpret_cast<const uint4*>(in + (long long)row * ld_in);
-  uint4 v[16];
+  uint4 v[NCH];
   __half2 am2 = __float2half2_rn(0.f);
 #pragma unroll
-  for (int i = 0; i < 16; ++i) {
+  for (int i = 0; i < NCH; ++i) {
     const int c = lane + 32 * i;
     if (c < nch) {
       v[i] = ip[c];
@@ -729,7 +696,7 @@ __global__ void __launch_bounds__(256) quantize_rows_e4m3_kernel(const __half* _
   if (lane == 0) scale[row] = q.scale;
   uint2* op = reinterpret_cast<uint2*>(out + (long long)row * ld_out);
 #pragma unroll
-  for (int i = 0; i < 16; ++i) {
+  for (int i = 0; i < NCH; ++i) {
     const int c = lane + 32 * i;
     if (c < nch) {
       const __half2* h = reinterpret_cast<const __half2*>(&v[i]);
@@ -813,8 +780,8 @@ extern "C" int udb_layernorm(const udb_layernorm_t* p, void* stream) {
 
 extern "C" int udb_quantize_rows_e4m3(const void* in, int64_t ld_in, void* out, int64_t ld_out, float* scale, int32_t rows,
                                       int32_t cols, void* stream) {
-  if (!in || !out || !scale || rows < 0 || cols < 8 || cols > 4096 || cols % 8) {
-    set_error("udb_quantize_rows_e4m3: bad arguments (rows %d, cols %d: need a multiple of 8 in [8, 4096])", rows, cols);
+  if (!in || !out || !scale || rows < 0 || cols < 8 || cols > 6144 || cols % 8) {
+    set_error("udb_quantize_rows_e4m3: bad arguments (rows %d, cols %d: need a multiple of 8 in [8, 6144])", rows, cols);
     return 1;
   }
   if (ld_in < cols || ld_in % 8 || ld_out < cols || ld_out % 8 || (reinterpret_cast<uintptr_t>(in) & 15) ||
@@ -825,8 +792,9 @@ extern "C" int udb_quantize_rows_e4m3(const void* in, int64_t ld_in, void* out, 
   }
   note_work(0.0, (double)rows * cols * (2 + 1) + 4.0 * rows);
   if (rows == 0) return 0;
-  quantize_rows_e4m3_kernel<<<(rows + 7) / 8, 256, 0, ST(stream)>>>(static_cast<const __half*>(in), ld_in, static_cast<uint8_t*>(out),
-                                                                    ld_out, scale, rows, cols);
+  const auto kernel = cols <= 4096 ? quantize_rows_e4m3_kernel<16> : quantize_rows_e4m3_kernel<24>;
+  kernel<<<(rows + 7) / 8, 256, 0, ST(stream)>>>(static_cast<const __half*>(in), ld_in, static_cast<uint8_t*>(out), ld_out, scale,
+                                                 rows, cols);
   return check_launch("quantize_rows_e4m3_kernel");
 }
 

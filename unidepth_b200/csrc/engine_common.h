@@ -152,6 +152,15 @@ struct Ctx {
     }
   }
 
+  // registered operand must hold e4m3 bytes (f16 bytes would be read as e4m3 pairs)
+  void expect_e4m3(const std::string& name) {
+    const Weight* w = W(name);
+    if (!rc && w->dtype != UDB_DT_E4M3) {
+      set_error("engine: packed tensor '%s' has dtype %d, expected e4m3 (%d)", name.c_str(), w->dtype, UDB_DT_E4M3);
+      rc = 1;
+    }
+  }
+
   // out[row(m), :] = resid + gamma * act(a @ w^T + bias)     (ops.gemm)
   struct G {
     const void* a; const void* w; int M, N, K; int lda = 0, ldw = 0;
@@ -303,7 +312,7 @@ static inline std::string shape_name(int B, int H, int W) {
 }
 
 // ------------------------------------------------------------------------------------------ DINOv2 blocks
-// Shape and packing mode of the DINOv2 block loop (UniDepthV2 uses every mode; UniDepthV1 ViT-L the default f16 one).
+// Shape and packing mode of the DINOv2 block loop (UniDepthV2 uses every mode; UniDepthV1 ViT-L the f16 and e4m3 ones).
 struct VitBlocks {
   int B, T, D, heads, depth;
   bool split = false;          // split-f16 precise mode: operands are [hi | lo] pairs, weights [N, 3K] = [hi | hi | lo]
@@ -324,13 +333,7 @@ static inline void vit_block_e4m3(Ctx& c, const std::string& b, float* x, const 
   c.expect2(b + "proj_w8", D, D);
   c.expect2(b + "fc1_w8", 4 * D, D);
   c.expect2(b + "fc2_w8", D, 4 * D);
-  for (const char* n : {"qkv_w8", "proj_w8", "fc1_w8", "fc2_w8"}) {   // f16 bytes would be read as e4m3 pairs
-    const Weight* w = c.W(b + n);
-    if (!c.rc && w->dtype != UDB_DT_E4M3) {
-      set_error("engine: packed tensor '%s' has dtype %d, expected e4m3 (%d)", (b + n).c_str(), w->dtype, UDB_DT_E4M3);
-      c.rc = 1;
-    }
-  }
+  for (const char* n : {"qkv_w8", "proj_w8", "fc1_w8", "fc2_w8"}) c.expect_e4m3(b + n);
   c.layernorm_e4m3(x, q8, qs, c.F(b + "n1w"), c.F(b + "n1b"), BT, D, 1e-6f);
   { Ctx::G q{q8, c.W(b + "qkv_w8")->p, BT, 3 * D, D}; q.a_scale = qs; q.w_scale = c.F(b + "qkv_w8s");
     q.bias = c.F(b + "qkv_b"); q.out = qkv; c.gemm(q); }

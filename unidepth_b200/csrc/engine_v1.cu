@@ -76,6 +76,43 @@ static void cvnxt_block(Ctx& c, const std::string& p, float* x, __half* x16, int
   ar.release(m);
 }
 
+// Encoder stages whose ConvNeXt blocks run in e4m3 mode (precision 2); the others keep the f16 block.  A fixed rule of the
+// schedule: a stage runs e4m3 only where its profiled block time is below the f16 block's.  On an H100 none is (DESIGN.md
+// section 8): in stages 0 and 1 the e4m3 MLP GEMMs save less than the GELU row quantiser costs, and in stages 2 and 3 the
+// GEMMs' saving is outweighed by that quantiser plus udb_dwconv7_ln_e4m3, which takes longer than the f16 depthwise
+// conv and LayerNorm together.  So ConvNeXt-L runs its f16 blocks in both modes.  unidepthv1.py FP8_STAGES packs the
+// same set.
+static constexpr bool kFp8Stage[4] = {false, false, false, false};
+
+// The same block in e4m3 mode: udb_dwconv7_ln_e4m3 writes fc1's e4m3 operand and row scales, the GELU output is quantised
+// per row for fc2, and both GEMMs read e4m3 weights with one scale per output channel; the epilogues are those of the
+// f16 block.  Its scratch -- the two e4m3 operands (rows x C, then rows x 4C bytes, sharing one rows x 4C region), the
+// row scales (rows x 4 bytes) and the f16 GELU output -- is rows x 4 bytes more than the f16 block's y, hN and GELU output.
+static void cvnxt_block_e4m3(Ctx& c, const std::string& p, float* x, __half* x16, int B, int Hh, int Ww, int C) {
+  Arena& ar = *c.ar;
+  const size_t m = ar.mark();
+  const long long rows = static_cast<long long>(B) * Hh * Ww;
+  void* a8 = ar.alloc(rows * 4 * C);
+  float* as = ar.f(rows);
+  __half* md = ar.h(rows * 4 * C);
+  c.expect2(p + "w1_8", 4 * C, C);
+  c.expect2(p + "w2_8", C, 4 * C);
+  c.expect_e4m3(p + "w1_8");
+  c.expect_e4m3(p + "w2_8");
+  const float* dw_w = c.F(p + "dw_w");
+  const float* dw_b = c.F(p + "dw_b");
+  const float* ln_w = c.F(p + "ln_w");
+  const float* ln_b = c.F(p + "ln_b");
+  c.launch([&] { return udb_dwconv7_ln_e4m3(x16, dw_w, dw_b, ln_w, ln_b, a8, as, B, Hh, Ww, C, c.st); });
+  { Ctx::G q{a8, c.W(p + "w1_8")->p, static_cast<int>(rows), 4 * C, C}; q.a_scale = as; q.w_scale = c.F(p + "w1_8s");
+    q.bias = c.F(p + "b1"); q.act = UDB_ACT_GELU; q.out = md; c.gemm(q); }
+  c.quantize_e4m3(md, 4 * C, a8, as, static_cast<int>(rows), 4 * C);
+  { Ctx::G q{a8, c.W(p + "w2_8")->p, static_cast<int>(rows), C, 4 * C}; q.a_scale = as; q.w_scale = c.F(p + "w2_8s");
+    q.bias = c.F(p + "b2"); q.gamma = c.F(p + "gamma"); q.resid = x; q.resid_f32 = 1; q.out = x; q.out_f32 = 1; q.out2 = x16;
+    q.out2_leaky = 0; c.gemm(q); }
+  ar.release(m);
+}
+
 // pre-processing of the input batch into the encoder's patch rows (unidepthv1.py _preprocess): 4x4 im2col rows of the
 // ConvNeXt stem (`patch` 0) or 14x14 DINOv2 patch rows (`patch` 14)
 static void preprocess(Ctx& c, const udb_v1_config_t& cf, const udb_infer_v1_args_t& a, const V1Geom& g, __half* patches,
@@ -199,7 +236,7 @@ static void conv_upsample(Ctx& c, const std::string& p, const float* lat, const 
 // tap kernel folds (patch tokens + cls token) into the running max of its slice (levels[s], decoder.py:371-379; slice s
 // holds cf.depths[s] blocks) and copies the raw cls rows of the last four blocks into clsbuf[k] (block last - k).
 static void dino_encoder(Ctx& c, const udb_v1_config_t& cf, const udb_infer_v1_args_t& a, const V1Geom& g, int gh, int gw,
-                         __half* const* levels, float* const* clsbuf) {
+                         __half* const* levels, float* const* clsbuf, bool fp8) {
   Arena& ar = *c.ar;
   const int B = a.B, D = cf.dims[0], N = gh * gw, T = N + 1;
   const size_t BN = static_cast<size_t>(B) * N, BT = static_cast<size_t>(B) * T;
@@ -221,6 +258,7 @@ static void dino_encoder(Ctx& c, const udb_v1_config_t& cf, const udb_infer_v1_a
     c.launch([&] { return udb_set_cls_rows(x, cls, pos, B, T, D, c.st); });
   }
   VitBlocks v{B, T, D, D / 64, depth};
+  v.fp8 = fp8;
   int slice = 0, start = 0;
   vit_blocks(c, "blocks.", x, v, [&](int i) {
     if (i == start + cf.depths[slice]) { start = i; ++slice; }
@@ -244,6 +282,11 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
     for (int i = 1; i < 4; ++i) { sh[i] = sh[i - 1] / 2; sw[i] = sw[i - 1] / 2; }
   }
   Stage stage;
+  // "precision": 0 (absent) = f16 operands, 2 = e4m3 operands for the encoder blocks' MLP (ConvNeXt) or all four linear
+  // layers (DINOv2); the stem, downsample layers and the decoder are the same in both
+  const double prec = e->scalars.count("precision") ? e->scalars["precision"] : 0.0;
+  if (prec != 0.0 && prec != 2.0) { set_error("udb_infer_v1: precision %g unsupported (0 f16, 2 e4m3)", prec); return 1; }
+  const bool f8 = prec == 2.0;
 
   // ---- pre-processing + stem (convnext.py:371-383: conv k4 s4 as an im2col GEMM, then LayerNorm2d)
   stage.next("udb_v1:preprocess+stem");
@@ -263,7 +306,7 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
   for (int k = 0; k < 4; ++k) clsbuf[k] = ar.f(static_cast<size_t>(B) * cls_dim[k]);     // clsbuf[k]: block (last - k)
   if (dino) {
     stage.next("udb_v1:dinov2_encoder");
-    dino_encoder(c, cf, a, g, sh[0], sw[0], levels, clsbuf);
+    dino_encoder(c, cf, a, g, sh[0], sw[0], levels, clsbuf, f8);
   } else {
     const size_t enc_mark = ar.mark();
     const long long n0 = static_cast<long long>(B) * sh[0] * sw[0];
@@ -298,7 +341,8 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
         x16 = xn16;
       }
       for (int j = 0; j < cf.depths[i]; ++j, ++blk) {
-        cvnxt_block(c, idx2("s%d.b%d.", i, j), x, x16, B, sh[i], sw[i], C, 1e-6f);
+        if (f8 && kFp8Stage[i]) cvnxt_block_e4m3(c, idx2("s%d.b%d.", i, j), x, x16, B, sh[i], sw[i], C);
+        else cvnxt_block(c, idx2("s%d.b%d.", i, j), x, x16, B, sh[i], sw[i], C, 1e-6f);
         c.launch([&] { return udb_max_accum_f16(x16, levels[i], n * C, j == 0, st); });
         const int from_end = total_blocks - 1 - blk;
         if (from_end < 4) c.launch([&] { return udb_spatial_mean_f32(x, clsbuf[from_end], B, sh[i] * sw[i], C, st); });

@@ -3,6 +3,7 @@
 // Compile with -gencode arch=compute_90a,code=sm_90a.
 #pragma once
 #include <cuda_fp16.h>
+#include <cuda_fp8.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -334,5 +335,39 @@ __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
   __half2 h = __floats2half2_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&h);
 }
+
+// ----------------------------------------------------------------------------- e4m3 quantisation
+// x rounded to nearest even at e4m3's precision, in f32 (|x| <= 464): 3 mantissa bits above 2^-6, multiples of 2^-9
+// below.  The e4m3x2 conversion that follows is then exact, so every byte is the round-to-nearest-even value of torch's
+// float8_e4m3fn cast by construction, whatever rounding the conversion instruction itself applies.
+__device__ __forceinline__ float round_e4m3(float x) {
+  const float a = fabsf(x);
+  float r;
+  if (a < 0.015625f) {
+    r = __fsub_rn(__fadd_rn(a, 24576.f), 24576.f);   // 24576 = 1.5 * 2^14: its ulp is 2^-9
+  } else {
+    const uint32_t u = __float_as_uint(a);
+    r = __uint_as_float((u + 0x7FFFFu + ((u >> 20) & 1u)) & 0xFFF00000u);
+  }
+  return copysignf(r, x);
+}
+
+// A row of e4m3 operands is q = e4m3(x * (448 / amax)) with the dequantisation scale s = amax / 448 (448 = the largest
+// finite e4m3 value); an all-zero row gets multiplier and scale 1.  Both are correctly rounded f32 divisions, so a host
+// model (torch: 448 / amax, x * inv, .to(float8_e4m3fn), amax / 448) reproduces every byte and scale.
+struct E4m3Row {
+  float inv, scale;
+  __device__ __forceinline__ explicit E4m3Row(float amax)
+      : inv(amax > 0.f ? 448.f / amax : 1.f), scale(amax > 0.f ? amax / 448.f : 1.f) {}
+  // four values, round to nearest even; |x * inv| exceeds 448 at most by the product's rounding, which round_e4m3
+  // brings back to 448 (torch's cast agrees there: it rounds everything below 464 to at most 448)
+  __device__ __forceinline__ uint32_t q4(float a, float b, float c, float d) const {
+    const auto q = [&](float x, float y) {
+      return (uint32_t)__nv_cvt_float2_to_fp8x2(make_float2(round_e4m3(__fmul_rn(x, inv)), round_e4m3(__fmul_rn(y, inv))),
+                                                __NV_SATFINITE, __NV_E4M3);
+    };
+    return q(a, b) | (q(c, d) << 16);
+  }
+};
 
 }  // namespace udb

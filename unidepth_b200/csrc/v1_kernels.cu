@@ -4,6 +4,7 @@
 // LayerNorm embedding, the small dense-attention pieces (row softmax, 4-query cross attention, Nystrom landmarks /
 // pseudo-inverse matmuls), single-output 3x3 convolutions and the V1 pre / post-processing.  All HBM- or
 // latency-bound CUDA-core work; the GEMM-shaped parts of V1 run on the wgmma kernels of gemm.cu / attention.cu.
+#include <cooperative_groups.h>
 #include <math.h>
 
 #include "common.h"
@@ -260,6 +261,187 @@ __global__ void __launch_bounds__(256) dwconv7_kernel(const __half* __restrict__
       }
     }
   }
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// ConvNeXt block head in e4m3 mode (udb_dwconv7_ln_e4m3): depthwise 7x7 -> f16 -> LayerNorm (eps 1e-6) -> e4m3 rows +
+// row scales, the A operand of the fc1 GEMM.  LayerNorm needs a pixel's whole channel row, so a CLUSTER of K blocks owns
+// a 128-pixel tile (TW x 128/TW, as dwconv7_kernel) across all channels: block k of the cluster takes the 64-channel
+// chunks k, k + K, ... (at most 3; K = ceil(C / 192), up to 8 for C = 1536), which bounds its shared memory whatever C
+// is.  Each chunk is convolved exactly as dwconv7_kernel does it (halo in shared memory, 8 consecutive x x 4 channels
+// per thread, the same f32 FMA order) and its f16 outputs stay in the block's shared memory.  The per-pixel sum, sum of
+// squared deviations and amax are each reduced over the cluster through distributed shared memory, in rank order, so
+// the result does not depend on scheduling; then every block writes its channels of each row quantised.
+// ------------------------------------------------------------------------------------------------------------------
+constexpr int DWL_PX = 128;
+constexpr int DWL_HALO_BYTES = 14 * 22 * DW_PS * 2;                 // one 64-channel chunk of the halo (either tile shape)
+constexpr int DWL_CPB = 3;                                          // 64-channel chunks per block at most
+constexpr int DWL_MAXC = 1536;
+constexpr int DWL_YS_LD = DWL_CPB * DW_CB + 8;                      // f16 conv outputs [128 px][this block's channels]
+constexpr int DWL_SMEM = DWL_HALO_BYTES + DWL_PX * DWL_YS_LD * 2 + 3 * DWL_PX * 4;
+
+template <int TW>
+__global__ void __launch_bounds__(256) dwconv7_ln_e4m3_kernel(const __half* __restrict__ x, const float* __restrict__ w,
+                                                             const float* __restrict__ bias, const float* __restrict__ ln_w,
+                                                             const float* __restrict__ ln_b, uint8_t* __restrict__ out,
+                                                             float* __restrict__ out_scale, int H, int W, int C, int tiles_x) {
+  constexpr int TH = DWL_PX / TW, HH = TH + 6, HW = TW + 6;
+  extern __shared__ __align__(16) unsigned char dwl_smem[];
+  __half* tile = reinterpret_cast<__half*>(dwl_smem);
+  __half* ys = reinterpret_cast<__half*>(dwl_smem + DWL_HALO_BYTES);
+  float (*part)[DWL_PX] = reinterpret_cast<float (*)[DWL_PX]>(dwl_smem + DWL_HALO_BYTES + DWL_PX * DWL_YS_LD * 2);   // sum / squares / amax
+  namespace cgr = cooperative_groups;
+  cgr::cluster_group cluster = cgr::this_cluster();
+  const int K = (int)cluster.num_blocks(), rank = (int)cluster.block_rank();
+  const int t = blockIdx.x / K;
+  const int tx0 = (t % tiles_x) * TW, ty0 = (t / tiles_x) * TH, b = blockIdx.y;
+  const __half* xb = x + (long long)b * H * W * C;
+  const int cg = threadIdx.x & 15, pg = threadIdx.x >> 4;
+  const int r = TW == 16 ? (pg >> 1) : pg, xh = TW == 16 ? (pg & 1) * 8 : 0;   // each thread: 8 consecutive x, 4 channels
+  pdl_wait();                                      // x16 is written by the previous block's fc2 GEMM
+  int nloc = 0;
+  for (int c0 = rank * DW_CB; c0 < C; c0 += K * DW_CB, ++nloc) {
+    if (nloc) __syncthreads();                     // the previous chunk's halo is no longer read
+    for (int i = threadIdx.x; i < HH * HW * (DW_CB / 8); i += 256) {
+      const int ch = i & 7, pix = i >> 3;
+      const int hy = pix / HW, hx = pix - hy * HW;
+      const int gy = ty0 + hy - 3, gx = tx0 + hx - 3;
+      uint4 v = make_uint4(0u, 0u, 0u, 0u);
+      if (gy >= 0 && gy < H && gx >= 0 && gx < W) v = __ldg(reinterpret_cast<const uint4*>(xb + ((long long)gy * W + gx) * C + c0 + ch * 8));
+      uint2* d = reinterpret_cast<uint2*>(tile + pix * DW_PS + ch * 8);
+      d[0] = make_uint2(v.x, v.y);
+      d[1] = make_uint2(v.z, v.w);
+    }
+    __syncthreads();
+    uint64_t acc[8][2];
+    {
+      const float4 bv = __ldg(reinterpret_cast<const float4*>(bias + c0 + cg * 4));
+#pragma unroll
+      for (int i = 0; i < 8; ++i) { acc[i][0] = pack2(bv.x, bv.y); acc[i][1] = pack2(bv.z, bv.w); }
+    }
+#pragma unroll 1
+    for (int dy = 0; dy < 7; ++dy) {
+      uint64_t in[14][2];
+#pragma unroll
+      for (int i = 0; i < 14; ++i) {
+        const uint2 u = *reinterpret_cast<const uint2*>(tile + ((r + dy) * HW + xh + i) * DW_PS + cg * 4);
+        const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&u.x));
+        const float2 c = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
+        in[i][0] = pack2(a.x, a.y);
+        in[i][1] = pack2(c.x, c.y);
+      }
+#pragma unroll
+      for (int dx = 0; dx < 7; ++dx) {
+        const float4 wv = __ldg(reinterpret_cast<const float4*>(w + (long long)(dy * 7 + dx) * C + c0 + cg * 4));
+        const uint64_t w0 = pack2(wv.x, wv.y), w1 = pack2(wv.z, wv.w);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          acc[i][0] = fma2(in[i + dx][0], w0, acc[i][0]);
+          acc[i][1] = fma2(in[i + dx][1], w1, acc[i][1]);
+        }
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      float a0, a1, a2, a3;
+      unpack2(acc[i][0], a0, a1);
+      unpack2(acc[i][1], a2, a3);
+      *reinterpret_cast<uint2*>(ys + (r * TW + xh + i) * DWL_YS_LD + nloc * DW_CB + cg * 4) =
+          make_uint2(pack_half2(a0, a1), pack_half2(a2, a3));
+    }
+  }
+  __syncthreads();
+  // LayerNorm + quantisation: warp per pixel; lane l holds 8 channels of local chunk l / 8 (global chunk rank + K * (l / 8))
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const bool mine = lane < nloc * 8;
+  const int col = (rank + K * (lane >> 3)) * DW_CB + (lane & 7) * 8;
+  const auto load = [&](int p, float (&f)[8]) {
+    const uint4 u = mine ? *reinterpret_cast<const uint4*>(ys + p * DWL_YS_LD + lane * 8) : make_uint4(0u, 0u, 0u, 0u);
+    const __half2* h = reinterpret_cast<const __half2*>(&u);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) { const float2 v = __half22float2(h[k]); f[2 * k] = v.x; f[2 * k + 1] = v.y; }
+  };
+  // a pixel's value over the cluster's blocks: lane k < K reads block k's partial (one distributed-shared-memory load per
+  // lane, not K dependent ones per lane), then every lane combines them in rank order, so the result does not depend on
+  // scheduling
+  const auto gather = [&](int which, int p) { return lane < K ? cluster.map_shared_rank(&part[which][0], lane)[p] : 0.f; };
+  const auto total = [&](int which, int p) {
+    const float g = gather(which, p);
+    float v = 0.f;
+    for (int k = 0; k < K; ++k) v += __shfl_sync(0xffffffffu, g, k);
+    return v;
+  };
+  const auto total_max = [&](int p) {
+    const float g = gather(2, p);
+    float v = 0.f;
+    for (int k = 0; k < K; ++k) v = fmaxf(v, __shfl_sync(0xffffffffu, g, k));
+    return v;
+  };
+  for (int p = warp; p < DWL_PX; p += 8) {
+    float f[8];
+    load(p, f);
+    float s = 0.f;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) s += f[k];
+    s = wsum(mine ? s : 0.f);
+    if (lane == 0) part[0][p] = s;
+  }
+  cluster.sync();
+  float mean[DWL_PX / 8];
+  #pragma unroll
+  for (int i = 0; i < DWL_PX / 8; ++i) {
+    const int p = warp + 8 * i;
+    float f[8];
+    load(p, f);
+    mean[i] = total(0, p) / (float)C;
+    float q = 0.f;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) q += (f[k] - mean[i]) * (f[k] - mean[i]);
+    q = wsum(mine ? q : 0.f);
+    if (lane == 0) part[1][p] = q;
+  }
+  cluster.sync();
+  float wk[8], bk[8];
+  if (mine) {
+    const float4 w0 = __ldg(reinterpret_cast<const float4*>(ln_w + col)), w1 = __ldg(reinterpret_cast<const float4*>(ln_w + col + 4));
+    const float4 b0 = __ldg(reinterpret_cast<const float4*>(ln_b + col)), b1 = __ldg(reinterpret_cast<const float4*>(ln_b + col + 4));
+    wk[0] = w0.x; wk[1] = w0.y; wk[2] = w0.z; wk[3] = w0.w; wk[4] = w1.x; wk[5] = w1.y; wk[6] = w1.z; wk[7] = w1.w;
+    bk[0] = b0.x; bk[1] = b0.y; bk[2] = b0.z; bk[3] = b0.w; bk[4] = b1.x; bk[5] = b1.y; bk[6] = b1.z; bk[7] = b1.w;
+  }
+  float rstd[DWL_PX / 8];
+  #pragma unroll
+  for (int i = 0; i < DWL_PX / 8; ++i) {
+    const int p = warp + 8 * i;
+    float f[8];
+    load(p, f);
+    rstd[i] = rsqrtf(total(1, p) / (float)C + 1e-6f);
+    float am = 0.f;
+    if (mine) {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) am = fmaxf(am, fabsf((f[k] - mean[i]) * rstd[i] * wk[k] + bk[k]));
+    }
+    am = wmax(am);
+    if (lane == 0) part[2][p] = am;
+  }
+  cluster.sync();
+  #pragma unroll
+  for (int i = 0; i < DWL_PX / 8; ++i) {
+    const int p = warp + 8 * i;
+    const int gy = ty0 + p / TW, gx = tx0 + p % TW;
+    if (gy >= H || gx >= W) continue;              // outside the map: computed for the statistics' shape only
+    const E4m3Row e(total_max(p));
+    const long long row = ((long long)b * H + gy) * W + gx;
+    if (rank == 0 && lane == 0) out_scale[row] = e.scale;
+    if (mine) {
+      float f[8];
+      load(p, f);
+      float y[8];
+#pragma unroll
+      for (int k = 0; k < 8; ++k) y[k] = (f[k] - mean[i]) * rstd[i] * wk[k] + bk[k];    // the expression of the amax pass
+      *reinterpret_cast<uint2*>(out + row * C + col) = make_uint2(e.q4(y[0], y[1], y[2], y[3]), e.q4(y[4], y[5], y[6], y[7]));
+    }
+  }
+  cluster.sync();                                  // no block leaves while another still reads its partials
 }
 
 // running element-wise maximum over a stage's block outputs (decoder.py:371-374 `max_stack`): dst = first ? src : max(dst, src)
@@ -915,6 +1097,39 @@ int udb_dwconv7_nhwc_f16(const void* x, const float* w, const float* bias, void*
     dwconv7_kernel<8><<<dim3(tx * ty, C / DW_CB, B), 256, 0, ST(stream)>>>(xh, w, bias, yh, H, W, C, tx);
   }
   return check_launch("dwconv7_kernel");
+}
+
+int udb_dwconv7_ln_e4m3(const void* x, const float* w, const float* bias, const float* ln_w, const float* ln_b, void* out,
+                        float* out_scale, int32_t B, int32_t H, int32_t W, int32_t C, void* stream) {
+  if (C <= 0 || C % DW_CB || C > DWL_MAXC) { set_error("udb_dwconv7_ln_e4m3: C=%d must be a multiple of 64 up to 1536", C); return 1; }
+  const struct { int v; const char* name; } dims[] = {{B, "B"}, {H, "H"}, {W, "W"}};
+  for (const auto& d : dims)
+    if (d.v < 1) { set_error("udb_dwconv7_ln_e4m3: %s=%d must be >= 1", d.name, d.v); return 1; }
+  const struct { const void* p; const char* name; } ptrs[] = {{x, "x"}, {w, "w"}, {bias, "bias"}, {ln_w, "ln_w"}, {ln_b, "ln_b"},
+                                                              {out, "out"}, {out_scale, "out_scale"}};
+  for (const auto& a : ptrs)
+    if (!a.p || (reinterpret_cast<uintptr_t>(a.p) & 15)) {
+      set_error("udb_dwconv7_ln_e4m3: `%s` must be a non-null, 16-byte aligned device pointer", a.name);
+      return 1;
+    }
+  const int chunks = C / DW_CB, K = (chunks + DWL_CPB - 1) / DWL_CPB;     // cluster size: 1..8
+  static std::atomic<uint64_t> attr_mask{0};
+  if (first_on_device(attr_mask)) {
+    for (auto kern : {dwconv7_ln_e4m3_kernel<16>, dwconv7_ln_e4m3_kernel<8>}) {
+      const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, DWL_SMEM);
+      if (e != cudaSuccess) { set_error("udb_dwconv7_ln_e4m3: cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return 1; }
+    }
+  }
+  const double px = (double)B * H * W;
+  note_work(2.0 * 49 * px * C + 8.0 * px * C, px * C * (2 + 1) + 4.0 * px);
+  // 16x8 or 8x16 (W x H) pixel tiles: whichever pads the map less (as udb_dwconv7_nhwc_f16)
+  const long long area16 = (long long)((W + 15) / 16) * ((H + 7) / 8), area8 = (long long)((W + 7) / 8) * ((H + 15) / 16);
+  const int tw = area16 <= area8 ? 16 : 8, tx = (W + tw - 1) / tw, ty = (H + DWL_PX / tw - 1) / (DWL_PX / tw);
+  const cudaError_t e = launch_ex(tw == 16 ? dwconv7_ln_e4m3_kernel<16> : dwconv7_ln_e4m3_kernel<8>, dim3(tx * ty * K, B), dim3(256),
+                                  DWL_SMEM, ST(stream), K, reinterpret_cast<const __half*>(x), w, bias, ln_w, ln_b,
+                                  reinterpret_cast<uint8_t*>(out), out_scale, H, W, C, tx);
+  if (e != cudaSuccess) { set_error("dwconv7_ln_e4m3_kernel launch: %s", cudaGetErrorString(e)); return 1; }
+  return check_launch("dwconv7_ln_e4m3_kernel");
 }
 
 int udb_max_accum_f16(const void* src, void* dst, int64_t n, int32_t first, void* stream) {

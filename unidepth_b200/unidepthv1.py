@@ -29,7 +29,11 @@ from . import _cabi as cabi
 from .spec_v1 import (ENCODER_CONVNEXT, ENCODER_DINOV2, V1_INTERPOLATE_OFFSET, V1Spec, param_shapes, v1_paddings,
                       v1_shapes)
 from ._engine_model import HUB_KWARGS, EngineModel, PyTorchModelHubMixin, f16, f32
-from .unidepthv2 import pack_vit_encoder
+from .unidepthv2 import pack_e4m3, pack_vit_encoder
+
+# ConvNeXt stages whose blocks run on e4m3 operands in precision "fp8" (engine_v1.cu kFp8Stage, the same fixed rule: a
+# stage runs e4m3 only where that is measured faster, which on an H100 is none of them, DESIGN.md section 8)
+FP8_STAGES = (False, False, False, False)
 
 
 def _offset_pos_embed(pos: torch.Tensor, gh: int, gw: int, offset: float) -> torch.Tensor:
@@ -69,6 +73,16 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         self.spec = V1Spec(config)
         self._add_params(param_shapes(config))
         self.image_shape = list(self.spec.image_shape)        # unidepthv1.py:447
+        # "f16" (default) or "fp8": speed mode -- the linear layers of the encoder blocks multiply FP8 E4M3 operands on the
+        # e4m3 wgmma (include/udb.h udb_gemm_e4m3): weights with one scale per output channel, activations quantised per
+        # row on the fly.  DINOv2 ViT-L: qkv, proj, fc1 and fc2, as UniDepthV2's fp8 mode.  ConvNeXt: the two MLP layers of
+        # the blocks of the stages in FP8_STAGES, fed by a fused depthwise 7x7 + LayerNorm + quantisation kernel
+        # (udb_dwconv7_ln_e4m3) -- an empty set, since no stage is faster that way, so ConvNeXt-L computes what "f16" does.  The stem, downsample layers, attention and the decoder stay f16.  Its accuracy is only measured on
+        # seeded synthetic weights (tests/test_v1_fp8_gpu.py), not on trained checkpoints.
+        self.precision = "f16"
+
+    def _fingerprint(self):
+        return (self.precision,) + super()._fingerprint()
 
     # ------------------------------------------------------------------ weight packing
     def _pack_tensors(self, dev):
@@ -76,11 +90,15 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         product caller (CUDA device); tests/test_engine_schedule_cpu.py runs it on the CPU to check, through the engine's
         dry run, that the packer registers exactly the operands the C schedule asks for."""
         s = self.spec
+        if self.precision not in ("f16", "fp8"):
+            raise ValueError(f"precision must be 'f16' or 'fp8', not {self.precision!r}")
+        fp8 = self.precision == "fp8"
         sd = {k: v.detach() for k, v in self.state_dict().items()}
         h16 = lambda t: t.to(f16).contiguous()
         c32 = lambda t: t.to(f32).contiguous()
         T: Dict[str, torch.Tensor] = {}
-        S: Dict[str, float] = {}
+        # an engine without "precision" runs the f16 mode, so the f16 packing registers exactly the scalars it always has
+        S: Dict[str, float] = {"precision": 2.0} if fp8 else {}
         pe, pd = "pixel_encoder.", "pixel_decoder."
         hid = s.hidden
 
@@ -94,23 +112,28 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
             out[:t.shape[0]] = t
             return out
 
-        def block(dst, src, conv_names):
-            """ConvNeXt block operands: depthwise weights tap-major [49, C] f32, MLP weights f16."""
+        def block(dst, src, conv_names, e4m3=False):
+            """ConvNeXt block operands: depthwise weights tap-major [49, C] f32, MLP weights f16, or e4m3 with per-output-channel
+            scales (`w1_8` / `w1_8s`, `w2_8` / `w2_8s`; pack_e4m3) for a block of the fp8 mode."""
             dw, norm, fc1, fc2 = conv_names
             w = sd[f"{src}{dw}.weight"]
             T[dst + "dw_w"] = c32(w.reshape(w.shape[0], 49).t())
             T[dst + "dw_b"] = c32(sd[f"{src}{dw}.bias"])
             T[dst + "ln_w"], T[dst + "ln_b"] = c32(sd[f"{src}{norm}.weight"]), c32(sd[f"{src}{norm}.bias"])
-            T[dst + "w1"], T[dst + "b1"] = h16(sd[f"{src}{fc1}.weight"]), c32(sd[f"{src}{fc1}.bias"])
-            T[dst + "w2"], T[dst + "b2"] = h16(sd[f"{src}{fc2}.weight"]), c32(sd[f"{src}{fc2}.bias"])
+            T[dst + "b1"], T[dst + "b2"] = c32(sd[f"{src}{fc1}.bias"]), c32(sd[f"{src}{fc2}.bias"])
+            if e4m3:
+                T[dst + "w1_8"], T[dst + "w1_8s"] = pack_e4m3(sd[f"{src}{fc1}.weight"])
+                T[dst + "w2_8"], T[dst + "w2_8s"] = pack_e4m3(sd[f"{src}{fc2}.weight"])
+            else:
+                T[dst + "w1"], T[dst + "w2"] = h16(sd[f"{src}{fc1}.weight"]), h16(sd[f"{src}{fc2}.weight"])
             T[dst + "gamma"] = c32(sd[f"{src}gamma"])
 
         hc, wc = s.common_grid()
         # ---- encoder
         if s.encoder == ENCODER_DINOV2:
-            # default f16 packing of the V2 encoder; the final norm, mask token and register tokens are never read
+            # the V2 encoder's f16 or fp8 packing; the final norm, mask token and register tokens are never read
             # (use_norm=False, dinov2.py:173-178)
-            T.update(pack_vit_encoder(sd, s.embed_dim, s.enc_depth, dev))
+            T.update(pack_vit_encoder(sd, s.embed_dim, s.enc_depth, dev, fp8=fp8))
             T["pos"] = c32(_offset_pos_embed(T["pos"], hc, wc, V1_INTERPOLATE_OFFSET))
         for i, depth in enumerate(s.depths if s.encoder == ENCODER_CONVNEXT else ()):
             if i == 0:
@@ -123,7 +146,7 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
                 T[f"ds{i}.ln_w"], T[f"ds{i}.ln_b"] = c32(sd[st + "downsample.0.weight"]), c32(sd[st + "downsample.0.bias"])
                 T[f"ds{i}.w"], T[f"ds{i}.b"] = h16(w.permute(0, 2, 3, 1).reshape(w.shape[0], -1)), c32(sd[st + "downsample.1.bias"])
             for j in range(depth):
-                block(f"s{i}.b{j}.", f"{st}blocks.{j}.", ("conv_dw", "norm", "mlp.fc1", "mlp.fc2"))
+                block(f"s{i}.b{j}.", f"{st}blocks.{j}.", ("conv_dw", "norm", "mlp.fc1", "mlp.fc2"), fp8 and FP8_STAGES[i])
 
         # ---- decoder: adapters, embeddings
         for l in range(4):
