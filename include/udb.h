@@ -377,6 +377,10 @@ typedef struct udb_v1_preprocess_t {
   void* patches;
 } udb_v1_preprocess_t;
 int udb_v1_preprocess(const udb_v1_preprocess_t* p, void* stream);
+/* The same rows as split-f16 operands (UniDepthV1 precision "split"; udb_gemm_t.a_split_k): each row holds
+ * [hi | lo], 2 x 64 (stem) or 2 x 640 (patch == 14) columns, hi = f16(v) -- bit for bit what udb_v1_preprocess
+ * writes -- and lo = f16(v - f32(hi)). */
+int udb_v1_preprocess_split(const udb_v1_preprocess_t* p, void* stream);
 
 /* DINOv2 block output -> UniDepthV1 decoder level (unidepthv1.py:322-326 adds each block's cls token to its patch tokens;
  * decoder.py:371-379 takes the max over a slice of blocks).  x f32 [B, 1+N, D] (cls row first):
@@ -384,12 +388,18 @@ int udb_v1_preprocess(const udb_v1_preprocess_t* p, void* stream);
  * f16 round-to-nearest is monotone, so the running max kept in f16 equals f16 of the f32 max.  cls_out (may be NULL)
  * [B, D] f32 = x[b,0,:], the raw cls row the camera head reads.  D % 8 == 0. */
 int udb_vit_tap(const float* x, void* acc, float* cls_out, int32_t B, int32_t N, int32_t D, int32_t first, void* stream);
+/* The same with the running max kept in f32 (acc f32 [B*N, D]; no rounding): UniDepthV1 precision "split". */
+int udb_vit_tap_f32(const float* x, float* acc, float* cls_out, int32_t B, int32_t N, int32_t D, int32_t first, void* stream);
 
 /* LayerNorm over the last dim for widths that are multiples of 64 up to 1536 (ConvNeXt channel LayerNorm / LayerNorm2d,
  * convnext.py:214,252-263; decoder LayerNorms).  in row r at in + r*ld_in (+ add[(r % add_mod)*dim ..] when add != NULL:
  * "tokens + positional embedding", decoder.py:92-94,224).  s2d_w > 0: rows are the pixels of [B, s2d_h, s2d_w] maps and
  * pixel (y,x) is written to row (b, y/2, x/2), columns ((y&1)*2+(x&1))*dim.. of the k2 s2 downsample's im2col matrix
- * [B*(s2d_h/2)*(s2d_w/2), ld_out] (a trailing odd row / column is dropped, as the strided convolution drops it). */
+ * [B*(s2d_h/2)*(s2d_w/2), ld_out] (a trailing odd row / column is dropped, as the strided convolution drops it).
+ * out_f32: 0 f16, 1 (any other non-zero value but 2) f32, UDB_LN_OUT_SPLIT (2) a split-f16 operand: hi = f16(y) where
+ * the f16 output goes and lo = f16(y - f32(hi)) ld_out/2 columns further right (ld_out even; ld_out/2 >= dim, or
+ * >= 4*dim with space-to-depth, so that a row holds [hi | lo] of a udb_gemm_t.a_split_k operand). */
+#define UDB_LN_OUT_SPLIT 2
 typedef struct udb_layernorm_any_t {
   const void* in;
   int32_t in_f32;
@@ -411,6 +421,10 @@ int udb_layernorm_any(const udb_layernorm_any_t* p, void* stream);
  * w f32 [49, C] (tap-major), bias f32 [C] -> y f16 NHWC.  C % 64 == 0. */
 int udb_dwconv7_nhwc_f16(const void* x, const float* w, const float* bias, void* y, int32_t B, int32_t H, int32_t W,
                          int32_t C, void* stream);
+/* The same convolution on f32 NHWC maps x -> y (same taps, zero padding, bias and f32 summation order: an input that is
+ * exactly f16 gives the f32 sums udb_dwconv7_nhwc_f16 rounds).  C % 32 == 0; B, H, W >= 1. */
+int udb_dwconv7_nhwc_f32(const float* x, const float* w, const float* bias, float* y, int32_t B, int32_t H, int32_t W,
+                         int32_t C, void* stream);
 /* ConvNeXt block head of UniDepthV1 precision "fp8" (convnext.py:208-212: conv_dw -> norm), fused: the depthwise 7x7 of
  * udb_dwconv7_nhwc_f16 (same x / w / bias, f32 accumulation, result rounded to f16 as that call stores it), then
  * LayerNorm over the channels (eps 1e-6, f32 statistics; ln_w / ln_b f32 [C]) written straight as FP8 E4M3 bytes out
@@ -422,12 +436,17 @@ int udb_dwconv7_ln_e4m3(const void* x, const float* w, const float* bias, const 
 
 /* dst = first ? src : max(dst, src) element-wise over n f16 values (decoder.py:371-374 max_stack over a stage's blocks). */
 int udb_max_accum_f16(const void* src, void* dst, int64_t n, int32_t first, void* stream);
+/* The same over n f32 values, n % 4 == 0. */
+int udb_max_accum_f32(const float* src, float* dst, int64_t n, int32_t first, void* stream);
 
 /* Mean over the HW pixels of an f32 NHWC map -> [B, C] (ConvNeXt "cls tokens", convnext.py:471). */
 int udb_spatial_mean_f32(const float* x, float* out, int32_t B, int32_t HW, int32_t C, void* stream);
 
 /* F.interpolate(bilinear, align_corners=False, antialias=True) of an f16 NHWC map (flat_interpolate, geometric.py:228-252). */
 int udb_aa_resize_nhwc_f16(const void* in, void* out, int32_t B, int32_t H, int32_t W, int32_t C, int32_t oh, int32_t ow,
+                           void* stream);
+/* The same resize of an f32 NHWC map, with the same weights and summation order.  C % 8 == 0. */
+int udb_aa_resize_nhwc_f32(const float* in, float* out, int32_t B, int32_t H, int32_t W, int32_t C, int32_t oh, int32_t ow,
                            void* stream);
 
 /* Ray embedding of one decoder level (decoder.py:203-220): analytic unit rays of K (intr4 = fx,fy,cx,cy per image, network
@@ -457,6 +476,9 @@ int udb_v1_camera_intrinsics(const float* x4, const float* gt_k, int32_t B, int3
  * over 16 blocks per image, partial results are merged by a second kernel). */
 int udb_cross_attn_small(const float* q, const float* q_pos, const void* kv, float* out, float* scratch, int32_t B, int32_t nq,
                          int32_t nk, int32_t D, float scale, void* stream);
+/* The same with kv f32 [B*nk, 2D] (UniDepthV1 precision "split"); same summation order. */
+int udb_cross_attn_small_f32(const float* q, const float* q_pos, const float* kv, float* out, float* scratch, int32_t B,
+                             int32_t nq, int32_t nk, int32_t D, float scale, void* stream);
 
 /* p[r, j] = softmax_j(scale * s[r, j]) over j < n_valid, f32 [rows, ld_in] -> f16 [rows, ld_out], columns >= n_valid zero
  * (the P operand of the dense single-head attentions aggregate_16 / prompt_camera, decoder.py:231-236). */
@@ -658,12 +680,17 @@ void udb_v1_destroy(udb_engine_v1* e);
 int udb_v1_set_weight(udb_engine_v1* e, const char* name, const void* dev_ptr, const int64_t* shape, int32_t ndim,
                       int32_t dtype);
 /* Host scalars of the packed V1 model (the three output-head biases) and the encoder mode "precision": 0 (or absent) = f16
- * operands, 2 = FP8 E4M3 operands for the two MLP linear layers of the ConvNeXt encoder blocks of the stages the schedule
+ * operands, 1 = split-f16 operands (parity mode, as UniDepthV2's): every GEMM operand of the encoder and of the camera
+ * head's context path is a [hi | lo] pair and its weight is packed [N, 3K] = [hi | hi | lo] (udb_gemm_t.a_split_k) --
+ * stem_w, ds{i}.w, s{i}.b{j}.w1 / w2 or the DINOv2 blocks and patch_w, adapt.{l}.w_cam (the adapters' copy feeding the
+ * camera head), cam.inf.w1 / w2 and cam.agg.kv_w -- the residual stream, the encoder levels and the camera context stay
+ * f32 and the DINOv2 attention runs in the fp32 kernel; the depth head reads the f16 (hi) half and runs as in the f16
+ * mode.  2 = FP8 E4M3 operands for the two MLP linear layers of the ConvNeXt encoder blocks of the stages the schedule
  * runs in e4m3 (engine_v1.cu kFp8Stage; none at present, as none is faster that way) (s{i}.b{j}.w1_8 [4C, C],
  * w2_8 [C, 4C] UDB_DT_E4M3 with f32 per-output-channel scales w1_8s / w2_8s; udb_dwconv7_ln_e4m3 and
  * udb_quantize_rows_e4m3 quantise the activations per row) or for the four linear layers of every DINOv2 block (the
- * blocks.{i}.*_w8 operands of the V2 engine's fp8 mode).  The stem, downsample layers, attention and the decoder stay
- * f16 in both. */
+ * blocks.{i}.*_w8 operands of the V2 engine's fp8 mode); there the stem, downsample layers, attention and the decoder
+ * stay f16. */
 int udb_v1_set_scalar(udb_engine_v1* e, const char* name, double value);
 /* Shape arithmetic of one V1 call, the engine's own copy of `_shapes` / `_paddings` (unidepthv1.py:30-46): the image is resized
  * by `ratio` to (resized_h, resized_w) -- the larger side-ratio that still fits the fixed network input -- and zero-padded

@@ -254,16 +254,22 @@ EXPORTS = {
     "udb_infer_v2": (i32, [vp, C.POINTER(InferArgs), vp]),
     # UniDepthV1 operators + engine
     "udb_v1_preprocess": (i32, [C.POINTER(V1Preprocess), vp]),
+    "udb_v1_preprocess_split": (i32, [C.POINTER(V1Preprocess), vp]),
     "udb_layernorm_any": (i32, [C.POINTER(LayerNormAny), vp]),
     "udb_dwconv7_nhwc_f16": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, vp]),
+    "udb_dwconv7_nhwc_f32": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, vp]),
     "udb_dwconv7_ln_e4m3": (i32, [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]),
     "udb_max_accum_f16": (i32, [vp, vp, i64, i32, vp]),
+    "udb_max_accum_f32": (i32, [vp, vp, i64, i32, vp]),
     "udb_spatial_mean_f32": (i32, [vp, vp, i32, i32, i32, vp]),
     "udb_vit_tap": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
+    "udb_vit_tap_f32": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
     "udb_aa_resize_nhwc_f16": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, vp]),
+    "udb_aa_resize_nhwc_f32": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, vp]),
     "udb_v1_rays_sh81": (i32, [C.POINTER(V1Rays), vp]),
     "udb_v1_camera_intrinsics": (i32, [vp, vp, i32, i32, i32, f32, i32, i32, i32, vp, vp, vp, vp]),
     "udb_cross_attn_small": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp]),
+    "udb_cross_attn_small_f32": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, f32, vp]),
     "udb_softmax_rows": (i32, [vp, vp, i64, i32, i32, i32, f32, vp]),
     "udb_add_f32": (i32, [vp, vp, vp, vp, i64, vp]),
     "udb_copy_rows_f32_to_f16": (i32, [vp, vp, i32, i32, i32, i64, i64, vp]),

@@ -113,16 +113,82 @@ static void cvnxt_block_e4m3(Ctx& c, const std::string& p, float* x, __half* x16
   ar.release(m);
 }
 
+// The same block in split-precision mode (precision 1): the depthwise 7x7 reads the f32 residual stream and writes f32,
+// LayerNorm writes the [hi | lo] operand of fc1, fc1 writes its GELU output as a split operand for fc2, and both GEMMs
+// read [N, 3K] = [hi | hi | lo] weights (udb_gemm_t.a_split_k).  There is no f16 copy of x in this mode.
+static void cvnxt_block_split(Ctx& c, const std::string& p, float* x, int B, int Hh, int Ww, int C) {
+  Arena& ar = *c.ar;
+  const size_t m = ar.mark();
+  const long long rows = static_cast<long long>(B) * Hh * Ww;
+  float* y = ar.f(rows * C);
+  __half* hN = ar.h(rows * 2 * C);
+  __half* md = ar.h(rows * 8 * C);
+  c.expect2(p + "w1", 4 * C, 3 * C);
+  c.expect2(p + "w2", C, 12 * C);
+  const float* dw_w = c.F(p + "dw_w");
+  const float* dw_b = c.F(p + "dw_b");
+  c.launch([&] { return udb_dwconv7_nhwc_f32(x, dw_w, dw_b, y, B, Hh, Ww, C, c.st); });
+  c.ln_any(y, 1, hN, UDB_LN_OUT_SPLIT, c.F(p + "ln_w"), c.F(p + "ln_b"), rows, C, 1e-6f, 2 * C);
+  { Ctx::G q{hN, c.H(p + "w1"), static_cast<int>(rows), 4 * C, 3 * C}; q.lda = 2 * C; q.a_split_k = C; q.bias = c.F(p + "b1");
+    q.act = UDB_ACT_GELU; q.out = md; q.ldc = 8 * C; q.out_split = 4 * C; c.gemm(q); }
+  { Ctx::G q{md, c.H(p + "w2"), static_cast<int>(rows), C, 12 * C}; q.lda = 8 * C; q.a_split_k = 4 * C; q.bias = c.F(p + "b2");
+    q.gamma = c.F(p + "gamma"); q.resid = x; q.resid_f32 = 1; q.out = x; q.out_f32 = 1; c.gemm(q); }
+  ar.release(m);
+}
+
 // pre-processing of the input batch into the encoder's patch rows (unidepthv1.py _preprocess): 4x4 im2col rows of the
-// ConvNeXt stem (`patch` 0) or 14x14 DINOv2 patch rows (`patch` 14)
+// ConvNeXt stem (`patch` 0) or 14x14 DINOv2 patch rows (`patch` 14); `split`: as [hi | lo] operands
 static void preprocess(Ctx& c, const udb_v1_config_t& cf, const udb_infer_v1_args_t& a, const V1Geom& g, __half* patches,
-                       int patch) {
+                       int patch, bool split = false) {
   udb_v1_preprocess_t p;
   memset(&p, 0, sizeof(p));
   p.rgb = a.rgb; p.rgb_is_u8 = a.rgb_is_u8; p.scale255 = a.scale255; p.normalize = a.normalize; p.B = a.B; p.H = a.H; p.W = a.W;
   p.rh = g.rh; p.rw = g.rw; p.pad_l = g.pad_l; p.pad_t = g.pad_t; p.net_h = cf.net_h; p.net_w = cf.net_w; p.patches = patches;
   p.patch = patch;
-  c.launch([&] { return udb_v1_preprocess(&p, c.st); });
+  c.launch([&] { return split ? udb_v1_preprocess_split(&p, c.st) : udb_v1_preprocess(&p, c.st); });
+}
+
+// ConvNeXt encoder in split-precision mode (convnext.py:371-383,289-298 as in run_v1's f16 encoder): split stem rows ->
+// stem GEMM to f32 -> LayerNorm f32 -> stages of cvnxt_block_split; each downsample is a space-to-depth LayerNorm with
+// split output and the k2 s2 GEMM on it.  The running max of each stage's block outputs is kept in f32 (levels[i]).
+static void convnext_encoder_split(Ctx& c, const udb_v1_config_t& cf, const udb_infer_v1_args_t& a, const V1Geom& g, const int* sh,
+                                   const int* sw, void* const* levels, float* const* clsbuf, int total_blocks) {
+  Arena& ar = *c.ar;
+  const size_t m = ar.mark();
+  const int B = a.B, C0 = cf.dims[0];
+  const long long n0 = static_cast<long long>(B) * sh[0] * sw[0];
+  __half* patches = ar.h(n0 * 128);
+  preprocess(c, cf, a, g, patches, 0, true);
+  float* y0 = ar.f(n0 * C0);
+  c.expect2("stem_w", C0, 192);
+  { Ctx::G q{patches, c.H("stem_w"), static_cast<int>(n0), C0, 192}; q.lda = 128; q.a_split_k = 64; q.bias = c.F("stem_b");
+    q.out = y0; q.out_f32 = 1; c.gemm(q); }
+  float* x = ar.f(n0 * C0);
+  c.ln_any(y0, 1, x, 1, c.F("stem_ln_w"), c.F("stem_ln_b"), n0, C0, 1e-6f);
+  int blk = 0;
+  for (int i = 0; i < 4; ++i) {
+    const int C = cf.dims[i];
+    const long long n = static_cast<long long>(B) * sh[i] * sw[i];
+    if (i > 0) {
+      const int Cp = cf.dims[i - 1];
+      __half* A = ar.h(n * 8 * Cp);
+      const std::string d = idx("ds%d.", i);
+      c.ln_any(x, 1, A, UDB_LN_OUT_SPLIT, c.F(d + "ln_w"), c.F(d + "ln_b"), static_cast<long long>(B) * sh[i - 1] * sw[i - 1], Cp, 1e-6f,
+               8 * Cp, nullptr, 0, sh[i - 1], sw[i - 1]);
+      float* xn = ar.f(n * C);
+      c.expect2(d + "w", C, 12 * Cp);
+      { Ctx::G q{A, c.H(d + "w"), static_cast<int>(n), C, 12 * Cp}; q.lda = 8 * Cp; q.a_split_k = 4 * Cp; q.bias = c.F(d + "b");
+        q.out = xn; q.out_f32 = 1; c.gemm(q); }
+      x = xn;
+    }
+    for (int j = 0; j < cf.depths[i]; ++j, ++blk) {
+      cvnxt_block_split(c, idx2("s%d.b%d.", i, j), x, B, sh[i], sw[i], C);
+      c.launch([&] { return udb_max_accum_f32(x, static_cast<float*>(levels[i]), n * C, j == 0, c.st); });
+      const int from_end = total_blocks - 1 - blk;
+      if (from_end < 4) c.launch([&] { return udb_spatial_mean_f32(x, clsbuf[from_end], B, sh[i] * sw[i], C, c.st); });
+    }
+  }
+  ar.release(m);
 }
 
 static inline long long rup(long long v, long long m) { return (v + m - 1) / m * m; }
@@ -235,23 +301,27 @@ static void conv_upsample(Ctx& c, const std::string& p, const float* lat, const 
 // bicubic resize of the 37x37 grid) as row-mapped residual -> cls rows -> the shared block loop.  After every block the
 // tap kernel folds (patch tokens + cls token) into the running max of its slice (levels[s], decoder.py:371-379; slice s
 // holds cf.depths[s] blocks) and copies the raw cls rows of the last four blocks into clsbuf[k] (block last - k).
+// Split-precision mode (`split`): split patch rows and patch weight [D, 3*640], the shared block loop's split mode and
+// f32 levels (udb_vit_tap_f32).
 static void dino_encoder(Ctx& c, const udb_v1_config_t& cf, const udb_infer_v1_args_t& a, const V1Geom& g, int gh, int gw,
-                         __half* const* levels, float* const* clsbuf, bool fp8) {
+                         void* const* levels, float* const* clsbuf, bool fp8, bool split) {
   Arena& ar = *c.ar;
   const int B = a.B, D = cf.dims[0], N = gh * gw, T = N + 1;
   const size_t BN = static_cast<size_t>(B) * N, BT = static_cast<size_t>(B) * T;
   int depth = 0;
   for (int i = 0; i < 4; ++i) depth += cf.depths[i];
   const size_t m = ar.mark();
-  __half* patches = ar.h(BN * 640);
-  preprocess(c, cf, a, g, patches, 14);
+  const int sx = split ? 2 : 1;
+  __half* patches = ar.h(BN * 640 * sx);
+  preprocess(c, cf, a, g, patches, 14, split);
   float* x = ar.f(BT * D);           // fp32 residual stream [B, 1 + N, D]
   {
-    c.expect2("patch_w", D, 640);
+    c.expect2("patch_w", D, split ? 3 * 640 : 640);
     c.expect2("pos", T, D);
     const float* pos = c.F("pos");
     const float* cls = c.F("cls");     // looked up here so that a dry run names it when it is missing
-    Ctx::G q{patches, c.H("patch_w"), static_cast<int>(BN), D, 640};
+    Ctx::G q{patches, c.H("patch_w"), static_cast<int>(BN), D, split ? 3 * 640 : 640};
+    q.lda = 640 * sx; q.a_split_k = split ? 640 : 0;
     q.bias = c.F("patch_b"); q.resid = pos; q.resid_f32 = 1; q.ldr = D; q.out = x; q.out_f32 = 1;
     q.rows_per_group = N; q.group_stride = T; q.row_offset = 1; q.resid_mod = N; q.resid_row_offset = 1;
     c.gemm(q);
@@ -259,11 +329,16 @@ static void dino_encoder(Ctx& c, const udb_v1_config_t& cf, const udb_infer_v1_a
   }
   VitBlocks v{B, T, D, D / 64, depth};
   v.fp8 = fp8;
+  v.split = split;
   int slice = 0, start = 0;
   vit_blocks(c, "blocks.", x, v, [&](int i) {
     if (i == start + cf.depths[slice]) { start = i; ++slice; }
     const int from_end = depth - 1 - i;
-    c.launch([&] { return udb_vit_tap(x, levels[slice], from_end < 4 ? clsbuf[from_end] : nullptr, B, N, D, i == start, c.st); });
+    float* cls_out = from_end < 4 ? clsbuf[from_end] : nullptr;
+    c.launch([&] {
+      return split ? udb_vit_tap_f32(x, static_cast<float*>(levels[slice]), cls_out, B, N, D, i == start, c.st)
+                   : udb_vit_tap(x, levels[slice], cls_out, B, N, D, i == start, c.st);
+    });
   });
   ar.release(m);
 }
@@ -283,16 +358,29 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
   }
   Stage stage;
   // "precision": 0 (absent) = f16 operands, 2 = e4m3 operands for the encoder blocks' MLP (ConvNeXt) or all four linear
-  // layers (DINOv2); the stem, downsample layers and the decoder are the same in both
+  // layers (DINOv2); the stem, downsample layers and the decoder are the same in both.  1 = split-f16 operands (parity
+  // mode): every GEMM of the encoder and of the camera head's context path (adapters, in_features, the aggregate block's
+  // kv) multiplies [hi | lo] operands with [hi | hi | lo] weights, and the encoder levels and camera context are f32;
+  // the depth head reads the hi half of the adapters' LayerNorm and runs as in the f16 mode.
   const double prec = e->scalars.count("precision") ? e->scalars["precision"] : 0.0;
-  if (prec != 0.0 && prec != 2.0) { set_error("udb_infer_v1: precision %g unsupported (0 f16, 2 e4m3)", prec); return 1; }
-  const bool f8 = prec == 2.0;
+  if (prec != 0.0 && prec != 1.0 && prec != 2.0) { set_error("udb_infer_v1: precision %g unsupported (0 f16, 1 split f16, 2 e4m3)", prec); return 1; }
+  const bool f8 = prec == 2.0, sp = prec == 1.0;
+  if (sp) {   // an f16 packing registered with precision 1 is named for what it is, not only by its first mis-shaped operand
+    const char* first = dino ? "patch_w" : "stem_w";
+    const int k3 = dino ? 3 * 640 : 3 * 64;
+    const Weight* w = c.W(first);
+    if (!c.rc && (w->ndim != 2 || w->shape[1] != k3)) {
+      set_error("udb_infer_v1: precision 1 (split f16) needs the split packing: '%s' has %lld columns, expected %d", first,
+                static_cast<long long>(w->shape[1]), k3);
+      return 1;
+    }
+  }
 
   // ---- pre-processing + stem (convnext.py:371-383: conv k4 s4 as an im2col GEMM, then LayerNorm2d)
   stage.next("udb_v1:preprocess+stem");
-  __half* levels[4];
+  void* levels[4];                  // f16, or f32 in split mode
   float* clsbuf[4];
-  for (int i = 0; i < 4; ++i) levels[i] = ar.h(static_cast<size_t>(B) * sh[i] * sw[i] * cf.dims[i]);
+  for (int i = 0; i < 4; ++i) levels[i] = ar.alloc(static_cast<size_t>(B) * sh[i] * sw[i] * cf.dims[i] * (sp ? 4 : 2));
   int total_blocks = 0;
   for (int i = 0; i < 4; ++i) total_blocks += cf.depths[i];
   // decoder.py:377-379: the cls tokens of the LAST FOUR BLOCKS, newest first
@@ -306,7 +394,10 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
   for (int k = 0; k < 4; ++k) clsbuf[k] = ar.f(static_cast<size_t>(B) * cls_dim[k]);     // clsbuf[k]: block (last - k)
   if (dino) {
     stage.next("udb_v1:dinov2_encoder");
-    dino_encoder(c, cf, a, g, sh[0], sw[0], levels, clsbuf, f8);
+    dino_encoder(c, cf, a, g, sh[0], sw[0], levels, clsbuf, f8, sp);
+  } else if (sp) {
+    stage.next("udb_v1:convnext_stages");
+    convnext_encoder_split(c, cf, a, g, sh, sw, levels, clsbuf, total_blocks);
   } else {
     const size_t enc_mark = ar.mark();
     const long long n0 = static_cast<long long>(B) * sh[0] * sw[0];
@@ -357,22 +448,35 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
   const long long Rq = static_cast<long long>(B) * nq;
   __half* featcat = ar.h(Rq * 4 * hid);                          // [B*nq, 4*hid]   (features_channels, decoder.py:224)
   __half* tokens = ar.h((Rq * 4 + 64) * hid);                    // [B, 4*nq, hid]  (features_tokens,   decoder.py:220)
+  // split mode: the camera head's copy of the tokens, f32 from split operands (the depth head keeps the f16 tokens)
+  float* cam_tokens = sp ? ar.f(Rq * 4 * hid) : nullptr;
   for (int l = 0; l < 4; ++l) {
     const size_t m = ar.mark();
     const int C = cf.dims[l];
-    const __half* src = levels[l];
+    const void* src = levels[l];
     if (sh[l] != hc || sw[l] != wc) {
-      __half* r = ar.h(Rq * C);
-      c.launch([&] { return udb_aa_resize_nhwc_f16(levels[l], r, B, sh[l], sw[l], C, hc, wc, st); });
+      void* r = ar.alloc(Rq * C * (sp ? 4 : 2));
+      c.launch([&] {
+        return sp ? udb_aa_resize_nhwc_f32(static_cast<const float*>(levels[l]), static_cast<float*>(r), B, sh[l], sw[l], C, hc, wc, st)
+                  : udb_aa_resize_nhwc_f16(levels[l], r, B, sh[l], sw[l], C, hc, wc, st);
+      });
       src = r;
     }
-    __half* an = ar.h(Rq * C);
     const std::string ad = idx("adapt.%d.", l);
-    ln16(c, src, 0, an, ad + "ln_w", ad + "ln_b", Rq, C, 1e-5f);
-    { Ctx::G q{an, c.H(ad + "w"), static_cast<int>(Rq), hid, C}; q.bias = c.F(ad + "b"); q.act = UDB_ACT_GELU; q.out = tokens;
+    const int sx = sp ? 2 : 1;
+    __half* an = ar.h(Rq * C * sx);
+    if (sp) c.ln_any(src, 1, an, UDB_LN_OUT_SPLIT, c.F(ad + "ln_w"), c.F(ad + "ln_b"), Rq, C, 1e-5f, 2 * C);
+    else ln16(c, src, 0, an, ad + "ln_w", ad + "ln_b", Rq, C, 1e-5f);
+    { Ctx::G q{an, c.H(ad + "w"), static_cast<int>(Rq), hid, C}; q.lda = C * sx; q.bias = c.F(ad + "b"); q.act = UDB_ACT_GELU; q.out = tokens;
       q.rows_per_group = nq; q.group_stride = 4 * nq; q.row_offset = l * nq; c.gemm(q); }
-    { Ctx::G q{an, c.H(ad + "w"), static_cast<int>(Rq), hid, C}; q.bias = c.F(ad + "b"); q.act = UDB_ACT_GELU; q.out = featcat + l * hid;
-      q.ldc = 4 * hid; c.gemm(q); }
+    { Ctx::G q{an, c.H(ad + "w"), static_cast<int>(Rq), hid, C}; q.lda = C * sx; q.bias = c.F(ad + "b"); q.act = UDB_ACT_GELU;
+      q.out = featcat + l * hid; q.ldc = 4 * hid; c.gemm(q); }
+    if (sp) {
+      c.expect2(ad + "w_cam", hid, 3 * C);
+      Ctx::G q{an, c.H(ad + "w_cam"), static_cast<int>(Rq), hid, 3 * C}; q.lda = 2 * C; q.a_split_k = C; q.bias = c.F(ad + "b");
+      q.act = UDB_ACT_GELU; q.out = cam_tokens; q.out_f32 = 1; q.rows_per_group = nq; q.group_stride = 4 * nq; q.row_offset = l * nq;
+      c.gemm(q);
+    }
     ar.release(m);
   }
   const float* tokens_pos = c.F("tokens_pos");                     // [4*nq, hid]: sine position + level embedding (decoder.py:410-433)
@@ -400,8 +504,29 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
     float* cl = cam_mlp(c, "cam.cls", toks, R4, hid, hid / 2, hid, nullptr, nullptr);
     // context = in_features(features + pos) ++ cls tokens
     const long long Rc = static_cast<long long>(B) * (4 * nq + 4);
-    __half* ctx = ar.h(Rc * hid);
-    {
+    void* ctx = ar.alloc(Rc * hid * (sp ? 4 : 2));            // f16, or f32 in split mode
+    if (sp) {
+      // the same steps on split operands: LayerNorm (f32 tokens + position, split out) -> in_features' two GEMMs -> f32
+      // context rows; the cls rows are copied in f32
+      const size_t m2 = ar.mark();
+      __half* a1 = ar.h(Rq * 4 * 2 * hid);
+      __half* m1 = ar.h(Rq * 4 * 4 * hid);
+      c.expect2("cam.inf.w1", 2 * hid, 3 * hid);
+      c.expect2("cam.inf.w2", hid, 6 * hid);
+      c.ln_any(cam_tokens, 1, a1, UDB_LN_OUT_SPLIT, c.F("cam.inf.nw"), c.F("cam.inf.nb"), Rq * 4, hid, 1e-5f, 2 * hid, tokens_pos, 4LL * nq);
+      { Ctx::G q{a1, c.H("cam.inf.w1"), static_cast<int>(Rq * 4), 2 * hid, 3 * hid}; q.lda = 2 * hid; q.a_split_k = hid;
+        q.bias = c.F("cam.inf.b1"); q.act = UDB_ACT_GELU; q.out = m1; q.ldc = 4 * hid; q.out_split = 2 * hid; c.gemm(q); }
+      { Ctx::G q{m1, c.H("cam.inf.w2"), static_cast<int>(Rq * 4), hid, 6 * hid}; q.lda = 4 * hid; q.a_split_k = 2 * hid;
+        q.bias = c.F("cam.inf.b2"); q.out = ctx; q.out_f32 = 1; q.rows_per_group = 4 * nq; q.group_stride = 4 * nq + 4; q.row_offset = 0;
+        c.gemm(q); }
+      ar.release(m2);
+      c.launch([&] {
+        const size_t row = sizeof(float) * hid;
+        return cuda_rc(cudaMemcpy2DAsync(static_cast<float*>(ctx) + 4LL * nq * hid, (4 * nq + 4) * row, cl, 4 * row, 4 * row, B,
+                                         cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(st)),
+                       "engine_v1: copying the camera tokens into the f32 context");
+      });
+    } else {
       const size_t m2 = ar.mark();
       __half* a1 = ar.h(Rq * 4 * hid);
       __half* m1 = ar.h(Rq * 4 * 2 * hid);
@@ -410,25 +535,37 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
       { Ctx::G q{m1, c.H("cam.inf.w2"), static_cast<int>(Rq * 4), hid, 2 * hid}; q.bias = c.F("cam.inf.b2"); q.out = ctx;
         q.rows_per_group = 4 * nq; q.group_stride = 4 * nq + 4; q.row_offset = 0; c.gemm(q); }
       ar.release(m2);
+      c.launch([&] { return udb_copy_rows_f32_to_f16(cl, ctx, B, 4, hid, 4LL * nq + 4, 4LL * nq, st); });
     }
-    c.launch([&] { return udb_copy_rows_f32_to_f16(cl, ctx, B, 4, hid, 4LL * nq + 4, 4LL * nq, st); });
     // aggregate: the 4 tokens attend to the context (single head of width hid, position term on q)
     float* t;
     {
       const std::string ag = "cam.agg.";
       float* xn = ar.f(static_cast<size_t>(R4) * hid);
       c.layernorm(cl, 1, xn, 1, c.F(ag + "nxw"), c.F(ag + "nxb"), R4, hid, 1e-5f);
-      __half* cn = ar.h(Rc * hid);
-      ln16(c, ctx, 0, cn, ag + "ncw", ag + "ncb", Rc, hid, 1e-5f);
-      __half* kv = ar.h(Rc * 2 * hid);
-      { Ctx::G q{cn, c.H(ag + "kv_w"), static_cast<int>(Rc), 2 * hid, hid}; q.bias = c.F(ag + "kv_b"); q.out = kv; c.gemm(q); }
+      void* kv;
+      if (sp) {         // split LayerNorm -> kv GEMM on split operands -> f32 (k | v)
+        __half* cn = ar.h(Rc * 2 * hid);
+        c.ln_any(ctx, 1, cn, UDB_LN_OUT_SPLIT, c.F(ag + "ncw"), c.F(ag + "ncb"), Rc, hid, 1e-5f, 2 * hid);
+        kv = ar.f(Rc * 2 * hid);
+        c.expect2(ag + "kv_w", 2 * hid, 3 * hid);
+        { Ctx::G q{cn, c.H(ag + "kv_w"), static_cast<int>(Rc), 2 * hid, 3 * hid}; q.lda = 2 * hid; q.a_split_k = hid;
+          q.bias = c.F(ag + "kv_b"); q.out = kv; q.out_f32 = 1; c.gemm(q); }
+      } else {
+        __half* cn = ar.h(Rc * hid);
+        ln16(c, ctx, 0, cn, ag + "ncw", ag + "ncb", Rc, hid, 1e-5f);
+        kv = ar.h(Rc * 2 * hid);
+        { Ctx::G q{cn, c.H(ag + "kv_w"), static_cast<int>(Rc), 2 * hid, hid}; q.bias = c.F(ag + "kv_b"); q.out = kv; c.gemm(q); }
+      }
       float* q = ar.f(static_cast<size_t>(R4) * hid);
       c.small_linear(xn, R4, hid, c.F(ag + "q_w"), hid, c.F(ag + "q_b"), UDB_ACT_NONE, nullptr, nullptr, q);
       float* at = ar.f(static_cast<size_t>(R4) * hid);
       float* scratch = ar.f(static_cast<size_t>(B) * 16 * 4 * (hid + 2));
       const float* cam_pos = c.F("cam.pos");
       c.launch([&] {
-        return udb_cross_attn_small(q, cam_pos, kv, at, scratch, B, 4, 4 * nq + 4, hid, 1.0f / sqrtf(static_cast<float>(hid)), st);
+        const float scale = 1.0f / sqrtf(static_cast<float>(hid));
+        return sp ? udb_cross_attn_small_f32(q, cam_pos, static_cast<const float*>(kv), at, scratch, B, 4, 4 * nq + 4, hid, scale, st)
+                  : udb_cross_attn_small(q, cam_pos, kv, at, scratch, B, 4, 4 * nq + 4, hid, scale, st);
       });
       float* t2 = ar.f(static_cast<size_t>(R4) * hid);
       c.small_linear(at, R4, hid, c.F(ag + "out_w"), hid, c.F(ag + "out_b"), UDB_ACT_NONE, c.F(ag + "ls1"), cl, t2);

@@ -66,8 +66,9 @@ __device__ __forceinline__ AAxis aa_axis(int i, int in_size, float scale) {
 // to (rh, rw) -> zero pad to the fixed network shape -> P x P stride-P patch rows f16:
 //   P = 4:  [B*gh*gw, 64]  (48 used: column c*16 + py*4 + px, the ConvNeXt stem conv's im2col, convnext.py:371-383)
 //   P = 14: [B*gh*gw, 640] (588 used: column c*196 + py*14 + px, the DINOv2 patch embedding's im2col, patch_embed.py)
+// SPLIT: rows of 2 x COLS halves, hi = f16(v) (the rows above) and lo = f16(v - f32(hi)) COLS columns to the right.
 // ------------------------------------------------------------------------------------------------------------------
-template <int P>
+template <int P, bool SPLIT>
 __global__ void __launch_bounds__(256) v1_preprocess_kernel(const udb_v1_preprocess_t p, int gh, int gw, float sh, float sw) {
   constexpr int COLS = P == 4 ? 64 : 640, USED = 3 * P * P, NV8 = COLS / 8;
   const long long total = (long long)p.B * gh * gw * NV8;   // NV8 x (8 columns) per patch row
@@ -103,6 +104,17 @@ __global__ void __launch_bounds__(256) v1_preprocess_kernel(const udb_v1_preproc
       }
       val[j] = acc;
     }
+    if (SPLIT) {
+      float lo[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) lo[j] = val[j] - __half2float(__float2half_rn(val[j]));
+      __half* dst = reinterpret_cast<__half*>(p.patches) + row * 2 * COLS + v8 * 8;
+      *reinterpret_cast<uint4*>(dst) =
+          make_uint4(pack_half2(val[0], val[1]), pack_half2(val[2], val[3]), pack_half2(val[4], val[5]), pack_half2(val[6], val[7]));
+      *reinterpret_cast<uint4*>(dst + COLS) =
+          make_uint4(pack_half2(lo[0], lo[1]), pack_half2(lo[2], lo[3]), pack_half2(lo[4], lo[5]), pack_half2(lo[6], lo[7]));
+      continue;
+    }
     *reinterpret_cast<uint4*>(reinterpret_cast<__half*>(p.patches) + row * COLS + v8 * 8) =
         make_uint4(pack_half2(val[0], val[1]), pack_half2(val[2], val[3]), pack_half2(val[4], val[5]), pack_half2(val[6], val[7]));
   }
@@ -114,9 +126,10 @@ __global__ void __launch_bounds__(256) v1_preprocess_kernel(const udb_v1_preproc
 // One warp per row, lane owns element pairs.  Extras: an additive f32 table (in = x[row] + add[row % add_mod]) for
 // "tokens + positional embedding" (decoder.py:92-94), and a space-to-depth output mapping that writes pixel (y, x) of
 // an [B,H,W,C] map into row (b, y/2, x/2), columns ((y&1)*2 + (x&1))*C + c of the k2 s2 downsample's im2col matrix
-// (odd trailing row / column dropped, as the strided conv does).
+// (odd trailing row / column dropped, as the strided conv does).  OUT: 0 f16, 1 f32, 2 split f16 (hi = f16(y) where the
+// f16 output goes, lo = f16(y - f32(hi)) ld_out / 2 columns further right).
 // ------------------------------------------------------------------------------------------------------------------
-template <bool IN_F32, bool OUT_F32, int R, int NV>
+template <bool IN_F32, int OUT, int R, int NV>
 __global__ void __launch_bounds__(256) layernorm_any_kernel(const udb_layernorm_any_t p) {
   // one warp normalises R consecutive rows; all loads of the R rows are issued before the first reduction (narrow rows
   // alone -- 192 channels = 384 B -- do not keep enough bytes in flight); NV = max float2 per lane per row
@@ -181,8 +194,14 @@ __global__ void __launch_bounds__(256) layernorm_any_kernel(const udb_layernorm_
         const float2 w = __ldg(reinterpret_cast<const float2*>(p.weight + e));
         const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + e));
         const float y0 = (x[r][i].x - mean) * rstd * w.x + bb.x, y1 = (x[r][i].y - mean) * rstd * w.y + bb.y;
-        if (OUT_F32) *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + obase + e) = make_float2(y0, y1);
-        else *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(p.out) + obase + e) = pack_half2(y0, y1);
+        if (OUT == 1) {
+          *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + obase + e) = make_float2(y0, y1);
+        } else {
+          *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(p.out) + obase + e) = pack_half2(y0, y1);
+          if (OUT == 2)
+            *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(p.out) + obase + (p.ld_out >> 1) + e) =
+                pack_half2(y0 - __half2float(__float2half_rn(y0)), y1 - __half2float(__float2half_rn(y1)));
+        }
       }
     }
   }
@@ -259,6 +278,63 @@ __global__ void __launch_bounds__(256) dwconv7_kernel(const __half* __restrict__
         unpack2(acc[i][1], a2, a3);
         *reinterpret_cast<uint2*>(y + (((long long)b * H + gy) * W + gx) * C + c0 + cg * 4) = make_uint2(pack_half2(a0, a1), pack_half2(a2, a3));
       }
+    }
+  }
+}
+
+// The same convolution on f32 NHWC maps (split-precision mode: it reads the f32 residual stream).  A block owns a 16x8
+// tile of 32 channels (the 22x14 halo in f32 is 39 KB of shared memory); each thread slides along 4 consecutive x of one
+// row for one 4-channel group.  Bias first, then dy outer / dx inner fmaf: the taps, padding and summation order of
+// dwconv7_kernel, so an input that is exactly f16 gives that kernel's f32 sums.
+constexpr int DWF_CB = 32, DWF_TW = 16, DWF_TH = 8;
+
+__global__ void __launch_bounds__(256) dwconv7_f32_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
+                                                         float* __restrict__ y, int H, int W, int C, int tiles_x) {
+  constexpr int HH = DWF_TH + 6, HW = DWF_TW + 6;
+  __shared__ __align__(16) float tile[HH * HW * DWF_CB];
+  const int tx0 = (blockIdx.x % tiles_x) * DWF_TW, ty0 = (blockIdx.x / tiles_x) * DWF_TH;
+  const int c0 = blockIdx.y * DWF_CB, b = blockIdx.z;
+  const float* xb = x + (long long)b * H * W * C;
+  for (int i = threadIdx.x; i < HH * HW * (DWF_CB / 4); i += 256) {
+    const int ch = i & 7, pix = i >> 3;
+    const int hy = pix / HW, hx = pix - hy * HW;
+    const int gy = ty0 + hy - 3, gx = tx0 + hx - 3;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (gy >= 0 && gy < H && gx >= 0 && gx < W) v = __ldg(reinterpret_cast<const float4*>(xb + ((long long)gy * W + gx) * C + c0 + ch * 4));
+    *reinterpret_cast<float4*>(tile + pix * DWF_CB + ch * 4) = v;
+  }
+  __syncthreads();
+  const int cg = threadIdx.x & 7, xs = ((threadIdx.x >> 3) & 3) * 4, r = threadIdx.x >> 5;
+  float acc[4][4];
+  {
+    const float4 bv = __ldg(reinterpret_cast<const float4*>(bias + c0 + cg * 4));
+#pragma unroll
+    for (int i = 0; i < 4; ++i) { acc[i][0] = bv.x; acc[i][1] = bv.y; acc[i][2] = bv.z; acc[i][3] = bv.w; }
+  }
+#pragma unroll 1
+  for (int dy = 0; dy < 7; ++dy) {
+    float4 in[10];
+#pragma unroll
+    for (int i = 0; i < 10; ++i) in[i] = *reinterpret_cast<const float4*>(tile + ((r + dy) * HW + xs + i) * DWF_CB + cg * 4);
+#pragma unroll
+    for (int dx = 0; dx < 7; ++dx) {
+      const float4 wv = __ldg(reinterpret_cast<const float4*>(w + (long long)(dy * 7 + dx) * C + c0 + cg * 4));
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        acc[i][0] = fmaf(in[i + dx].x, wv.x, acc[i][0]);
+        acc[i][1] = fmaf(in[i + dx].y, wv.y, acc[i][1]);
+        acc[i][2] = fmaf(in[i + dx].z, wv.z, acc[i][2]);
+        acc[i][3] = fmaf(in[i + dx].w, wv.w, acc[i][3]);
+      }
+    }
+  }
+  const int gy = ty0 + r;
+  if (gy < H) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int gx = tx0 + xs + i;
+      if (gx < W)
+        *reinterpret_cast<float4*>(y + (((long long)b * H + gy) * W + gx) * C + c0 + cg * 4) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
     }
   }
 }
@@ -459,9 +535,23 @@ __global__ void __launch_bounds__(256) max_accum_kernel(const uint4* __restrict_
   }
 }
 
+// the same running maximum over f32 values (split-precision mode keeps the encoder levels in f32)
+__global__ void __launch_bounds__(256) max_accum_f32_kernel(const float4* __restrict__ src, float4* __restrict__ dst, long long n4, int first) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+    float4 s = src[i];
+    if (!first) {
+      const float4 d = dst[i];
+      s = make_float4(fmaxf(s.x, d.x), fmaxf(s.y, d.y), fmaxf(s.z, d.z), fmaxf(s.w, d.w));
+    }
+    dst[i] = s;
+  }
+}
+
 // DINOv2 block output -> decoder level (unidepthv1.py:322-326, decoder.py:371-379): one thread per 8 channels of a patch
 // token, acc = first ? f16(x_tok + x_cls) : max(acc, f16(x_tok + x_cls)); the trailing B*D/8 work items copy the raw cls
 // rows to cls_out.  HBM-bound: 32 B of x read and 16 (first) or 32 B of acc moved per item; the cls row stays in L1/L2.
+// F32: the level is kept in f32 (split-precision mode), acc holds 2 x uint4 = 8 floats per item, no rounding.
+template <bool F32>
 __global__ void __launch_bounds__(256) vit_tap_kernel(const float* __restrict__ x, uint4* __restrict__ acc, float* __restrict__ cls_out,
                                                      int B, int N, int D, int first) {
   const int d8 = D / 8;
@@ -484,6 +574,19 @@ __global__ void __launch_bounds__(256) vit_tap_kernel(const float* __restrict__ 
     const float4* tok = reinterpret_cast<const float4*>(x + ((long long)b * (N + 1) + 1 + t) * D + c);
     const float4* cls = reinterpret_cast<const float4*>(x + (long long)b * (N + 1) * D + c);
     const float4 a0 = tok[0], a1 = tok[1], c0 = __ldg(cls), c1 = __ldg(cls + 1);
+    if (F32) {
+      float4 s0 = make_float4(a0.x + c0.x, a0.y + c0.y, a0.z + c0.z, a0.w + c0.w);
+      float4 s1 = make_float4(a1.x + c1.x, a1.y + c1.y, a1.z + c1.z, a1.w + c1.w);
+      float4* af = reinterpret_cast<float4*>(acc) + 2 * i;
+      if (!first) {
+        const float4 d0 = af[0], d1 = af[1];
+        s0 = make_float4(fmaxf(s0.x, d0.x), fmaxf(s0.y, d0.y), fmaxf(s0.z, d0.z), fmaxf(s0.w, d0.w));
+        s1 = make_float4(fmaxf(s1.x, d1.x), fmaxf(s1.y, d1.y), fmaxf(s1.z, d1.z), fmaxf(s1.w, d1.w));
+      }
+      af[0] = s0;
+      af[1] = s1;
+      continue;
+    }
     uint4 v = make_uint4(pack_half2(a0.x + c0.x, a0.y + c0.y), pack_half2(a0.z + c0.z, a0.w + c0.w),
                          pack_half2(a1.x + c1.x, a1.y + c1.y), pack_half2(a1.z + c1.z, a1.w + c1.w));
     if (!first) {
@@ -516,8 +619,28 @@ __global__ void __launch_bounds__(256) spatial_mean_kernel(const float* __restri
   }
 }
 
-// antialiased bilinear resize of an NHWC f16 map (flat_interpolate, geometric.py:228-252): one thread per 8 channels
-__global__ void __launch_bounds__(256) aa_resize_nhwc_kernel(const __half* __restrict__ in, __half* __restrict__ out, int B, int H, int W, int C,
+// antialiased bilinear resize of an NHWC f16 or f32 map (flat_interpolate, geometric.py:228-252): one thread per 8
+// channels; the same weights and summation order for both element types
+__device__ __forceinline__ void load8(const __half* p, float (&f)[8]) {
+  const uint4 u = *reinterpret_cast<const uint4*>(p);
+  const __half2* h = reinterpret_cast<const __half2*>(&u);
+#pragma unroll
+  for (int q = 0; q < 4; ++q) { const float2 t = __half22float2(h[q]); f[2 * q] = t.x; f[2 * q + 1] = t.y; }
+}
+__device__ __forceinline__ void load8(const float* p, float (&f)[8]) {
+  const float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + 4);
+  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
+}
+__device__ __forceinline__ void store8(__half* p, const float (&f)[8]) {
+  *reinterpret_cast<uint4*>(p) = make_uint4(pack_half2(f[0], f[1]), pack_half2(f[2], f[3]), pack_half2(f[4], f[5]), pack_half2(f[6], f[7]));
+}
+__device__ __forceinline__ void store8(float* p, const float (&f)[8]) {
+  *reinterpret_cast<float4*>(p) = make_float4(f[0], f[1], f[2], f[3]);
+  *reinterpret_cast<float4*>(p + 4) = make_float4(f[4], f[5], f[6], f[7]);
+}
+
+template <class T>
+__global__ void __launch_bounds__(256) aa_resize_nhwc_kernel(const T* __restrict__ in, T* __restrict__ out, int B, int H, int W, int C,
                                                             int oh, int ow, float sh, float sw) {
   const int cv = C >> 3;
   const long long total = (long long)B * oh * ow * cv;
@@ -534,22 +657,17 @@ __global__ void __launch_bounds__(256) aa_resize_nhwc_kernel(const __half* __res
 #pragma unroll
       for (int j = 0; j < 8; ++j) r[j] = 0.f;
       for (int jx = 0; jx < ax.xsize; ++jx) {
-        const uint4 u = *reinterpret_cast<const uint4*>(in + (((long long)b * H + ay.xmin + jy) * W + ax.xmin + jx) * C + c8 * 8);
-        const __half2* h = reinterpret_cast<const __half2*>(&u);
+        float f[8];
+        load8(in + (((long long)b * H + ay.xmin + jy) * W + ax.xmin + jx) * C + c8 * 8, f);
         const float wx = ax.w(jx);
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const float2 f = __half22float2(h[q]);
-          r[2 * q] += wx * f.x;
-          r[2 * q + 1] += wx * f.y;
-        }
+        for (int j = 0; j < 8; ++j) r[j] += wx * f[j];
       }
       const float wy = ay.w(jy);
 #pragma unroll
       for (int j = 0; j < 8; ++j) acc[j] += wy * r[j];
     }
-    *reinterpret_cast<uint4*>(out + pix * C + c8 * 8) =
-        make_uint4(pack_half2(acc[0], acc[1]), pack_half2(acc[2], acc[3]), pack_half2(acc[4], acc[5]), pack_half2(acc[6], acc[7]));
+    store8(out + pix * C + c8 * 8, acc);
   }
 }
 
@@ -671,10 +789,25 @@ __global__ void v1_camera_intrinsics_kernel(const float* x4, const float* gt_k, 
 // 4-query cross attention of the camera head (decoder.py:95, AttentionBlock num_heads=1): q f32 [B*nq, D] (+ q_pos), kv f16
 // [B*nk, 2D] (k | v), out f32 [B*nq, D].  Keys are split over CA_SPLITS blocks per image (flash-decoding style): each block
 // reads its slice of K and V ONCE for all queries and writes a partial (max, sum, weighted V); a second kernel merges.
+// KV = float: the same kernel on f32 keys and values (split-precision mode), same summation order.
 constexpr int CA_SPLITS = 16, CA_MAXQ = 4;
 
+__device__ __forceinline__ float2 load2(const __half* p) { return __half22float2(*reinterpret_cast<const __half2*>(p)); }
+__device__ __forceinline__ float2 load2(const float* p) { return *reinterpret_cast<const float2*>(p); }
+__device__ __forceinline__ void ldg8(const __half* p, float (&f)[8]) {
+  const uint4 u = __ldg(reinterpret_cast<const uint4*>(p));
+  const __half2* h = reinterpret_cast<const __half2*>(&u);
+#pragma unroll
+  for (int t = 0; t < 4; ++t) { const float2 v = __half22float2(h[t]); f[2 * t] = v.x; f[2 * t + 1] = v.y; }
+}
+__device__ __forceinline__ void ldg8(const float* p, float (&f)[8]) {
+  const float4 a = __ldg(reinterpret_cast<const float4*>(p)), b = __ldg(reinterpret_cast<const float4*>(p + 4));
+  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
+}
+
+template <class KV>
 __global__ void __launch_bounds__(256) cross_attn_partial_kernel(const float* __restrict__ q, const float* __restrict__ q_pos,
-                                                                const __half* __restrict__ kv, float* __restrict__ part, int nq, int nk, int D,
+                                                                const KV* __restrict__ kv, float* __restrict__ part, int nq, int nk, int D,
                                                                 float scale) {
   extern __shared__ float sm[];
   const int chunk = (nk + CA_SPLITS - 1) / CA_SPLITS;
@@ -687,16 +820,13 @@ __global__ void __launch_bounds__(256) cross_attn_partial_kernel(const float* __
   for (int i = threadIdx.x; i < nq * D; i += 256)
     qs[i] = (q[(long long)b * nq * D + i] + (q_pos ? q_pos[i] : 0.f)) * scale;
   __syncthreads();
-  const __half* kb = kv + (long long)b * nk * 2 * D;
+  const KV* kb = kv + (long long)b * nk * 2 * D;
   for (int j = warp; j < n; j += 8) {
     float a[CA_MAXQ] = {0.f, 0.f, 0.f, 0.f};
-    const __half* kr = kb + (long long)(j0 + j) * 2 * D;
+    const KV* kr = kb + (long long)(j0 + j) * 2 * D;
     for (int d = lane * 8; d < D; d += 256) {
-      const uint4 u = __ldg(reinterpret_cast<const uint4*>(kr + d));
-      const __half2* h = reinterpret_cast<const __half2*>(&u);
       float kf[8];
-#pragma unroll
-      for (int t = 0; t < 4; ++t) { const float2 f = __half22float2(h[t]); kf[2 * t] = f.x; kf[2 * t + 1] = f.y; }
+      ldg8(kr + d, kf);
 #pragma unroll
       for (int qi = 0; qi < CA_MAXQ; ++qi)
         if (qi < nq) {
@@ -731,7 +861,7 @@ __global__ void __launch_bounds__(256) cross_attn_partial_kernel(const float* __
   for (int d = threadIdx.x * 2; d < D; d += 512) {
     float acc[CA_MAXQ][2] = {{0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}};
     for (int j = 0; j < n; ++j) {
-      const float2 vf = __half22float2(*reinterpret_cast<const __half2*>(kb + (long long)(j0 + j) * 2 * D + D + d));
+      const float2 vf = load2(kb + (long long)(j0 + j) * 2 * D + D + d);
 #pragma unroll
       for (int qi = 0; qi < CA_MAXQ; ++qi)
         if (qi < nq) {
@@ -1052,28 +1182,51 @@ int udb_v1_preprocess(const udb_v1_preprocess_t* p, void* stream) {
   if (p->patch == 14) {
     if (p->net_h % 14 || p->net_w % 14) { set_error("udb_v1_preprocess: network shape %dx%d is not a multiple of 14", p->net_h, p->net_w); return 1; }
     const int gh = p->net_h / 14, gw = p->net_w / 14;
-    v1_preprocess_kernel<14><<<grid_1d((long long)p->B * gh * gw * 80), 256, 0, ST(stream)>>>(*p, gh, gw, sh, sw);
+    v1_preprocess_kernel<14, false><<<grid_1d((long long)p->B * gh * gw * 80), 256, 0, ST(stream)>>>(*p, gh, gw, sh, sw);
     return check_launch("v1_preprocess_kernel<14>");
   }
   if (p->patch != 0 && p->patch != 4) { set_error("udb_v1_preprocess: patch %d unsupported (0 / 4 or 14)", p->patch); return 1; }
   if (p->net_h < 4 || p->net_w < 4) { set_error("udb_v1_preprocess: bad network shape"); return 1; }
   const int gh = (p->net_h - 4) / 4 + 1, gw = (p->net_w - 4) / 4 + 1;
-  v1_preprocess_kernel<4><<<grid_1d((long long)p->B * gh * gw * 8), 256, 0, ST(stream)>>>(*p, gh, gw, sh, sw);
+  v1_preprocess_kernel<4, false><<<grid_1d((long long)p->B * gh * gw * 8), 256, 0, ST(stream)>>>(*p, gh, gw, sh, sw);
   return check_launch("v1_preprocess_kernel");
+}
+
+int udb_v1_preprocess_split(const udb_v1_preprocess_t* p, void* stream) {
+  const float sh = (float)p->H / (float)p->rh, sw = (float)p->W / (float)p->rw;
+  if (p->patch == 14) {
+    if (p->net_h % 14 || p->net_w % 14) { set_error("udb_v1_preprocess_split: network shape %dx%d is not a multiple of 14", p->net_h, p->net_w); return 1; }
+    const int gh = p->net_h / 14, gw = p->net_w / 14;
+    v1_preprocess_kernel<14, true><<<grid_1d((long long)p->B * gh * gw * 80), 256, 0, ST(stream)>>>(*p, gh, gw, sh, sw);
+    return check_launch("v1_preprocess_split_kernel<14>");
+  }
+  if (p->patch != 0 && p->patch != 4) { set_error("udb_v1_preprocess_split: patch %d unsupported (0 / 4 or 14)", p->patch); return 1; }
+  if (p->net_h < 4 || p->net_w < 4) { set_error("udb_v1_preprocess_split: bad network shape"); return 1; }
+  const int gh = (p->net_h - 4) / 4 + 1, gw = (p->net_w - 4) / 4 + 1;
+  v1_preprocess_kernel<4, true><<<grid_1d((long long)p->B * gh * gw * 8), 256, 0, ST(stream)>>>(*p, gh, gw, sh, sw);
+  return check_launch("v1_preprocess_split_kernel");
 }
 
 int udb_layernorm_any(const udb_layernorm_any_t* p, void* stream) {
   if (p->dim % 64 || p->dim > 1536 || p->dim <= 0) { set_error("udb_layernorm_any: dim %d unsupported (multiple of 64, <= 1536)", p->dim); return 1; }
+  const bool split = p->out_f32 == UDB_LN_OUT_SPLIT;
+  if (split && (p->ld_out % 2 || p->ld_out / 2 < (p->s2d_w > 0 ? 4LL : 1LL) * p->dim)) {
+    set_error("udb_layernorm_any: split output needs an even ld_out with room for both halves (ld_out=%lld, dim=%d%s)",
+              (long long)p->ld_out, p->dim, p->s2d_w > 0 ? ", space-to-depth" : "");
+    return 1;
+  }
   if (p->rows <= 0) return 0;
   note_work(0.0, (double)p->rows * p->dim * ((p->in_f32 ? 4 : 2) + (p->out_f32 ? 4 : 2)));
   // rows per warp by width: 4 up to 256 channels, 2 up to 768, 1 beyond (registers: R * dim / 32 floats)
 #define UDB_LN_ANY(R_, NV_)                                                                                        \
   do {                                                                                                             \
     const int grid = (int)((p->rows + 8 * (R_) - 1) / (8 * (R_)));                                                 \
-    if (p->in_f32 && p->out_f32) layernorm_any_kernel<true, true, R_, NV_><<<grid, 256, 0, ST(stream)>>>(*p);     \
-    else if (p->in_f32) layernorm_any_kernel<true, false, R_, NV_><<<grid, 256, 0, ST(stream)>>>(*p);             \
-    else if (p->out_f32) layernorm_any_kernel<false, true, R_, NV_><<<grid, 256, 0, ST(stream)>>>(*p);            \
-    else layernorm_any_kernel<false, false, R_, NV_><<<grid, 256, 0, ST(stream)>>>(*p);                           \
+    if (split && p->in_f32) layernorm_any_kernel<true, 2, R_, NV_><<<grid, 256, 0, ST(stream)>>>(*p);             \
+    else if (split) layernorm_any_kernel<false, 2, R_, NV_><<<grid, 256, 0, ST(stream)>>>(*p);                    \
+    else if (p->in_f32 && p->out_f32) layernorm_any_kernel<true, 1, R_, NV_><<<grid, 256, 0, ST(stream)>>>(*p);   \
+    else if (p->in_f32) layernorm_any_kernel<true, 0, R_, NV_><<<grid, 256, 0, ST(stream)>>>(*p);                 \
+    else if (p->out_f32) layernorm_any_kernel<false, 1, R_, NV_><<<grid, 256, 0, ST(stream)>>>(*p);               \
+    else layernorm_any_kernel<false, 0, R_, NV_><<<grid, 256, 0, ST(stream)>>>(*p);                               \
   } while (0)
   if (p->dim <= 256) UDB_LN_ANY(4, 4);
   else if (p->dim <= 768) UDB_LN_ANY(2, 12);
@@ -1132,6 +1285,24 @@ int udb_dwconv7_ln_e4m3(const void* x, const float* w, const float* bias, const 
   return check_launch("dwconv7_ln_e4m3_kernel");
 }
 
+int udb_dwconv7_nhwc_f32(const float* x, const float* w, const float* bias, float* y, int32_t B, int32_t H, int32_t W, int32_t C, void* stream) {
+  if (C <= 0 || C % DWF_CB || B < 1 || H < 1 || W < 1) {
+    set_error("udb_dwconv7_nhwc_f32: B=%d H=%d W=%d C=%d unsupported (C a multiple of 32, the rest >= 1)", B, H, W, C);
+    return 1;
+  }
+  note_work(2.0 * 49 * B * H * W * C, 8.0 * B * H * W * C);
+  const int tx = (W + DWF_TW - 1) / DWF_TW, ty = (H + DWF_TH - 1) / DWF_TH;
+  dwconv7_f32_kernel<<<dim3(tx * ty, C / DWF_CB, B), 256, 0, ST(stream)>>>(x, w, bias, y, H, W, C, tx);
+  return check_launch("dwconv7_f32_kernel");
+}
+
+int udb_max_accum_f32(const float* src, float* dst, int64_t n, int32_t first, void* stream) {
+  if (n % 4) { set_error("udb_max_accum_f32: n must be a multiple of 4"); return 1; }
+  note_work(0.0, (first ? 8.0 : 12.0) * n);
+  max_accum_f32_kernel<<<grid_1d(n / 4), 256, 0, ST(stream)>>>(reinterpret_cast<const float4*>(src), reinterpret_cast<float4*>(dst), n / 4, first);
+  return check_launch("max_accum_f32_kernel");
+}
+
 int udb_max_accum_f16(const void* src, void* dst, int64_t n, int32_t first, void* stream) {
   if (n % 8) { set_error("udb_max_accum_f16: n must be a multiple of 8"); return 1; }
   note_work(0.0, (first ? 4.0 : 6.0) * n);
@@ -1143,8 +1314,16 @@ int udb_vit_tap(const float* x, void* acc, float* cls_out, int32_t B, int32_t N,
   if (D % 8 || D <= 0 || N <= 0 || B <= 0) { set_error("udb_vit_tap: bad shape B=%d N=%d D=%d (D %% 8 == 0)", B, N, D); return 1; }
   const long long items = (long long)B * N * (D / 8) + (cls_out ? (long long)B * (D / 8) : 0);
   note_work((double)B * N * D, (double)B * N * D * (4.0 + (first ? 2.0 : 4.0)) + (cls_out ? 8.0 * B * D : 0.0));
-  vit_tap_kernel<<<grid_1d(items), 256, 0, ST(stream)>>>(x, reinterpret_cast<uint4*>(acc), cls_out, B, N, D, first);
+  vit_tap_kernel<false><<<grid_1d(items), 256, 0, ST(stream)>>>(x, reinterpret_cast<uint4*>(acc), cls_out, B, N, D, first);
   return check_launch("vit_tap_kernel");
+}
+
+int udb_vit_tap_f32(const float* x, float* acc, float* cls_out, int32_t B, int32_t N, int32_t D, int32_t first, void* stream) {
+  if (D % 8 || D <= 0 || N <= 0 || B <= 0) { set_error("udb_vit_tap_f32: bad shape B=%d N=%d D=%d (D %% 8 == 0)", B, N, D); return 1; }
+  const long long items = (long long)B * N * (D / 8) + (cls_out ? (long long)B * (D / 8) : 0);
+  note_work((double)B * N * D, (double)B * N * D * (4.0 + (first ? 4.0 : 8.0)) + (cls_out ? 8.0 * B * D : 0.0));
+  vit_tap_kernel<true><<<grid_1d(items), 256, 0, ST(stream)>>>(x, reinterpret_cast<uint4*>(acc), cls_out, B, N, D, first);
+  return check_launch("vit_tap_f32_kernel");
 }
 
 int udb_spatial_mean_f32(const float* x, float* out, int32_t B, int32_t HW, int32_t C, void* stream) {
@@ -1156,9 +1335,17 @@ int udb_spatial_mean_f32(const float* x, float* out, int32_t B, int32_t HW, int3
 int udb_aa_resize_nhwc_f16(const void* in, void* out, int32_t B, int32_t H, int32_t W, int32_t C, int32_t oh, int32_t ow, void* stream) {
   if (C % 8) { set_error("udb_aa_resize_nhwc_f16: C must be a multiple of 8"); return 1; }
   note_work(0.0, 2.0 * B * C * ((double)H * W + (double)oh * ow));
-  aa_resize_nhwc_kernel<<<grid_1d((long long)B * oh * ow * (C / 8)), 256, 0, ST(stream)>>>(
+  aa_resize_nhwc_kernel<__half><<<grid_1d((long long)B * oh * ow * (C / 8)), 256, 0, ST(stream)>>>(
       reinterpret_cast<const __half*>(in), reinterpret_cast<__half*>(out), B, H, W, C, oh, ow, (float)H / (float)oh, (float)W / (float)ow);
   return check_launch("aa_resize_nhwc_kernel");
+}
+
+int udb_aa_resize_nhwc_f32(const float* in, float* out, int32_t B, int32_t H, int32_t W, int32_t C, int32_t oh, int32_t ow, void* stream) {
+  if (C % 8) { set_error("udb_aa_resize_nhwc_f32: C must be a multiple of 8"); return 1; }
+  note_work(0.0, 4.0 * B * C * ((double)H * W + (double)oh * ow));
+  aa_resize_nhwc_kernel<float><<<grid_1d((long long)B * oh * ow * (C / 8)), 256, 0, ST(stream)>>>(
+      in, out, B, H, W, C, oh, ow, (float)H / (float)oh, (float)W / (float)ow);
+  return check_launch("aa_resize_nhwc_f32_kernel");
 }
 
 int udb_v1_rays_sh81(const udb_v1_rays_t* p, void* stream) {
@@ -1174,26 +1361,44 @@ int udb_v1_camera_intrinsics(const float* x4, const float* gt_k, int32_t B, int3
   return check_launch("v1_camera_intrinsics_kernel");
 }
 
-int udb_cross_attn_small(const float* q, const float* q_pos, const void* kv, float* out, float* scratch, int32_t B, int32_t nq, int32_t nk,
-                         int32_t D, float scale, void* stream) {
-  if (nq < 1 || nq > CA_MAXQ || D % 256 || !scratch) { set_error("udb_cross_attn_small: nq=%d D=%d unsupported (nq <= 4, D %% 256 == 0)", nq, D); return 1; }
+}  // extern "C"
+
+namespace udb {
+// udb_cross_attn_small / udb_cross_attn_small_f32: f16 or f32 (k | v) rows
+template <class KV>
+static int cross_attn_small(const char* fn, const float* q, const float* q_pos, const KV* kv, float* out, float* scratch, int B, int nq, int nk,
+                            int D, float scale, void* stream) {
+  if (nq < 1 || nq > CA_MAXQ || D % 256 || !scratch) { set_error("%s: nq=%d D=%d unsupported (nq <= 4, D %% 256 == 0)", fn, nq, D); return 1; }
   const int chunk = (nk + CA_SPLITS - 1) / CA_SPLITS;
   const size_t smem = (size_t)(nq * D + nq * chunk + 16) * 4;
-  if (smem > 200 * 1024) { set_error("udb_cross_attn_small: nk=%d too large", nk); return 1; }
+  if (smem > 200 * 1024) { set_error("%s: nk=%d too large", fn, nk); return 1; }
   static std::atomic<size_t> set_for[64];
   int dev = 0;
   cudaGetDevice(&dev);
   if (smem > 48 * 1024 && smem > set_for[dev & 63].load()) {
-    if (cudaFuncSetAttribute(cross_attn_partial_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
-      set_error("udb_cross_attn_small: cudaFuncSetAttribute failed"); return 1;
+    if (cudaFuncSetAttribute(cross_attn_partial_kernel<KV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+      set_error("%s: cudaFuncSetAttribute failed", fn); return 1;
     }
     set_for[dev & 63].store(smem);
   }
-  note_work(4.0 * B * nq * (double)nk * D, 4.0 * B * nk * D);
-  cross_attn_partial_kernel<<<dim3(CA_SPLITS, B), 256, smem, ST(stream)>>>(q, q_pos, reinterpret_cast<const __half*>(kv), scratch, nq, nk, D, scale);
-  if (check_launch("cross_attn_partial_kernel")) return 1;
+  note_work(4.0 * B * nq * (double)nk * D, 2.0 * sizeof(KV) * B * nk * D);
+  cross_attn_partial_kernel<KV><<<dim3(CA_SPLITS, B), 256, smem, ST(stream)>>>(q, q_pos, kv, scratch, nq, nk, D, scale);
+  if (check_launch(sizeof(KV) == 2 ? "cross_attn_partial_kernel" : "cross_attn_partial_f32_kernel")) return 1;
   cross_attn_merge_kernel<<<dim3(nq, B), 256, 0, ST(stream)>>>(scratch, out, nq, D);
   return check_launch("cross_attn_merge_kernel");
+}
+}  // namespace udb
+
+extern "C" {
+
+int udb_cross_attn_small(const float* q, const float* q_pos, const void* kv, float* out, float* scratch, int32_t B, int32_t nq, int32_t nk,
+                         int32_t D, float scale, void* stream) {
+  return cross_attn_small("udb_cross_attn_small", q, q_pos, reinterpret_cast<const __half*>(kv), out, scratch, B, nq, nk, D, scale, stream);
+}
+
+int udb_cross_attn_small_f32(const float* q, const float* q_pos, const float* kv, float* out, float* scratch, int32_t B, int32_t nq,
+                             int32_t nk, int32_t D, float scale, void* stream) {
+  return cross_attn_small("udb_cross_attn_small_f32", q, q_pos, kv, out, scratch, B, nq, nk, D, scale, stream);
 }
 
 int udb_softmax_rows(const float* s, void* p, int64_t rows, int32_t n_valid, int32_t ld_in, int32_t ld_out, float scale, void* stream) {

@@ -36,6 +36,15 @@ from .unidepthv2 import pack_e4m3, pack_vit_encoder
 FP8_STAGES = (False, False, False, False)
 
 
+def split_weight(w: torch.Tensor) -> torch.Tensor:
+    """GEMM weight [N, K] of the split-precision mode: [N, 3K] = [hi | hi | lo] f16 with hi = f16(w), lo = f16(w - hi)
+    (include/udb.h udb_gemm_t.a_split_k; the layout unidepthv2.pack_vit_encoder(split=True) packs)."""
+    w = w.to(f32)
+    hi = w.to(f16)
+    lo = (w - hi.to(f32)).to(f16)
+    return torch.cat([hi, hi, lo], dim=1).contiguous()
+
+
 def _offset_pos_embed(pos: torch.Tensor, gh: int, gw: int, offset: float) -> torch.Tensor:
     """DINOv2 position table of a gh x gw patch grid with a nonzero interpolate_offset (dinov2.py:267-304): bicubic
     resize of the M x M grid with scale factors ((gh + offset) / M, (gw + offset) / M), height first, so the sampling
@@ -79,6 +88,10 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         # the blocks of the stages in FP8_STAGES, fed by a fused depthwise 7x7 + LayerNorm + quantisation kernel
         # (udb_dwconv7_ln_e4m3) -- an empty set, since no stage is faster that way, so ConvNeXt-L computes what "f16" does.  The stem, downsample layers, attention and the decoder stay f16.  Its accuracy is only measured on
         # seeded synthetic weights (tests/test_v1_fp8_gpu.py), not on trained checkpoints.
+        # "split": parity / debugging mode, as UniDepthV2's -- every GEMM operand of the encoder and of the camera head's
+        # context path (the adapters' camera copy, in_features, the aggregate block's kv) is a hi + lo pair fed through the
+        # same wgmma GEMM (include/udb.h udb_gemm_t.a_split_k), the encoder levels and the camera context stay f32, and
+        # ViT-L's attention runs in the fp32 kernel.  The depth head runs as in "f16".  Slower; not a speed mode.
         self.precision = "f16"
 
     def _fingerprint(self):
@@ -90,15 +103,17 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         product caller (CUDA device); tests/test_engine_schedule_cpu.py runs it on the CPU to check, through the engine's
         dry run, that the packer registers exactly the operands the C schedule asks for."""
         s = self.spec
-        if self.precision not in ("f16", "fp8"):
-            raise ValueError(f"precision must be 'f16' or 'fp8', not {self.precision!r}")
-        fp8 = self.precision == "fp8"
+        if self.precision not in ("split", "f16", "fp8"):
+            raise ValueError(f"precision must be 'split', 'f16' or 'fp8', not {self.precision!r}")
+        split, fp8 = self.precision == "split", self.precision == "fp8"
         sd = {k: v.detach() for k, v in self.state_dict().items()}
         h16 = lambda t: t.to(f16).contiguous()
         c32 = lambda t: t.to(f32).contiguous()
+        # GEMM weight of the split-precision mode's operands: [N, 3K] = [hi | hi | lo], or f16 in the other modes
+        s16 = lambda t: split_weight(t) if split else h16(t)
         T: Dict[str, torch.Tensor] = {}
         # an engine without "precision" runs the f16 mode, so the f16 packing registers exactly the scalars it always has
-        S: Dict[str, float] = {"precision": 2.0} if fp8 else {}
+        S: Dict[str, float] = {"precision": 2.0} if fp8 else ({"precision": 1.0} if split else {})
         pe, pd = "pixel_encoder.", "pixel_decoder."
         hid = s.hidden
 
@@ -112,9 +127,10 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
             out[:t.shape[0]] = t
             return out
 
-        def block(dst, src, conv_names, e4m3=False):
-            """ConvNeXt block operands: depthwise weights tap-major [49, C] f32, MLP weights f16, or e4m3 with per-output-channel
-            scales (`w1_8` / `w1_8s`, `w2_8` / `w2_8s`; pack_e4m3) for a block of the fp8 mode."""
+        def block(dst, src, conv_names, e4m3=False, enc16=h16):
+            """ConvNeXt block operands: depthwise weights tap-major [49, C] f32, MLP weights f16 (`enc16`: split in the
+            encoder's split mode), or e4m3 with per-output-channel scales (`w1_8` / `w1_8s`, `w2_8` / `w2_8s`; pack_e4m3) for
+            a block of the fp8 mode."""
             dw, norm, fc1, fc2 = conv_names
             w = sd[f"{src}{dw}.weight"]
             T[dst + "dw_w"] = c32(w.reshape(w.shape[0], 49).t())
@@ -125,7 +141,7 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
                 T[dst + "w1_8"], T[dst + "w1_8s"] = pack_e4m3(sd[f"{src}{fc1}.weight"])
                 T[dst + "w2_8"], T[dst + "w2_8s"] = pack_e4m3(sd[f"{src}{fc2}.weight"])
             else:
-                T[dst + "w1"], T[dst + "w2"] = h16(sd[f"{src}{fc1}.weight"]), h16(sd[f"{src}{fc2}.weight"])
+                T[dst + "w1"], T[dst + "w2"] = enc16(sd[f"{src}{fc1}.weight"]), enc16(sd[f"{src}{fc2}.weight"])
             T[dst + "gamma"] = c32(sd[f"{src}gamma"])
 
         hc, wc = s.common_grid()
@@ -133,26 +149,28 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         if s.encoder == ENCODER_DINOV2:
             # the V2 encoder's f16 or fp8 packing; the final norm, mask token and register tokens are never read
             # (use_norm=False, dinov2.py:173-178)
-            T.update(pack_vit_encoder(sd, s.embed_dim, s.enc_depth, dev, fp8=fp8))
+            T.update(pack_vit_encoder(sd, s.embed_dim, s.enc_depth, dev, split=split, fp8=fp8))
             T["pos"] = c32(_offset_pos_embed(T["pos"], hc, wc, V1_INTERPOLATE_OFFSET))
         for i, depth in enumerate(s.depths if s.encoder == ENCODER_CONVNEXT else ()):
             if i == 0:
-                T["stem_w"] = h16(zpad(sd[pe + "stem.0.weight"].reshape(s.dims[0], 48), s.dims[0], 64))
+                T["stem_w"] = s16(zpad(sd[pe + "stem.0.weight"].reshape(s.dims[0], 48), s.dims[0], 64))
                 T["stem_b"] = c32(sd[pe + "stem.0.bias"])
                 T["stem_ln_w"], T["stem_ln_b"] = c32(sd[pe + "stem.1.weight"]), c32(sd[pe + "stem.1.bias"])
             st = f"{pe}stages.{i}."
             if i > 0:
                 w = sd[st + "downsample.1.weight"]                               # [C, Cp, 2, 2] -> [C, (dy,dx,ci)]
                 T[f"ds{i}.ln_w"], T[f"ds{i}.ln_b"] = c32(sd[st + "downsample.0.weight"]), c32(sd[st + "downsample.0.bias"])
-                T[f"ds{i}.w"], T[f"ds{i}.b"] = h16(w.permute(0, 2, 3, 1).reshape(w.shape[0], -1)), c32(sd[st + "downsample.1.bias"])
+                T[f"ds{i}.w"], T[f"ds{i}.b"] = s16(w.permute(0, 2, 3, 1).reshape(w.shape[0], -1)), c32(sd[st + "downsample.1.bias"])
             for j in range(depth):
-                block(f"s{i}.b{j}.", f"{st}blocks.{j}.", ("conv_dw", "norm", "mlp.fc1", "mlp.fc2"), fp8 and FP8_STAGES[i])
+                block(f"s{i}.b{j}.", f"{st}blocks.{j}.", ("conv_dw", "norm", "mlp.fc1", "mlp.fc2"), fp8 and FP8_STAGES[i], s16)
 
         # ---- decoder: adapters, embeddings
         for l in range(4):
             a = f"{pd}input_adapter.input_adapters.{l}"
             T[f"adapt.{l}.ln_w"], T[f"adapt.{l}.ln_b"] = c32(sd[a + ".0.weight"]), c32(sd[a + ".0.bias"])
             T[f"adapt.{l}.w"], T[f"adapt.{l}.b"] = h16(sd[a + ".1.weight"]), c32(sd[a + ".1.bias"])
+            if split:       # the adapter's copy for the camera head, which reads it on split operands
+                T[f"adapt.{l}.w_cam"] = split_weight(sd[a + ".1.weight"])
             t = f"{pd}token_adapter.input_adapters.{l}"
             T[f"tok.{l}.ln_w"], T[f"tok.{l}.ln_b"] = c32(sd[t + ".0.weight"]), c32(sd[t + ".0.bias"])
             T[f"tok.{l}.w"], T[f"tok.{l}.b"] = c32(sd[t + ".1.weight"]), c32(sd[t + ".1.bias"])
@@ -175,8 +193,8 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         T["cam.cls.w1"], T["cam.cls.b1"] = c32(sd[cl + "cls_project.1.weight"]), c32(sd[cl + "cls_project.1.bias"])
         T["cam.cls.w2"], T["cam.cls.b2"] = c32(sd[cl + "cls_project.3.weight"]), c32(sd[cl + "cls_project.3.bias"])
         T["cam.inf.nw"], T["cam.inf.nb"] = c32(sd[cl + "in_features.norm.weight"]), c32(sd[cl + "in_features.norm.bias"])
-        T["cam.inf.w1"], T["cam.inf.b1"] = h16(sd[cl + "in_features.proj1.weight"]), c32(sd[cl + "in_features.proj1.bias"])
-        T["cam.inf.w2"], T["cam.inf.b2"] = h16(sd[cl + "in_features.proj2.weight"]), c32(sd[cl + "in_features.proj2.bias"])
+        T["cam.inf.w1"], T["cam.inf.b1"] = s16(sd[cl + "in_features.proj1.weight"]), c32(sd[cl + "in_features.proj1.bias"])
+        T["cam.inf.w2"], T["cam.inf.b2"] = s16(sd[cl + "in_features.proj2.weight"]), c32(sd[cl + "in_features.proj2.bias"])
         T["cam.pos"] = c32(sd[cl + "latents_pos"].reshape(4, hid))
 
         def cam_block(dst, src, kv_half):
@@ -184,7 +202,7 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
                          ("ncb", "norm_attnctx.bias"), ("q_w", "q.weight"), ("q_b", "q.bias"), ("kv_b", "kv.bias"),
                          ("out_w", "out.weight"), ("out_b", "out.bias"), ("ls1", "ls1.gamma"), ("ls2", "ls2.gamma")):
                 T[dst + a] = c32(sd[src + b])
-            T[dst + "kv_w"] = h16(sd[src + "kv.weight"]) if kv_half else c32(sd[src + "kv.weight"])
+            T[dst + "kv_w"] = s16(sd[src + "kv.weight"]) if kv_half else c32(sd[src + "kv.weight"])
             mlp32(dst + "mlp", src + "mlp")
 
         cam_block("cam.agg.", cl + "aggregate.", True)
