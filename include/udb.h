@@ -203,12 +203,13 @@ typedef struct udb_layernorm_t {
   const float* weight;
   const float* bias;
   int32_t rows, dim;
-  int64_t ld_in, ld_out;
+  int64_t ld_in, ld_out; /* ld_out >= dim + out_split */
   int32_t rows_per_group, group_stride, row_offset;
   float eps;
   int32_t dim_valid; /* 0 = dim.  f16->f16 rows of 64/128/256 only: statistics over the first dim_valid
                         columns (zero-padded channel rows, e.g. ViT-B's 96-channel map stored as 128) */
-  int32_t out_split; /* > 0 (f32 -> f16 rows only): also store lo = f16(y - f32(hi)) at column + out_split */
+  int32_t out_split; /* > 0: also store lo = f16(y - f32(hi)) at column + out_split.  Only with in_f32 = 1 and
+                        out_f32 = 0: any other combination (or a negative value) is rejected */
 } udb_layernorm_t;
 
 int udb_layernorm(const udb_layernorm_t* p, void* stream);
@@ -272,12 +273,13 @@ typedef struct udb_small_linear_t {
   float* y;
   int32_t M, N, K;
   int32_t act;
-  int32_t ldx, ldy, ldr; /* row strides (elements) of x, y, resid; 0 = dense (K, N, N) */
+  int32_t ldx, ldy, ldr; /* row strides (elements) of x, y, resid; 0 = dense (K, N, N).  16-byte loads along K when
+                            K % 128 == 0, ldx % 4 == 0 and x, w are 16-byte aligned; one float per lane otherwise */
 } udb_small_linear_t;
 int udb_small_linear_f32(const udb_small_linear_t* p, void* stream);
 
 /* Self-attention over the 4 camera tokens, fp32 (layers/attention.py:110-138 with pos_embed added
- * to q only).  q [B,4,C], kv [B,4,2C] (k then v), pos [4,C] -> out [B,4,C]. */
+ * to q only).  q [B,4,C], kv [B,4,2C] (k then v), pos [4,C] -> out [B,4,C].  B >= 1, heads >= 1, C % heads == 0. */
 int udb_camera_attn4_f32(const float* q, const float* kv, const float* pos, float* out, int32_t B,
                          int32_t C, int32_t heads, void* stream);
 
@@ -439,7 +441,7 @@ int udb_max_accum_f16(const void* src, void* dst, int64_t n, int32_t first, void
 /* The same over n f32 values, n % 4 == 0. */
 int udb_max_accum_f32(const float* src, float* dst, int64_t n, int32_t first, void* stream);
 
-/* Mean over the HW pixels of an f32 NHWC map -> [B, C] (ConvNeXt "cls tokens", convnext.py:471). */
+/* Mean over the HW pixels of an f32 NHWC map -> [B, C] (ConvNeXt "cls tokens", convnext.py:471).  B, HW, C >= 1. */
 int udb_spatial_mean_f32(const float* x, float* out, int32_t B, int32_t HW, int32_t C, void* stream);
 
 /* F.interpolate(bilinear, align_corners=False, antialias=True) of an f16 NHWC map (flat_interpolate, geometric.py:228-252). */
@@ -481,14 +483,16 @@ int udb_cross_attn_small_f32(const float* q, const float* q_pos, const float* kv
                              int32_t nq, int32_t nk, int32_t D, float scale, void* stream);
 
 /* p[r, j] = softmax_j(scale * s[r, j]) over j < n_valid, f32 [rows, ld_in] -> f16 [rows, ld_out], columns >= n_valid zero
- * (the P operand of the dense single-head attentions aggregate_16 / prompt_camera, decoder.py:231-236). */
+ * (the P operand of the dense single-head attentions aggregate_16 / prompt_camera, decoder.py:231-236).  rows >= 0,
+ * 1 <= n_valid <= ld_in and n_valid <= ld_out; columns >= n_valid of s are never read. */
 int udb_softmax_rows(const float* s, void* p, int64_t rows, int32_t n_valid, int32_t ld_in, int32_t ld_out, float scale,
                      void* stream);
 
 /* out = a + b (f32; out and/or an f16 copy), n % 4 == 0 (decoder.py:246-252 `latents + rays_embedding`). */
 int udb_add_f32(const float* a, const float* b, float* out, void* out_f16, int64_t n, void* stream);
 
-/* f32 [groups*rows_per_group, D] -> f16 rows (g*dst_group_stride + dst_row0 + r) of dst (decoder.py:94 torch.cat). */
+/* f32 [groups*rows_per_group, D] -> f16 rows (g*dst_group_stride + dst_row0 + r) of dst (decoder.py:94 torch.cat).
+ * groups, rows_per_group, D >= 1. */
 int udb_copy_rows_f32_to_f16(const float* src, void* dst, int32_t groups, int32_t rows_per_group, int32_t D,
                              int64_t dst_group_stride, int64_t dst_row0, void* stream);
 
@@ -510,8 +514,9 @@ int udb_nystrom_k2_pinv(const void* landmarks, float* k2, float* z, float* tmp, 
 int udb_nystrom_zk3(const float* z, const void* k3, int32_t ldk3, void* out, int32_t ldo, int32_t B, int32_t heads, void* stream);
 
 /* V1 post-processing (unidepthv1.py:66-94,352-366).  mean_maps: the three exp'ed maps (gh*2, gh*4, gh*8 grids) antialias-
- * resized to the network shape and averaged.  postprocess: crop the paddings, antialias-resize to (H, W) -> depth; points =
- * spherical_zbuffer_to_euclidean(theta, phi, z) with the angles of the unit ray of k4 (fx,fy,cx,cy) through each pixel. */
+ * resized to the network shape and averaged (B, gh, gw, net_h, net_w >= 1).  postprocess: crop the paddings, antialias-resize
+ * to (H, W) -> depth; points = spherical_zbuffer_to_euclidean(theta, phi, z) with the angles of the unit ray of k4
+ * (fx,fy,cx,cy) through each pixel.  B, H, W >= 1, paddings >= 0 and the cropped size net - pads >= 1 on both axes. */
 int udb_v1_mean_maps(const float* o8, const float* o4, const float* o2, float* mean, int32_t B, int32_t gh, int32_t gw,
                      int32_t net_h, int32_t net_w, void* stream);
 typedef struct udb_v1_postprocess_t {

@@ -1,4 +1,6 @@
-"""Host-side layout checks of udb_gemm_f16, udb_attention_f16 and udb_conv3x3_halo_f16 (include/udb.h).
+"""Host-side layout checks of udb_gemm_f16, udb_attention_f16, udb_conv3x3_halo_f16 and the CUDA-core launchers
+udb_layernorm, udb_softmax_rows, udb_camera_attn4_f32, udb_spatial_mean_f32, udb_copy_rows_f32_to_f16, udb_v1_mean_maps
+and udb_v1_postprocess (include/udb.h).
 
 Every call runs in a fresh interpreter with CUDA_VISIBLE_DEVICES="" and plain integers as fake device pointers, so no
 kernel can launch even on a machine with a GPU, even if a check were missing or came after the first CUDA call.  For each
@@ -17,7 +19,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 BASE = 1 << 28          # fake device addresses, 1 KB aligned
 P = {name: BASE + i * (1 << 22) for i, name in enumerate(
-    ("a", "w", "out", "out2", "resid", "bias", "gamma", "ln_c1", "head_w", "stats", "q", "k", "v", "x"))}
+    ("a", "w", "out", "out2", "resid", "bias", "gamma", "ln_c1", "head_w", "stats", "q", "k", "v", "x", "pos", "mean", "k4"))}
 
 GEMM = {"a": P["a"], "w": P["w"], "M": 256, "N": 128, "K": 64, "lda": 64, "ldw": 64, "a_mode": 0,
         "bias": P["bias"], "out": P["out"], "out_f32": 1, "ldc": 128, "store_mode": 0}
@@ -35,6 +37,23 @@ ATTN_SPLIT = dict(ATTN, ldq=256, ldk=256, ldv=256, ldo=256, split=1, lo_off_q=12
 HALO = {"x": P["x"], "w": P["w"], "bias": P["bias"], "B": 1, "H": 32, "W": 32, "C": 64, "cstride": 128, "coff": 64, "cout": 64,
         "out": P["out"], "ldc": 64}
 HALO_HEAD = dict(HALO, cout=32, out=0, ldc=0, head_w=P["head_w"], head_out=P["out"])
+LN = {"inp": P["x"], "in_f32": 1, "out": P["out"], "out_f32": 0, "weight": P["w"], "bias": P["bias"], "rows": 100, "dim": 256,
+      "ld_in": 256, "ld_out": 256, "eps": 1e-6}
+LN_SPLIT = dict(LN, ld_out=512, out_split=256)
+V1POST = {"mean": P["mean"], "k4": P["k4"], "B": 1, "net_h": 64, "net_w": 96, "pad_l": 3, "pad_r": 4, "pad_t": 5, "pad_b": 6,
+          "H": 40, "W": 50, "out_depth": P["out"], "out_points": P["out2"]}
+
+
+def call(fn, *args):
+    """a plain-argument launcher: the stream (NULL) is appended"""
+    return {"fn": fn, "args": list(args) + [None]}
+
+
+SOFTMAX = ("udb_softmax_rows", P["x"], P["out"], 300, 100, 128, 128, 0.3)
+CAM4 = ("udb_camera_attn4_f32", P["q"], P["k"], P["pos"], P["out"], 2, 512, 8)
+SPMEAN = ("udb_spatial_mean_f32", P["x"], P["out"], 2, 49, 96)
+COPYROWS = ("udb_copy_rows_f32_to_f16", P["x"], P["out"], 2, 3, 64, 10, 1)
+MEANMAPS = ("udb_v1_mean_maps", P["x"], P["q"], P["k"], P["out"], 1, 4, 6, 64, 96)
 
 # valid calls: they must pass every layout check (and then fail without a device)
 VALID = {
@@ -47,6 +66,10 @@ VALID = {
     "attn": ("attn", ATTN), "attn_split": ("attn", ATTN_SPLIT),
     "attn_slices": ("attn", dict(ATTN, ldq=192, q_col0=64, ldo=200, o_col0=2)),
     "halo": ("halo", HALO), "halo_head": ("halo", HALO_HEAD), "halo_column_slice": ("halo", dict(HALO, out=P["out"] + 4, ldc=66)),
+    "layernorm": ("ln", LN), "layernorm_split": ("ln", LN_SPLIT), "layernorm_f16_small": ("ln", dict(LN, in_f32=0, dim=128, ld_in=128)),
+    "softmax_rows": ("call", call(*SOFTMAX)), "softmax_rows_n_valid_eq_ld": ("call", call(*SOFTMAX[:4], 128, 128, 128, 0.3)),
+    "camera_attn4": ("call", call(*CAM4)), "spatial_mean": ("call", call(*SPMEAN)), "copy_rows": ("call", call(*COPYROWS)),
+    "v1_mean_maps": ("call", call(*MEANMAPS)), "v1_postprocess": ("v1post", V1POST),
 }
 
 # rejected layouts: (which call, struct fields, regexes the error message must match)
@@ -105,6 +128,31 @@ REJECT = {
     "halo_out_misaligned": ("halo", dict(HALO, out=P["out"] + 2), [r"`out`", r"4-byte"]),
     "halo_head_w_null": ("halo", dict(HALO_HEAD, head_w=0), [r"`head_w`"]),
     "halo_bias_null": ("halo", dict(HALO, bias=0), [r"bias"]),
+    # --- LayerNorm: the lo half only exists for f32 -> f16 rows, and it must fit in the row
+    "ln_split_f16_in_small_kernel": ("ln", dict(LN_SPLIT, in_f32=0), [r"`out_split`", r"f32 input"]),
+    "ln_split_f16_in_general": ("ln", dict(LN, in_f32=0, dim=384, ld_in=384, ld_out=768, out_split=384), [r"`out_split`"]),
+    "ln_split_f32_out": ("ln", dict(LN_SPLIT, out_f32=1), [r"`out_split`", r"f16 output"]),
+    "ln_split_negative": ("ln", dict(LN, out_split=-8), [r"`out_split`"]),
+    "ln_ld_out_below_dim": ("ln", dict(LN, ld_out=128), [r"`ld_out`", r"dim"]),
+    "ln_ld_out_below_dim_plus_split": ("ln", dict(LN_SPLIT, ld_out=384), [r"`ld_out`", r"out_split"]),
+    # --- small dense pieces and the V1 tails
+    "softmax_n_valid_past_ld_in": ("call", call(*SOFTMAX[:4], 129, 128, 256, 0.3), [r"n_valid=129", r"ld_in"]),
+    "softmax_n_valid_past_ld_out": ("call", call(*SOFTMAX[:4], 129, 256, 128, 0.3), [r"n_valid=129", r"ld_out"]),
+    "softmax_n_valid0": ("call", call(*SOFTMAX[:4], 0, 128, 128, 0.3), [r"n_valid=0"]),
+    "softmax_rows_negative": ("call", call(*SOFTMAX[:3], -1, *SOFTMAX[4:]), [r"rows=-1"]),
+    "camera_attn4_C_not_multiple_of_heads": ("call", call(*CAM4[:6], 500, 8), [r"C=500", r"heads"]),
+    "camera_attn4_heads0": ("call", call(*CAM4[:6], 512, 0), [r"heads=0"]),
+    "spatial_mean_HW0": ("call", call(*SPMEAN[:4], 0, 96), [r"HW=0", r">= 1"]),
+    "spatial_mean_C0": ("call", call(*SPMEAN[:5], 0), [r"C=0", r">= 1"]),
+    "spatial_mean_B0": ("call", call(*SPMEAN[:3], 0, 49, 96), [r"B=0", r">= 1"]),
+    "copy_rows_D0": ("call", call(*COPYROWS[:5], 0, 10, 1), [r"D=0", r">= 1"]),
+    "copy_rows_groups0": ("call", call(*COPYROWS[:3], 0, 3, 64, 10, 1), [r"groups=0", r">= 1"]),
+    "mean_maps_gh0": ("call", call(*MEANMAPS[:6], 0, 6, 64, 96), [r"gh=0", r">= 1"]),
+    "mean_maps_net_w0": ("call", call(*MEANMAPS[:9], 0), [r"net_w=0", r">= 1"]),
+    "v1_postprocess_crop_h0": ("v1post", dict(V1POST, pad_t=30, pad_b=34), [r"net_h - pad_t - pad_b=0", r">= 1"]),
+    "v1_postprocess_crop_w_negative": ("v1post", dict(V1POST, pad_l=50, pad_r=50), [r"net_w - pad_l - pad_r=-4"]),
+    "v1_postprocess_negative_pad": ("v1post", dict(V1POST, pad_l=-1), [r"paddings"]),
+    "v1_postprocess_H0": ("v1post", dict(V1POST, H=0), [r"H=0", r">= 1"]),
 }
 
 # what a valid call meets after the checks without a device: the tensor-map encoder or the driver
@@ -118,15 +166,19 @@ def _child_main():
     from unidepth_b200 import _cabi
     lib = _cabi.lib()
     structs = {"gemm": (_cabi.Gemm, lib.udb_gemm_f16), "attn": (_cabi.Attn, lib.udb_attention_f16),
-               "halo": (_cabi.ConvHalo, lib.udb_conv3x3_halo_f16)}
+               "halo": (_cabi.ConvHalo, lib.udb_conv3x3_halo_f16), "ln": (_cabi.LayerNorm, lib.udb_layernorm),
+               "v1post": (_cabi.V1Postprocess, lib.udb_v1_postprocess)}
     res = {}
     for name, (kind, fields) in json.load(sys.stdin).items():
-        cls, fn = structs[kind]
-        s = cls()
-        for k, v in fields.items():
-            setattr(s, k, v)
         n0 = lib.udb_launch_count()
-        rc = fn(C.byref(s), None)
+        if kind == "call":
+            rc = getattr(lib, fields["fn"])(*fields["args"])
+        else:
+            cls, fn = structs[kind]
+            s = cls()
+            for k, v in fields.items():
+                setattr(s, k, v)
+            rc = fn(C.byref(s), None)
         res[name] = {"rc": rc, "msg": lib.udb_last_error().decode(), "launched": lib.udb_launch_count() - n0}
     json.dump(res, sys.stdout)
 

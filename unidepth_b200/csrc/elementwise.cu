@@ -315,7 +315,8 @@ __global__ void __launch_bounds__(256) set_cls_rows_ln_kernel(float* x, __half* 
 
 // ------------------------------------------------------------------------------------ camera head (fp32)
 // one warp per output feature and 8 rows (the 32-row camera head is latency bound: favour many
-// small warps over reuse); lanes stride over K with 128-bit loads when K % 128 == 0
+// small warps over reuse); lanes stride over K with 128-bit loads when K % 128 == 0 and every row of x and w starts on
+// a 16-byte boundary (a row-strided view may begin 4 bytes into an allocation); otherwise one float per lane
 __global__ void __launch_bounds__(128) small_linear_kernel(const udb_small_linear_t p) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n = blockIdx.x * 4 + warp;
@@ -326,7 +327,7 @@ __global__ void __launch_bounds__(128) small_linear_kernel(const udb_small_linea
 #pragma unroll
   for (int m = 0; m < 8; ++m) acc[m] = 0.f;
   const float* wr = p.w + (long long)n * p.K;
-  if ((p.K & 127) == 0 && (ldx & 3) == 0) {
+  if ((p.K & 127) == 0 && (ldx & 3) == 0 && ((reinterpret_cast<uintptr_t>(p.x) | reinterpret_cast<uintptr_t>(p.w)) & 15) == 0) {
     for (int k = lane * 4; k < p.K; k += 128) {
       const float4 wv = __ldg(reinterpret_cast<const float4*>(wr + k));
 #pragma unroll
@@ -736,6 +737,15 @@ extern "C" int udb_layernorm_e4m3(const udb_layernorm_t* p, float* out_scale, vo
 }
 
 extern "C" int udb_layernorm(const udb_layernorm_t* p, void* stream) {
+  if (p->out_split < 0 || (p->out_split > 0 && (!p->in_f32 || p->out_f32))) {
+    set_error("udb_layernorm: `out_split` %d needs f32 input and f16 output (in_f32 %d, out_f32 %d)", p->out_split, p->in_f32,
+              p->out_f32);
+    return 1;
+  }
+  if (p->ld_out < (int64_t)p->dim + p->out_split) {
+    set_error("udb_layernorm: `ld_out` %lld < dim %d + out_split %d", (long long)p->ld_out, p->dim, p->out_split);
+    return 1;
+  }
   note_work(0.0, (double)p->rows * p->dim * ((p->in_f32 ? 4 : 2) + (p->out_f32 ? 4 : 2) + (p->out_split ? 2 : 0)));
   if (p->dim_valid < 0 || p->dim_valid > p->dim || p->dim_valid % 8) {
     set_error("udb_layernorm: dim_valid %d must be a multiple of 8 in [0, dim]", p->dim_valid);
@@ -836,6 +846,10 @@ extern "C" int udb_small_linear_f32(const udb_small_linear_t* p, void* stream) {
 }
 
 extern "C" int udb_camera_attn4_f32(const float* q, const float* kv, const float* pos, float* out, int32_t B, int32_t C, int32_t heads, void* stream) {
+  if (B < 1 || heads < 1 || C < heads || C % heads) {
+    set_error("udb_camera_attn4_f32: B=%d, C=%d, heads=%d: needs B >= 1, heads >= 1 and C a multiple of heads", B, C, heads);
+    return 1;
+  }
   const int warps = B * heads * 4;
   camera_attn4_kernel<<<(warps * 32 + 127) / 128, 128, 0, ST(stream)>>>(q, kv, pos, out, B, C, heads);
   return check_launch("camera_attn4_kernel");

@@ -1327,6 +1327,7 @@ int udb_vit_tap_f32(const float* x, float* acc, float* cls_out, int32_t B, int32
 }
 
 int udb_spatial_mean_f32(const float* x, float* out, int32_t B, int32_t HW, int32_t C, void* stream) {
+  if (B < 1 || HW < 1 || C < 1) { set_error("udb_spatial_mean_f32: B=%d HW=%d C=%d must all be >= 1", B, HW, C); return 1; }
   dim3 grid((C + 31) / 32, B);
   spatial_mean_kernel<<<grid, 256, 0, ST(stream)>>>(x, out, HW, C);
   return check_launch("spatial_mean_kernel");
@@ -1402,6 +1403,12 @@ int udb_cross_attn_small_f32(const float* q, const float* q_pos, const float* kv
 }
 
 int udb_softmax_rows(const float* s, void* p, int64_t rows, int32_t n_valid, int32_t ld_in, int32_t ld_out, float scale, void* stream) {
+  if (rows < 0 || n_valid < 1 || n_valid > ld_in || n_valid > ld_out) {
+    set_error("udb_softmax_rows: rows=%lld n_valid=%d ld_in=%d ld_out=%d: needs rows >= 0 and 1 <= n_valid <= ld_in, ld_out",
+              (long long)rows, n_valid, ld_in, ld_out);
+    return 1;
+  }
+  if (rows == 0) return 0;
   softmax_rows_kernel<<<(int)((rows + 7) / 8), 256, 0, ST(stream)>>>(s, reinterpret_cast<__half*>(p), rows, n_valid, ld_in, ld_out, scale);
   return check_launch("softmax_rows_kernel");
 }
@@ -1416,6 +1423,10 @@ int udb_add_f32(const float* a, const float* b, float* out, void* out_f16, int64
 
 int udb_copy_rows_f32_to_f16(const float* src, void* dst, int32_t groups, int32_t rows_per_group, int32_t D, int64_t dst_group_stride,
                              int64_t dst_row0, void* stream) {
+  if (groups < 1 || rows_per_group < 1 || D < 1) {
+    set_error("udb_copy_rows_f32_to_f16: groups=%d rows_per_group=%d D=%d must all be >= 1", groups, rows_per_group, D);
+    return 1;
+  }
   copy_rows_f16_kernel<<<grid_1d((long long)groups * rows_per_group * D), 256, 0, ST(stream)>>>(src, reinterpret_cast<__half*>(dst), groups,
                                                                                                 rows_per_group, D, dst_group_stride, dst_row0);
   return check_launch("copy_rows_f16_kernel");
@@ -1496,11 +1507,22 @@ int udb_nystrom_zk3(const float* z, const void* k3, int32_t ldk3, void* out, int
 
 int udb_v1_mean_maps(const float* o8, const float* o4, const float* o2, float* mean, int32_t B, int32_t gh, int32_t gw, int32_t net_h,
                      int32_t net_w, void* stream) {
+  const struct { int v; const char* name; } dims[] = {{B, "B"}, {gh, "gh"}, {gw, "gw"}, {net_h, "net_h"}, {net_w, "net_w"}};
+  for (const auto& d : dims)
+    if (d.v < 1) { set_error("udb_v1_mean_maps: %s=%d must be >= 1", d.name, d.v); return 1; }
   v1_mean_maps_kernel<<<grid_1d((long long)B * net_h * net_w), 256, 0, ST(stream)>>>(o8, o4, o2, mean, B, gh, gw, net_h, net_w);
   return check_launch("v1_mean_maps_kernel");
 }
 
 int udb_v1_postprocess(const udb_v1_postprocess_t* p, void* stream) {
+  const struct { int v; const char* name; } dims[] = {{p->B, "B"}, {p->H, "H"}, {p->W, "W"},
+                                                       {p->net_h - p->pad_t - p->pad_b, "net_h - pad_t - pad_b"},
+                                                       {p->net_w - p->pad_l - p->pad_r, "net_w - pad_l - pad_r"}};
+  for (const auto& d : dims)
+    if (d.v < 1) { set_error("udb_v1_postprocess: %s=%d must be >= 1", d.name, d.v); return 1; }
+  const int pads[] = {p->pad_l, p->pad_r, p->pad_t, p->pad_b};
+  for (int i = 0; i < 4; ++i)
+    if (pads[i] < 0) { set_error("udb_v1_postprocess: paddings (pad_l, pad_r, pad_t, pad_b) must be >= 0"); return 1; }
   v1_postprocess_kernel<<<grid_1d((long long)p->B * p->H * p->W), 256, 0, ST(stream)>>>(*p);
   return check_launch("v1_postprocess_kernel");
 }
