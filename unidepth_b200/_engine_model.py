@@ -106,6 +106,11 @@ class EngineModel(nn.Module):
     def _fingerprint(self):
         return tuple((p.data_ptr(), p._version) for p in self.parameters())
 
+    def _pack_weights(self, dev):
+        """The operands that depend on the weights alone, packed once per weight version: by default all of
+        `_pack_tensors`."""
+        return self._pack_tensors(dev)
+
     def _weights(self):
         """The packed (tensors, scalars), repacked once per weight version; a repack drops the engine and its caches."""
         if self._packed is None or self._packed_key != self._fingerprint():
@@ -115,7 +120,7 @@ class EngineModel(nn.Module):
                                    "(model.to('cuda')); there is no CPU fallback")
             torch.cuda.set_device(dev)      # callers hold `with torch.cuda.device(self.device)`
             self._drop_engine()             # it borrows the pointers of the tensors about to be replaced
-            self._packed = self._pack_tensors(dev)
+            self._packed = self._pack_weights(dev)
             self._packed_key = self._fingerprint()
         return self._packed
 
@@ -132,16 +137,26 @@ class EngineModel(nn.Module):
         for name, v in scalars.items():
             cabi.check(getattr(lib, set_scalar)(handle, name.encode(), float(v)), f"{set_scalar}({name})")
 
-    def _create_engine(self, cfg, key=None):
-        """A new engine for the config struct `cfg`, with the current packed weights registered; `key` is what the
-        caller compares to decide when to rebuild it."""
-        tensors, scalars = self._weights()
-        create = self._ENGINE_FNS[0]
+    def _create_engine(self, cfg, key=None, tensors=None, check=None):
+        """A new engine for the config struct `cfg`, with `tensors` (default: the packed weights) and the packed scalars
+        registered; `key` is what the caller compares to decide when to rebuild it.  `check(handle)` may refuse the new
+        engine by raising: it is destroyed and the current engine stays as it was.  Otherwise the new engine replaces the
+        current one, which is dropped with its workspaces and graphs."""
+        packed, scalars = self._weights()
+        tensors = packed if tensors is None else tensors
+        create, destroy = self._ENGINE_FNS[:2]
         handle = C.c_void_p()
         cabi.check(getattr(cabi.lib(), create)(C.byref(cfg), C.byref(handle)), create)
-        for name, t in tensors.items():
-            assert t.is_cuda, name
-        self._register(handle, tensors, scalars)
+        try:
+            for name, t in tensors.items():
+                assert t.is_cuda, name
+            self._register(handle, tensors, scalars)
+            if check is not None:
+                check(handle)
+        except BaseException:
+            getattr(cabi.lib(), destroy)(handle)
+            raise
+        self._drop_engine()
         self._engine, self._engine_key, self._engine_device = handle, key, self.device
         return handle
 

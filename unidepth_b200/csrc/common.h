@@ -22,6 +22,10 @@ void note_work(double flops, double bytes);
 
 int num_sms();   // of the CURRENT device (cached per device)
 
+// Shape bounds of udb_cross_attn_small(_f32): 0, or 1 with the error set under the name `fn`.  The V1 engine checks its
+// camera head's context length with it before anything is enqueued, so that its dry run names the bound.
+int cross_attn_small_check(const char* fn, int nq, int nk, int D);
+
 // true the first time it is called on the current device for this mask (per-device one-time setup such as
 // cudaFuncSetAttribute: function attributes are per device / context, not per process)
 inline bool first_on_device(std::atomic<uint64_t>& mask) {

@@ -356,6 +356,19 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
     sh[0] = (net_h - 4) / 4 + 1; sw[0] = (net_w - 4) / 4 + 1;
     for (int i = 1; i < 4; ++i) { sh[i] = sh[i - 1] / 2; sw[i] = sw[i - 1] / 2; }
   }
+  // Bounds the network grid puts on the kernels, checked here so that the dry run names them before anything is launched:
+  // the 1/8 and 1/4 decoder levels run Nystrom attention with 128 landmarks, which needs more tokens than landmarks (the
+  // reference's xformers module pools segments of seq // 128 rows, and switches to exact attention at exactly 128), and
+  // the camera head's single-head cross attention over the 4*hc*wc + 4 context tokens has a shared-memory bound.
+  {
+    const int n8 = 4 * sh[2] * sw[2];
+    if (n8 <= 128) {
+      set_error("udb_v1: network shape %dx%d gives %d tokens at the 1/8 decoder level (%dx%d); Nystrom attention needs more "
+                "than its 128 landmarks", net_h, net_w, n8, 2 * sh[2], 2 * sw[2]);
+      return 1;
+    }
+    if (cross_attn_small_check("udb_v1: camera head cross attention", 4, 4 * sh[2] * sw[2] + 4, hid)) return 1;
+  }
   Stage stage;
   // "precision": 0 (absent) = f16 operands, 2 = e4m3 operands for the encoder blocks' MLP (ConvNeXt) or all four linear
   // layers (DINOv2); the stem, downsample layers and the decoder are the same in both.  1 = split-f16 operands (parity

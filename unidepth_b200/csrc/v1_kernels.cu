@@ -1365,14 +1365,22 @@ int udb_v1_camera_intrinsics(const float* x4, const float* gt_k, int32_t B, int3
 }  // extern "C"
 
 namespace udb {
+int cross_attn_small_check(const char* fn, int nq, int nk, int D) {
+  if (nq < 1 || nq > CA_MAXQ || D % 256) { set_error("%s: nq=%d D=%d unsupported (nq <= 4, D %% 256 == 0)", fn, nq, D); return 1; }
+  // the partial kernel stages the nq queries and the scores of one split's keys in shared memory (at most 200 KB)
+  const int chunk = (nk + CA_SPLITS - 1) / CA_SPLITS;
+  if ((size_t)(nq * D + nq * chunk + 16) * 4 > 200 * 1024) { set_error("%s: nk=%d too large for nq=%d D=%d", fn, nk, nq, D); return 1; }
+  return 0;
+}
+
 // udb_cross_attn_small / udb_cross_attn_small_f32: f16 or f32 (k | v) rows
 template <class KV>
 static int cross_attn_small(const char* fn, const float* q, const float* q_pos, const KV* kv, float* out, float* scratch, int B, int nq, int nk,
                             int D, float scale, void* stream) {
-  if (nq < 1 || nq > CA_MAXQ || D % 256 || !scratch) { set_error("%s: nq=%d D=%d unsupported (nq <= 4, D %% 256 == 0)", fn, nq, D); return 1; }
+  if (!scratch) { set_error("%s: nq=%d D=%d unsupported (nq <= 4, D %% 256 == 0)", fn, nq, D); return 1; }
+  if (cross_attn_small_check(fn, nq, nk, D)) return 1;
   const int chunk = (nk + CA_SPLITS - 1) / CA_SPLITS;
   const size_t smem = (size_t)(nq * D + nq * chunk + 16) * 4;
-  if (smem > 200 * 1024) { set_error("%s: nk=%d too large", fn, nk); return 1; }
   static std::atomic<size_t> set_for[64];
   int dev = 0;
   cudaGetDevice(&dev);

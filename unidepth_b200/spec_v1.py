@@ -1,5 +1,5 @@
 """Static description of UniDepthV1 (ConvNeXt-L or DINOv2 ViT-L/14 encoder) for the inference path: hyper-parameters
-read from the reference's config format, the parameter table under the reference's state-dict names, and the fixed-shape
+read from the reference's config format, the parameter table under the reference's state-dict names, and the shape
 arithmetic of `infer` (reference: unidepth/models/unidepthv1/unidepthv1.py:30-46 `_paddings` / `_shapes`,
 :416-447 `build`; unidepthv1/decoder.py:465-533 `Decoder.build`; backbones/convnext.py:301-448, backbones/dinov2.py)."""
 from __future__ import annotations
@@ -60,7 +60,7 @@ class V1Spec:
         self.dec_depths = tuple(m["pixel_decoder"]["depths"])    # blocks at 1/16, 1/8 (Nystrom), 1/4 (Nystrom)
         self.heads = m["num_heads"]
         self.expansion = m["expansion"]
-        self.image_shape = tuple(config["data"]["image_shape"])  # fixed network input (462, 616)
+        self.image_shape = tuple(config["data"]["image_shape"])  # the config's network input (462, 616)
         # decoder.py:489-492: token adapters read the cls tokens of the last four BLOCKS, newest first
         per_block = [c for d, c in zip(self.depths, self.dims) for _ in range(d)]
         self.cls_dims = tuple(per_block[-i - 1] for i in range(4))
@@ -69,19 +69,21 @@ class V1Spec:
         if self.encoder == ENCODER_DINOV2 and (self.image_shape[0] % PATCH or self.image_shape[1] % PATCH):
             raise NotImplementedError(f"network shape {self.image_shape} is not a multiple of the {PATCH}-pixel patch")
 
-    def common_grid(self) -> Tuple[int, int]:
-        """(hc, wc): the decoder's common token grid (decoder.py:381-392, the second-smallest level).  ConvNeXt: stride-4
-        stem then two 2x downsamples; DINOv2: the single 14-pixel patch grid (462x616 -> 33x44)."""
+    def common_grid(self, image_shape=None) -> Tuple[int, int]:
+        """(hc, wc): the decoder's common token grid (decoder.py:381-392, the second-smallest level) of the network shape
+        `image_shape` (default: the config's).  ConvNeXt: stride-4 stem then two 2x downsamples; DINOv2: the single
+        14-pixel patch grid (462x616 -> 33x44)."""
+        net_h, net_w = self.image_shape if image_shape is None else image_shape
         if self.encoder == ENCODER_DINOV2:
-            return self.image_shape[0] // PATCH, self.image_shape[1] // PATCH
-        sh = [(self.image_shape[0] - 4) // 4 + 1, (self.image_shape[1] - 4) // 4 + 1]
+            return net_h // PATCH, net_w // PATCH
+        sh = [(net_h - 4) // 4 + 1, (net_w - 4) // 4 + 1]
         for _ in range(2):
             sh = [sh[0] // 2, sh[1] // 2]
         return sh[0], sh[1]
 
 
 def v1_shapes(image_hw: Tuple[int, int], network_hw: Tuple[int, int]):
-    """unidepthv1.py:38-46: ((h', w'), ratio) of the aspect-preserving resize into the fixed network shape."""
+    """unidepthv1.py:38-46: ((h', w'), ratio) of the aspect-preserving resize into the network shape."""
     h, w = image_hw
     if network_hw[1] / network_hw[0] > w / h:
         ratio = network_hw[0] / h

@@ -20,12 +20,14 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-from typing import Dict, Optional
+import operator
+from typing import Dict, Optional, Tuple
 
 import torch
 import torch.nn.functional as F
 
 from . import _cabi as cabi
+from .spec import PATCH
 from .spec_v1 import (ENCODER_CONVNEXT, ENCODER_DINOV2, V1_INTERPOLATE_OFFSET, V1Spec, param_shapes, v1_paddings,
                       v1_shapes)
 from ._engine_model import HUB_KWARGS, EngineModel, PyTorchModelHubMixin, f16, f32
@@ -48,8 +50,8 @@ def split_weight(w: torch.Tensor) -> torch.Tensor:
 def _offset_pos_embed(pos: torch.Tensor, gh: int, gw: int, offset: float) -> torch.Tensor:
     """DINOv2 position table of a gh x gw patch grid with a nonzero interpolate_offset (dinov2.py:267-304): bicubic
     resize of the M x M grid with scale factors ((gh + offset) / M, (gw + offset) / M), height first, so the sampling
-    positions use 1 / scale_factor rather than M / gh.  pos [1 + M*M, D] -> [1 + gh*gw, D], cls row first.  UniDepthV1
-    runs one fixed network shape, so this is a constant of the weights, evaluated at pack time."""
+    positions use 1 / scale_factor rather than M / gh.  pos [1 + M*M, D] -> [1 + gh*gw, D], cls row first.  A constant
+    of the weights and the network shape, evaluated when the engine for that shape is made."""
     D = pos.shape[1]
     M = math.isqrt(pos.shape[0] - 1)
     grid = pos[1:].float().reshape(1, M, M, D).permute(0, 3, 1, 2)
@@ -62,7 +64,7 @@ def _offset_pos_embed(pos: torch.Tensor, gh: int, gw: int, offset: float) -> tor
 def _sine_position_embedding(h: int, w: int, num_pos_feats: int, device) -> torch.Tensor:
     """PositionEmbeddingSine(num_pos_feats, normalize=True) of an all-valid h x w grid -> [h*w, 2*num_pos_feats]
     (layers/positional_encoding.py:15-59: y features then x features, sin on even / cos on odd feature indices).
-    Evaluated once per weight version on the host side (a constant of the shape)."""
+    Evaluated on the host side when the engine for a network shape is made (a constant of the shape)."""
     eps, scale = 1e-6, 2 * math.pi
     y = torch.arange(1, h + 1, dtype=f32, device=device)[:, None].expand(h, w) / (h + eps) * scale
     x = torch.arange(1, w + 1, dtype=f32, device=device)[None, :].expand(h, w) / (w + eps) * scale
@@ -81,7 +83,9 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         super().__init__(config, eps, max_cached_workspaces=4)
         self.spec = V1Spec(config)
         self._add_params(param_shapes(config))
-        self.image_shape = list(self.spec.image_shape)        # unidepthv1.py:447
+        # the network shape `infer` resizes and pads every input to (unidepthv1.py:443), read on every call as the
+        # reference does: [height, width], landscape or square (see _network_shape)
+        self.image_shape = list(self.spec.image_shape)
         # "f16" (default) or "fp8": speed mode -- the linear layers of the encoder blocks multiply FP8 E4M3 operands on the
         # e4m3 wgmma (include/udb.h udb_gemm_e4m3): weights with one scale per output channel, activations quantised per
         # row on the fly.  DINOv2 ViT-L: qkv, proj, fc1 and fc2, as UniDepthV2's fp8 mode.  ConvNeXt: the two MLP layers of
@@ -97,11 +101,62 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
     def _fingerprint(self):
         return (self.precision,) + super()._fingerprint()
 
+    def _network_shape(self) -> Tuple[int, int]:
+        """`image_shape` as (net_h, net_w), checked before anything is packed or launched for it."""
+        shp = self.image_shape
+        try:
+            h, w = shp
+            if isinstance(h, bool) or isinstance(w, bool):
+                raise TypeError
+            h, w = operator.index(h), operator.index(w)
+        except (TypeError, ValueError):
+            raise ValueError(f"UniDepthV1.image_shape must be two integers [height, width], not {shp!r}") from None
+        if h < 64 or w < 64:
+            raise ValueError(f"UniDepthV1.image_shape {[h, w]}: each side must be at least 64 pixels")
+        if self.spec.encoder == ENCODER_DINOV2 and (h % PATCH or w % PATCH):
+            raise NotImplementedError(f"network shape {(h, w)} is not a multiple of the {PATCH}-pixel patch")
+        if h > w:
+            raise NotImplementedError(
+                f"UniDepthV1.image_shape {[h, w]}: portrait network shapes are not supported.  The reference's decoder "
+                "orders every token grid as sorted([h, w]) (decoder.py:384-396), so it runs a portrait shape as its "
+                "transpose; use a landscape or square shape (height <= width)")
+        return h, w
+
     # ------------------------------------------------------------------ weight packing
     def _pack_tensors(self, dev):
-        """({engine tensor name: tensor on `dev`}, {scalar name: float}): plain torch layout work.  `_weights` is the only
-        product caller (CUDA device); tests/test_engine_schedule_cpu.py runs it on the CPU to check, through the engine's
-        dry run, that the packer registers exactly the operands the C schedule asks for."""
+        """({engine tensor name: tensor on `dev`}, {scalar name: float}): plain torch layout work, the weights and the
+        two operands of the network shape `image_shape`.  The product packs the two parts separately (`_weights`,
+        `_shape_operands`); tests/test_engine_schedule_cpu.py runs this on the CPU to check, through the engine's dry run,
+        that the packer registers exactly the operands the C schedule asks for."""
+        T, S = self._pack_weights(dev)
+        T.update(self._shape_operands(self._network_shape(), dev))
+        return T, S
+
+    def _shape_operands(self, shape: Tuple[int, int], dev) -> Dict[str, torch.Tensor]:
+        """The operands that depend on the network shape: "tokens_pos", the sine position embedding of the decoder's
+        common grid plus the level embedding MLP of the four learned level vectors (decoder.py:410-433), and for DINOv2
+        "pos", the patch grid's position table (dinov2.py:267-304)."""
+        s = self.spec
+        sd = self.state_dict()
+        pd = "pixel_decoder."
+        hid = s.hidden
+        hc, wc = s.common_grid(shape)
+        c32 = lambda t: t.to(f32).contiguous()
+        T: Dict[str, torch.Tensor] = {}
+        if s.encoder == ENCODER_DINOV2:
+            pos = c32(sd["pixel_encoder.pos_embed"].detach().reshape(-1, s.embed_dim))
+            T["pos"] = c32(_offset_pos_embed(pos, hc, wc, V1_INTERPOLATE_OFFSET))
+        le = F.linear(F.gelu(F.linear(sd[pd + "level_embeds"].float(), sd[pd + "level_embed_layer.0.weight"].float(),
+                                      sd[pd + "level_embed_layer.0.bias"].float())),
+                      sd[pd + "level_embed_layer.2.weight"].float(), sd[pd + "level_embed_layer.2.bias"].float())
+        le = F.layer_norm(le, (hid,), sd[pd + "level_embed_layer.3.weight"].float(), sd[pd + "level_embed_layer.3.bias"].float(), 1e-5)
+        pos = _sine_position_embedding(hc, wc, hid // 2, dev)
+        T["tokens_pos"] = c32((pos[None, :, :] + le[:, None, :]).reshape(4 * hc * wc, hid))
+        return T
+
+    def _pack_weights(self, dev):
+        """The weight operands and scalars: everything but `_shape_operands`, so a change of network shape repacks
+        nothing here."""
         s = self.spec
         if self.precision not in ("split", "f16", "fp8"):
             raise ValueError(f"precision must be 'split', 'f16' or 'fp8', not {self.precision!r}")
@@ -144,13 +199,12 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
                 T[dst + "w1"], T[dst + "w2"] = enc16(sd[f"{src}{fc1}.weight"]), enc16(sd[f"{src}{fc2}.weight"])
             T[dst + "gamma"] = c32(sd[f"{src}gamma"])
 
-        hc, wc = s.common_grid()
         # ---- encoder
         if s.encoder == ENCODER_DINOV2:
             # the V2 encoder's f16 or fp8 packing; the final norm, mask token and register tokens are never read
-            # (use_norm=False, dinov2.py:173-178)
+            # (use_norm=False, dinov2.py:173-178).  Its "pos" is the checkpoint's grid: the shape's table replaces it.
             T.update(pack_vit_encoder(sd, s.embed_dim, s.enc_depth, dev, split=split, fp8=fp8))
-            T["pos"] = c32(_offset_pos_embed(T["pos"], hc, wc, V1_INTERPOLATE_OFFSET))
+            del T["pos"]
         for i, depth in enumerate(s.depths if s.encoder == ENCODER_CONVNEXT else ()):
             if i == 0:
                 T["stem_w"] = s16(zpad(sd[pe + "stem.0.weight"].reshape(s.dims[0], 48), s.dims[0], 64))
@@ -174,14 +228,6 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
             t = f"{pd}token_adapter.input_adapters.{l}"
             T[f"tok.{l}.ln_w"], T[f"tok.{l}.ln_b"] = c32(sd[t + ".0.weight"]), c32(sd[t + ".0.bias"])
             T[f"tok.{l}.w"], T[f"tok.{l}.b"] = c32(sd[t + ".1.weight"]), c32(sd[t + ".1.bias"])
-        # level embedding MLP of the four learned level vectors + sine position embedding of the common grid
-        # (decoder.py:410-433): constants of (weights, network shape), folded once here
-        le = F.linear(F.gelu(F.linear(sd[pd + "level_embeds"].float(), sd[pd + "level_embed_layer.0.weight"].float(),
-                                      sd[pd + "level_embed_layer.0.bias"].float())),
-                      sd[pd + "level_embed_layer.2.weight"].float(), sd[pd + "level_embed_layer.2.bias"].float())
-        le = F.layer_norm(le, (hid,), sd[pd + "level_embed_layer.3.weight"].float(), sd[pd + "level_embed_layer.3.bias"].float(), 1e-5)
-        pos = _sine_position_embedding(hc, wc, hid // 2, dev)
-        T["tokens_pos"] = c32((pos[None, :, :] + le[:, None, :]).reshape(4 * hc * wc, hid))
 
         def mlp32(dst, src):
             T[dst + ".nw"], T[dst + ".nb"] = c32(sd[src + ".norm.weight"]), c32(sd[src + ".norm.bias"])
@@ -268,22 +314,35 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         cfg.hidden, cfg.heads, cfg.expansion = s.hidden, s.heads, s.expansion
         for i in range(3):
             cfg.dec_depths[i] = s.dec_depths[i]
-        cfg.net_h, cfg.net_w = self.image_shape
+        cfg.net_h, cfg.net_w = self._network_shape()
         cfg.encoder = s.encoder
         return cfg
 
     def _get_engine(self):
-        self._weights()
-        if self._engine is not None:
+        """The engine of the current network shape.  A new shape makes a new engine with the packed weights and the
+        shape's own operands; the previous engine, its workspaces and its graphs are dropped only once the new one has
+        passed a dry run, which names any bound the shape breaks before anything is launched."""
+        T, _ = self._weights()
+        shape = self._network_shape()
+        if self._engine is not None and self._engine_key == shape:
             return self._engine
-        return self._create_engine(self._engine_config())
+        ops = self._shape_operands(shape, self.device)
+
+        def check(handle):
+            lib = cabi.lib()
+            if lib.udb_v1_workspace_bytes(handle, 1, *shape) == 0:
+                raise NotImplementedError(f"UniDepthV1.image_shape {list(shape)}: {lib.udb_last_error().decode()}")
+
+        handle = self._create_engine(self._engine_config(), shape, tensors={**T, **ops}, check=check)
+        self._shape_ops = ops              # the engine borrows their pointers
+        return handle
 
     def _forward_engine(self, rgb: torch.Tensor, K: Optional[torch.Tensor], skip_camera: bool, scale255: bool, normalize: bool):
         eng = self._get_engine()
         lib = cabi.lib()
         dev = rgb.device
         B, _, H, W = rgb.shape
-        ws = self._workspace((B, H, W), lambda: lib.udb_v1_workspace_bytes(eng, B, H, W))
+        ws = self._workspace((self._engine_key, B, H, W), lambda: lib.udb_v1_workspace_bytes(eng, B, H, W))
         out = {"intrinsics": torch.empty((B, 3, 3), device=dev, dtype=f32),
                "points": torch.empty((B, 3, H, W), device=dev, dtype=f32),
                "depth": torch.empty((B, 1, H, W), device=dev, dtype=f32)}
@@ -305,6 +364,7 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
             rgbs = rgbs.unsqueeze(0)
         if intrinsics is not None and intrinsics.ndim == 2:
             intrinsics = intrinsics.unsqueeze(0)
+        shape = self._network_shape()
         dev = self.device
         if dev.type != "cuda":
             raise RuntimeError("unidepth_b200 has no CPU path: move the model to a CUDA device")
@@ -328,9 +388,9 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
                 if K.shape[0] != B:
                     raise ValueError(f"intrinsics holds {K.shape[0]} matrices for a batch of {B} images")
                 K = K.contiguous()
-            self._weights()
+            self._get_engine()
             run = lambda x, inputs: self._forward_engine(x, inputs.get("K"), skip_camera, scale255, normalize)
-            key = (tuple(rgbs.shape), rgbs.dtype, scale255, normalize, K is not None, bool(skip_camera))
+            key = (shape, tuple(rgbs.shape), rgbs.dtype, scale255, normalize, K is not None, bool(skip_camera))
             return self._run_graphed(run, rgbs, {} if K is None else {"K": K}, key)
 
     def forward(self, *args, **kwargs):
