@@ -2,7 +2,7 @@
 
     model = torch.hub.load(<this repo>, "UniDepth", version="v2", backbone="vitl14", pretrained=True, source="local")
 
-UniDepthV2 (ViT-L/B/S) and UniDepthV1 with the ConvNeXt-L encoder are implemented on the CUDA path (SURVEY.md section 8);
+UniDepthV2 (ViT-L/B/S), UniDepthV2old (ViT-L/S) and UniDepthV1 with the ConvNeXt-L encoder are implemented on the CUDA path (SURVEY.md section 8);
 the other entries the reference lists raise NotImplementedError instead of silently loading something else."""
 dependencies = ["torch"]
 
@@ -10,12 +10,12 @@ import json
 import os
 
 _HERE = os.path.dirname(os.path.realpath(__file__))
-_SUPPORTED = {"v2": ("vitl14", "vitb14", "vits14"), "v1": ("cnvnxtl",)}
-_KNOWN_ELSEWHERE = {"v1": ("vitl14",), "v2old": ("vitl14", "vits14")}
+_SUPPORTED = {"v2": ("vitl14", "vitb14", "vits14"), "v1": ("cnvnxtl",), "v2old": ("vitl14", "vits14")}
+_KNOWN_ELSEWHERE = {"v1": ("vitl14",)}
 
 
 def UniDepth(version="v2", backbone="vitl14", pretrained=True):
-    from unidepth_b200 import UniDepthV1, UniDepthV2
+    from unidepth_b200 import UniDepthV1, UniDepthV2, UniDepthV2old
 
     if version not in _SUPPORTED and version not in _KNOWN_ELSEWHERE:
         raise AssertionError(f"version must be one of {sorted(set(_SUPPORTED) | set(_KNOWN_ELSEWHERE))}")
@@ -25,7 +25,7 @@ def UniDepth(version="v2", backbone="vitl14", pretrained=True):
         raise AssertionError(f"backbone for version {version} must be one of {list(_SUPPORTED.get(version, ()))}")
     cfg_path = os.path.join(_HERE, "unidepth_b200", "configs", f"config_{version}_{backbone}.json")
     with open(cfg_path) as fh:
-        model = (UniDepthV1 if version == "v1" else UniDepthV2)(json.load(fh))
+        model = {"v1": UniDepthV1, "v2": UniDepthV2, "v2old": UniDepthV2old}[version](json.load(fh))
     if pretrained:
         # same checkpoint location as the reference; needs network access (or a warm HF cache)
         import torch

@@ -334,6 +334,10 @@ typedef struct udb_ray_embed_t {
   int32_t out_f32;
 } udb_ray_embed_t;
 int udb_ray_embed(const udb_ray_embed_t* p, void* stream);
+/* The same resampled unit rays as UniDepthV2old's ray features (decoder_old.py:111-121, positional_embedding.py:218-256
+ * with use_log and cat_orig): sin(pi * scales[k] * axis) for the three axes of the ray (axis-major, 3*bands features),
+ * then the ray itself, zero-filled up to the row stride ld_out >= 3*bands + 3 */
+int udb_ray_embed_cat_orig(const udb_ray_embed_t* p, int32_t ld_out, void* stream);
 
 /* x2 bilinear up-sample, align_corners=False (layers/upsample.py:215), NHWC f16 -> f16.
  * Optionally fused: out = up(x) is followed by nothing; see udb_gemm for the convT add. */
@@ -726,6 +730,99 @@ typedef struct udb_infer_v1_args_t {
 } udb_infer_v1_args_t;
 
 int udb_infer_v1(udb_engine_v1* e, const udb_infer_v1_args_t* a, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * UniDepthV2old engine: the whole `UniDepthV2old.infer` path (DINOv2 ViT-L/14 or ViT-S/14) as one call (reference
+ * unidepth/models/unidepthv2/unidepthv2_old.py:198-282, decoder_old.py).  One engine per network shape (net_h, net_w),
+ * which `udb_v2old_geometry` derives from the input size and the resolution level; otherwise the contract of the V1 engine:
+ * the caller owns the packed weights (names in unidepth_b200/unidepthv2old.py::_pack_tensors), workspace and outputs, and
+ * nothing is allocated, copied or synchronised inside udb_infer_v2old.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct udb_engine_v2old udb_engine_v2old;
+
+typedef struct udb_v2old_config_t {
+  int32_t embed_dim, enc_depth, enc_heads;  /* DINOv2: 1024 / 24 / 16 (ViT-L) or 384 / 12 / 6 (ViT-S) */
+  int32_t output_idx[4];  /* encoder blocks (1-based) whose normed patch tokens feed the decoder (21..24 or 9..12) */
+  int32_t hidden, heads, expansion;   /* 512 / 8 / 4 */
+  int32_t nystrom_depth;  /* Nystrom blocks at the first decoder level (config pixel_decoder.depths[0]: 6) */
+  int32_t net_h, net_w;   /* the network shape, multiples of 14 */
+} udb_v2old_config_t;
+
+int udb_v2old_create(const udb_v2old_config_t* cfg, udb_engine_v2old** out);
+void udb_v2old_destroy(udb_engine_v2old* e);
+int udb_v2old_set_weight(udb_engine_v2old* e, const char* name, const void* dev_ptr, const int64_t* shape, int32_t ndim,
+                         int32_t dtype);
+int udb_v2old_set_scalar(udb_engine_v2old* e, const char* name, double value);
+/* Shape arithmetic of `infer` (unidepthv2_old.py:45-92): the pixel count of `resolution_level` (clipped to [0, 10]; pass
+ * 10 for the reference's None) between pixels_lo and pixels_hi patches, and the network shape with the input's aspect
+ * ratio at that many patches (both sides multiples of 14), with ratio = net_h / H.  The reference's warnings (level out
+ * of range, aspect ratio out of bounds) are the caller's. */
+typedef struct udb_v2old_geometry_t {
+  int32_t pixels;          /* patches of the resolution level */
+  int32_t net_h, net_w;
+  double ratio;
+} udb_v2old_geometry_t;
+int udb_v2old_geometry(int32_t H, int32_t W, int32_t resolution_level, int32_t pixels_lo, int32_t pixels_hi,
+                       udb_v2old_geometry_t* out);
+/* bytes of workspace udb_infer_v2old needs for (B, H, W) (0 + udb_last_error on failure), from a dry run of the
+ * schedule that launches nothing: udb_v2old_schedule_bytes only sizes (and names the first missing or mis-shaped
+ * operand), udb_v2old_workspace_bytes also records the shape as prepared; call it once per (B, H, W) before
+ * udb_infer_v2old, outside stream capture. */
+size_t udb_v2old_schedule_bytes(udb_engine_v2old* e, int32_t B, int32_t H, int32_t W);
+size_t udb_v2old_workspace_bytes(udb_engine_v2old* e, int32_t B, int32_t H, int32_t W);
+
+#define UDB_V2OLD_BILINEAR 0
+#define UDB_V2OLD_NEAREST_EXACT 1
+
+typedef struct udb_infer_v2old_args_t {
+  const void* rgb;         /* [B,3,H,W] uint8 or float32 */
+  int32_t rgb_is_u8;
+  int32_t scale255;        /* divide by 255 first (uint8, or float data with max > 5) */
+  int32_t normalize;       /* ImageNet mean / std (data in [0,1] after the optional /255) */
+  int32_t B, H, W;
+  const float* intrinsics; /* optional GT pinhole K [B,3,3] (input image frame): rays and points use it */
+  int32_t interpolation;   /* depth resize to H x W: UDB_V2OLD_BILINEAR or UDB_V2OLD_NEAREST_EXACT */
+  void* workspace;
+  size_t workspace_bytes;
+  float* out_intrinsics;   /* [B,3,3] predicted K at the input size */
+  float* out_points;       /* [B,3,H,W] */
+  float* out_depth;        /* [B,1,H,W] */
+  float* out_confidence;   /* [B,1,H,W] */
+} udb_infer_v2old_args_t;
+
+int udb_infer_v2old(udb_engine_v2old* e, const udb_infer_v2old_args_t* a, void* stream);
+
+/* Kernels of the UniDepthV2old decoder no other model runs (unidepth_b200/csrc/v1_kernels.cu). */
+/* PixelShuffle(2) of NHWC f16 [B,h,w,C] -> depthwise 7x7 (zero pad; w tap-major [49, C/4] f32, bias [C/4]) -> ReLU ->
+ * NHWC f16 [B,2h,2w,ldo], channels C/4..ldo-1 zero (layers/upsample.py:110-121 before the 3x3 conv) */
+int udb_pshuffle_dw7_relu(const void* x, const float* w, const float* bias, void* out, int32_t B, int32_t h, int32_t wd, int32_t C,
+                          int32_t ldo, void* stream);
+typedef struct udb_v2old_heads_t {
+  const float* levels[3];  /* level i: f32 NHWC [B, 2gh<<i, 2gw<<i, 32] = [depth MLP 16 | confidence MLP 16] */
+  const float* w;          /* [2][48][49]: to_depth then to_confidence, input channel block 2-i for level i */
+  float bias_depth, bias_conf;
+  int32_t B, gh, gw, net_h, net_w;
+  float* logdepth;         /* [B, net_h, net_w] */
+  float* confidence;       /* [B, net_h, net_w], after the sigmoid */
+} udb_v2old_heads_t;
+int udb_v2old_heads(const udb_v2old_heads_t* p, void* stream);
+/* in place on [B, hw] log-depth: LayerNorm over each map, exp, (x + shift) * exp(log_scale), softplus(beta 10);
+ * scale_shift [B, 2] = (log_scale, shift) */
+int udb_v2old_depth_tail(float* depth, const float* scale_shift, int32_t B, int64_t hw, void* stream);
+typedef struct udb_v2old_postprocess_t {
+  const float* depth;      /* [B, net_h, net_w] */
+  const float* confidence; /* [B, net_h, net_w] */
+  const float* k4;         /* [B, 4] fx, fy, cx, cy of the points' K at the input size */
+  int32_t B, net_h, net_w, H, W, mode;   /* mode: UDB_V2OLD_BILINEAR or UDB_V2OLD_NEAREST_EXACT */
+  float* out_depth;        /* [B,1,H,W] */
+  float* out_confidence;   /* [B,1,H,W] antialiased bilinear */
+  float* out_points;       /* [B,3,H,W] */
+} udb_v2old_postprocess_t;
+int udb_v2old_postprocess(const udb_v2old_postprocess_t* p, void* stream);
+/* x4 [B,4] camera-head output -> intr4_rays [B,4] (gt_k * ratio, else the prediction at the network shape), k_out [B,3,3]
+ * (the prediction at the input size), k4_points [B,4] (gt_k, else the prediction at the input size) */
+int udb_v2old_camera(const float* x4, const float* gt_k, int32_t B, int32_t net_h, int32_t net_w, float ratio, float* intr4_rays,
+                     float* k_out, float* k4_points, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Peer-memory plumbing of the multi-GPU output gather (one process per GPU on one node; SURVEY.md section 8e).

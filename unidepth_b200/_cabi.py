@@ -177,6 +177,33 @@ class InferV1Args(C.Structure):
     ]
 
 
+class V2oldConfig(C.Structure):
+    _fields_ = [("embed_dim", i32), ("enc_depth", i32), ("enc_heads", i32), ("output_idx", i32 * 4), ("hidden", i32),
+                ("heads", i32), ("expansion", i32), ("nystrom_depth", i32), ("net_h", i32), ("net_w", i32)]
+
+
+class V2oldGeometry(C.Structure):
+    _fields_ = [("pixels", i32), ("net_h", i32), ("net_w", i32), ("ratio", C.c_double)]
+
+
+class InferV2oldArgs(C.Structure):
+    _fields_ = [
+        ("rgb", vp), ("rgb_is_u8", i32), ("scale255", i32), ("normalize", i32), ("B", i32), ("H", i32), ("W", i32),
+        ("intrinsics", vp), ("interpolation", i32), ("workspace", vp), ("workspace_bytes", C.c_size_t),
+        ("out_intrinsics", vp), ("out_points", vp), ("out_depth", vp), ("out_confidence", vp),
+    ]
+
+
+class V2oldHeads(C.Structure):
+    _fields_ = [("levels", vp * 3), ("w", vp), ("bias_depth", f32), ("bias_conf", f32), ("B", i32), ("gh", i32), ("gw", i32),
+                ("net_h", i32), ("net_w", i32), ("logdepth", vp), ("confidence", vp)]
+
+
+class V2oldPostprocess(C.Structure):
+    _fields_ = [("depth", vp), ("confidence", vp), ("k4", vp), ("B", i32), ("net_h", i32), ("net_w", i32), ("H", i32), ("W", i32),
+                ("mode", i32), ("out_depth", vp), ("out_confidence", vp), ("out_points", vp)]
+
+
 class NearestNeighbor(C.Structure):
     _fields_ = [
         ("x", vp), ("y", vp), ("lengths1", vp), ("lengths2", vp), ("N", i32), ("P1", i32), ("P2", i32), ("pad0", i32),
@@ -237,6 +264,7 @@ EXPORTS = {
     "udb_camera_attn4_f32": (i32, [vp, vp, vp, vp, i32, i32, i32, vp]),
     "udb_camera_intrinsics": (i32, [vp, i32, i32, i32, f32, i32, i32, vp, vp, vp, vp]),
     "udb_ray_embed": (i32, [C.POINTER(RayEmbed), vp]),
+    "udb_ray_embed_cat_orig": (i32, [C.POINTER(RayEmbed), i32, vp]),
     "udb_upsample2x_nhwc_f16": (i32, [vp, vp, i32, i32, i32, i32, vp]),
     "udb_resize_ac_pad_nhwc_f16": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, i32, vp]),
     "udb_reflect_pad1_nhwc_f16": (i32, [vp, vp, i32, i32, i32, i32, vp]),
@@ -286,6 +314,19 @@ EXPORTS = {
     "udb_v1_geometry": (i32, [i32, i32, i32, i32, C.POINTER(V1Geometry)]),
     "udb_v1_workspace_bytes": (C.c_size_t, [vp, i32, i32, i32]),
     "udb_infer_v1": (i32, [vp, C.POINTER(InferV1Args), vp]),
+    "udb_v2old_create": (i32, [C.POINTER(V2oldConfig), C.POINTER(vp)]),
+    "udb_v2old_destroy": (None, [vp]),
+    "udb_v2old_set_weight": (i32, [vp, C.c_char_p, vp, C.POINTER(i64), i32, i32]),
+    "udb_v2old_set_scalar": (i32, [vp, C.c_char_p, C.c_double]),
+    "udb_v2old_geometry": (i32, [i32, i32, i32, i32, i32, C.POINTER(V2oldGeometry)]),
+    "udb_v2old_schedule_bytes": (C.c_size_t, [vp, i32, i32, i32]),
+    "udb_v2old_workspace_bytes": (C.c_size_t, [vp, i32, i32, i32]),
+    "udb_infer_v2old": (i32, [vp, C.POINTER(InferV2oldArgs), vp]),
+    "udb_pshuffle_dw7_relu": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]),
+    "udb_v2old_heads": (i32, [C.POINTER(V2oldHeads), vp]),
+    "udb_v2old_depth_tail": (i32, [vp, vp, i32, i64, vp]),
+    "udb_v2old_postprocess": (i32, [C.POINTER(V2oldPostprocess), vp]),
+    "udb_v2old_camera": (i32, [vp, vp, i32, i32, i32, f32, vp, vp, vp, vp]),
     # evaluation metrics
     "udb_nearest_neighbor": (i32, [C.POINTER(NearestNeighbor), vp]),
     "udb_depth_metrics": (i32, [C.POINTER(DepthMetrics), vp]),

@@ -430,7 +430,9 @@ __device__ __forceinline__ float aa_w(float scale, int k, float center) {
 }
 
 // one warp per output token
-__global__ void __launch_bounds__(256) ray_embed_kernel(const udb_ray_embed_t p) {
+// ld_cat: 0 for UniDepthV2's angle features, else UniDepthV2old's Fourier features of the ray with the ray appended,
+// rows of ld_cat values
+__global__ void __launch_bounds__(256) ray_embed_kernel(const udb_ray_embed_t p, const int ld_cat) {
   const int tok = blockIdx.x * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   const int n = p.gh * p.gw;
@@ -462,6 +464,20 @@ __global__ void __launch_bounds__(256) ray_embed_kernel(const udb_ray_embed_t p)
   ax = warp_sum(ax); ay = warp_sum(ay); az = warp_sum(az);
   const float nrm = fmaxf(sqrtf(ax * ax + ay * ay + az * az), 1e-4f);
   ax /= nrm; ay /= nrm; az /= nrm;
+  if (ld_cat) {
+    // UniDepthV2old (decoder_old.py:111-121 / 237-247, positional_embedding.py:218-256 with use_log, cat_orig): sin of each
+    // axis of the unit ray times the `bands` frequencies and pi (axis-major), then the ray itself, zero up to `ld_cat`
+    const float r3[3] = {ax, ay, az};
+    const float pi = 3.14159265358979323846f;
+    for (int f = lane; f < ld_cat; f += 32) {
+      float v = 0.f;
+      if (f < 3 * p.bands) v = sinf(r3[f / p.bands] * __ldg(p.scales + (f % p.bands)) * pi);
+      else if (f < 3 * p.bands + 3) v = r3[f - 3 * p.bands];
+      if (p.out_f32) reinterpret_cast<float*>(p.out)[(long long)tok * ld_cat + f] = v;
+      else reinterpret_cast<__half*>(p.out)[(long long)tok * ld_cat + f] = __float2half_rn(v);
+    }
+    return;
+  }
   const float polar = acosf(az);
   const float xcl = fmaxf(fabsf(ax), 1e-3f) * ((ax >= 0.f) ? 1.f : -1.f);
   const float azim = atan2f(ay, xcl);
@@ -885,8 +901,24 @@ extern "C" int udb_camera_adjust_k(const float* K, int32_t B, float factor, int3
 extern "C" int udb_ray_embed(const udb_ray_embed_t* p, void* stream) {
   const int toks = p->B * p->gh * p->gw;
   note_work(0.0, (double)toks * 2 * p->bands * (p->out_f32 ? 4 : 2));
-  ray_embed_kernel<<<(toks + 7) / 8, 256, 0, ST(stream)>>>(*p);
+  ray_embed_kernel<<<(toks + 7) / 8, 256, 0, ST(stream)>>>(*p, 0);
   return check_launch("ray_embed_kernel");
+}
+
+extern "C" int udb_ray_embed_cat_orig(const udb_ray_embed_t* p, int32_t ld_out, void* stream) {
+  if (!p || !p->intr4 || !p->scales || !p->out) { set_error("udb_ray_embed_cat_orig: null argument (intr4, scales and out are required)"); return 1; }
+  if (p->bands < 1 || ld_out < 3 * p->bands + 3) {
+    set_error("udb_ray_embed_cat_orig: needs bands >= 1 and ld_out >= 3*bands + 3 (bands=%d ld_out=%d)", p->bands, ld_out);
+    return 1;
+  }
+  if (p->B < 1 || p->gh < 1 || p->gw < 1 || p->net_h < 1 || p->net_w < 1) {
+    set_error("udb_ray_embed_cat_orig: B=%d gh=%d gw=%d net_h=%d net_w=%d must all be >= 1", p->B, p->gh, p->gw, p->net_h, p->net_w);
+    return 1;
+  }
+  const int toks = p->B * p->gh * p->gw;
+  note_work(0.0, (double)toks * ld_out * (p->out_f32 ? 4 : 2));
+  ray_embed_kernel<<<(toks + 7) / 8, 256, 0, ST(stream)>>>(*p, ld_out);
+  return check_launch("ray_embed_cat_orig_kernel");
 }
 
 extern "C" int udb_upsample2x_nhwc_f16(const void* in, void* out, int32_t B, int32_t H, int32_t W, int32_t C, void* stream) {

@@ -311,6 +311,134 @@ static inline std::string shape_name(int B, int H, int W) {
   return b;
 }
 
+// ------------------------------------------------------------------------------------------ decoder blocks
+// Shared by the UniDepthV1 and UniDepthV2old decoders (layers/{attention,nystrom_attention,mlp,convnext}.py).
+// LayerNorm to f16 for any decoder / encoder width: the V2 kernels where they apply (128-multiples up to 1024 from f32,
+// 64/128/256 from f16), the generic one otherwise
+static inline void ln16(Ctx& c, const void* in, int in_f32, void* out, const std::string& wn, const std::string& bn, long long rows,
+                 int dim, float eps) {
+  const bool v2_ok = in_f32 ? (dim % 128 == 0 && dim <= 1024) : (dim == 64 || dim == 128 || dim == 256 || (dim % 128 == 0 && dim <= 1024));
+  if (v2_ok) c.layernorm(in, in_f32, out, 0, c.F(wn), c.F(bn), static_cast<int>(rows), dim, eps);
+  else c.ln_any(in, in_f32, out, 0, c.F(wn), c.F(bn), rows, dim, eps);
+}
+
+// MLP tail on the f32 residual stream x [rows, C]:  x += gamma * (W2 gelu(W1 LN(x) + b1) + b2)        (layers/mlp.py:9-35)
+static inline void mlp_resid(Ctx& c, const std::string& p, float* x, long long rows, int C, int mid, const float* gamma,
+                      __half* x16 = nullptr) {
+  Arena& ar = *c.ar;
+  const size_t m = ar.mark();
+  __half* hN = ar.h(rows * C);
+  __half* md = ar.h(rows * mid);
+  ln16(c, x, 1, hN, p + "nw", p + "nb", rows, C, 1e-5f);
+  { Ctx::G q{hN, c.H(p + "w1"), static_cast<int>(rows), mid, C}; q.bias = c.F(p + "b1"); q.act = UDB_ACT_GELU; q.out = md; c.gemm(q); }
+  { Ctx::G q{md, c.H(p + "w2"), static_cast<int>(rows), C, mid}; q.bias = c.F(p + "b2"); q.gamma = gamma; q.resid = x; q.resid_f32 = 1;
+    q.out = x; q.out_f32 = 1; q.out2 = x16; q.out2_leaky = 0; c.gemm(q); }
+  ar.release(m);
+}
+
+// ConvNeXt-style block on an NHWC map: x f32 (+ its f16 copy x16) [B,H,W,C] updated in place
+// (convnext.py:208-223 with eps 1e-6; layers/convnext.py:34-44 with eps 1e-5)
+static inline void cvnxt_block(Ctx& c, const std::string& p, float* x, __half* x16, int B, int Hh, int Ww, int C, float eps) {
+  Arena& ar = *c.ar;
+  const size_t m = ar.mark();
+  const long long rows = static_cast<long long>(B) * Hh * Ww;
+  __half* y = ar.h(rows * C);
+  __half* hN = ar.h(rows * C);
+  __half* md = ar.h(rows * 4 * C);
+  const float* dw_w = c.F(p + "dw_w");
+  const float* dw_b = c.F(p + "dw_b");
+  c.launch([&] { return udb_dwconv7_nhwc_f16(x16, dw_w, dw_b, y, B, Hh, Ww, C, c.st); });
+  ln16(c, y, 0, hN, p + "ln_w", p + "ln_b", rows, C, eps);
+  { Ctx::G q{hN, c.H(p + "w1"), static_cast<int>(rows), 4 * C, C}; q.bias = c.F(p + "b1"); q.act = UDB_ACT_GELU; q.out = md; c.gemm(q); }
+  { Ctx::G q{md, c.H(p + "w2"), static_cast<int>(rows), C, 4 * C}; q.bias = c.F(p + "b2"); q.gamma = c.F(p + "gamma"); q.resid = x;
+    q.resid_f32 = 1; q.out = x; q.out_f32 = 1; q.out2 = x16; q.out2_leaky = 0; c.gemm(q); }
+  ar.release(m);
+}
+
+static inline long long rup(long long v, long long m) { return (v + m - 1) / m * m; }
+
+// Single-head (head dim = D) attention block with a separate context (decoder.py:225-236 aggregate_16 / prompt_camera),
+// computed densely: S = q k^T (GEMM) -> row softmax -> P v (GEMM with v^T as the K-major operand).
+static inline void dense_attn_block(Ctx& c, const std::string& p, float* x, int B, int nq, int D, const void* ctx, int ctx_f32, int nk,
+                             const float* pos_ctx) {
+  Arena& ar = *c.ar;
+  const size_t m = ar.mark();
+  const long long Rq = static_cast<long long>(B) * nq, Rk = static_cast<long long>(B) * nk;
+  const int kp = static_cast<int>(rup(nk, 64));
+  __half* xn = ar.h(Rq * D);
+  __half* cn = ar.h((Rk + 64) * D);
+  ln16(c, x, 1, xn, p + "nxw", p + "nxb", Rq, D, 1e-5f);
+  ln16(c, ctx, ctx_f32, cn, p + "ncw", p + "ncb", Rk, D, 1e-5f);
+  c.launch([&] {
+    return cuda_rc(cudaMemsetAsync(cn + Rk * D, 0, sizeof(__half) * 64 * D, static_cast<cudaStream_t>(c.st)),
+                   "engine: zeroing the padding rows of the normalised context of ", p);
+  });
+  __half* q = ar.h(Rq * D);
+  { Ctx::G g{xn, c.H(p + "q_w"), static_cast<int>(Rq), D, D}; g.bias = c.F(p + "q_b"); g.out = q; c.gemm(g); }
+  __half* k = ar.h(static_cast<long long>(B) * kp * D);
+  c.launch([&] {
+    return cuda_rc(cudaMemsetAsync(k, 0, sizeof(__half) * B * kp * D, static_cast<cudaStream_t>(c.st)),
+                   "engine: zeroing the padded keys of ", p);
+  });
+  { Ctx::G g{cn, c.H(p + "k_w"), static_cast<int>(Rk), D, D}; g.bias = c.F(p + "k_b"); g.out = k;
+    g.rows_per_group = nk; g.group_stride = kp; g.row_offset = 0;
+    if (pos_ctx) { g.resid = pos_ctx; g.resid_f32 = 1; g.ldr = D; g.resid_mod = nk; g.resid_row_offset = 0; }
+    c.gemm(g); }
+  __half* vt = ar.h(static_cast<long long>(B) * D * kp);
+  float* S = ar.f(static_cast<long long>(nq) * kp);
+  __half* P = ar.h(static_cast<long long>(nq) * kp);
+  __half* o = ar.h(Rq * D);
+  const float scale = 1.0f / sqrtf(static_cast<float>(D));
+  for (int b = 0; b < B; ++b) {
+    // v^T [D, kp] = W_v . ctx_b^T  (the value bias is added after P v: softmax rows sum to 1)
+    { Ctx::G g{c.H(p + "v_w"), cn + static_cast<long long>(b) * nk * D, D, kp, D}; g.out = vt + static_cast<long long>(b) * D * kp; c.gemm(g); }
+    { Ctx::G g{q + static_cast<long long>(b) * nq * D, k + static_cast<long long>(b) * kp * D, nq, kp, D}; g.out = S; g.out_f32 = 1; c.gemm(g); }
+    c.launch([&] { return udb_softmax_rows(S, P, nq, nk, kp, kp, scale, c.st); });
+    { Ctx::G g{P, vt + static_cast<long long>(b) * D * kp, nq, D, kp}; g.bias = c.F(p + "v_b"); g.out = o + static_cast<long long>(b) * nq * D; c.gemm(g); }
+  }
+  { Ctx::G g{o, c.H(p + "out_w"), static_cast<int>(Rq), D, D}; g.bias = c.F(p + "out_b"); g.gamma = c.F(p + "ls1"); g.resid = x; g.resid_f32 = 1;
+    g.out = x; g.out_f32 = 1; c.gemm(g); }
+  ar.release(m);
+  mlp_resid(c, p + "m", x, Rq, D, 4 * D, c.F(p + "ls2"));
+}
+
+// Multi-head self-attention block with 64-wide heads and a positional term added to q (decoder.py:239-241,256-258,271-273):
+// exact attention (AttentionBlock) or the Nystrom approximation with 128 landmarks (NystromBlock).
+static inline void mh_attn_block(Ctx& c, const std::string& p, float* x, int B, int n, int C, int heads, const float* pos, bool nystrom) {
+  Arena& ar = *c.ar;
+  const size_t m = ar.mark();
+  const long long R = static_cast<long long>(B) * n;
+  __half* xn = ar.h(R * C);
+  __half* cn = ar.h(R * C);
+  ln16(c, x, 1, xn, p + "nxw", p + "nxb", R, C, 1e-5f);
+  ln16(c, x, 1, cn, p + "ncw", p + "ncb", R, C, 1e-5f);
+  __half* q = ar.h(R * C);
+  { Ctx::G g{xn, c.H(p + "q_w"), static_cast<int>(R), C, C}; g.bias = c.F(p + "q_b"); g.resid = pos; g.resid_f32 = 1; g.out = q; c.gemm(g); }
+  __half* kv = ar.h(R * 2 * C);
+  { Ctx::G g{cn, c.H(p + "kv_w"), static_cast<int>(R), 2 * C, C}; g.bias = c.F(p + "kv_b"); g.out = kv; c.gemm(g); }
+  __half* o = ar.h(R * C);
+  if (!nystrom) {
+    c.attention(q, kv, kv, o, B, heads, n, n, C, 2 * C, 2 * C, C, 0, 0, C, 0.125f);
+  } else {
+    const long long L = static_cast<long long>(B) * 128, mm = static_cast<long long>(B) * heads * 128 * 128;
+    __half* lm = ar.h(L * 2 * C);          // (q landmarks | k landmarks)
+    float* k2 = ar.f(mm);
+    float* z = ar.f(mm);
+    float* tmp = ar.f(3 * mm);
+    __half* k3 = ar.h(L * C);
+    __half* w2 = ar.h(L * C);
+    c.launch([&] { return udb_nystrom_landmarks(q, C, kv, 2 * C, lm, B, n, heads, c.st); });
+    c.launch([&] { return udb_nystrom_k2_pinv(lm, k2, z, tmp, B, heads, 6, c.st); });
+    c.attention(lm, kv, kv, k3, B, heads, 128, n, 2 * C, 2 * C, 2 * C, C, 0, 0, C, 0.125f);        // softmax(ql k^T) v
+    c.launch([&] { return udb_nystrom_zk3(z, k3, C, w2, C, B, heads, c.st); });           // pinv . kernel_3
+    c.attention(q, lm, w2, o, B, heads, n, 128, C, 2 * C, C, C, 0, C, 0, 0.125f);                  // softmax(q kl^T) (pinv kernel_3)
+  }
+  { Ctx::G g{o, c.H(p + "out_w"), static_cast<int>(R), C, C}; g.bias = c.F(p + "out_b"); g.gamma = c.F(p + "ls1"); g.resid = x; g.resid_f32 = 1;
+    g.out = x; g.out_f32 = 1; c.gemm(g); }
+  ar.release(m);
+  mlp_resid(c, p + "m", x, R, C, 4 * C, c.F(p + "ls2"));
+}
+
 // ------------------------------------------------------------------------------------------ DINOv2 blocks
 // Shape and packing mode of the DINOv2 block loop (UniDepthV2 uses every mode; UniDepthV1 ViT-L the f16 and e4m3 ones).
 struct VitBlocks {

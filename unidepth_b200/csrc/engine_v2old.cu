@@ -1,0 +1,407 @@
+// Whole-path engine for UniDepthV2old.infer (DINOv2 ViT-L/14 or ViT-S/14) behind udb_v2old_create / udb_v2old_set_weight /
+// udb_v2old_workspace_bytes / udb_infer_v2old (include/udb.h).  Host-side schedule only, on the skeleton of the other two
+// engines (engine_common.h): the shared DINOv2 block loop, V1's decoder blocks (adapters, dense and Nystrom attention,
+// ConvNeXt blocks, the camera head's cross attention) and the V2old kernels of v1_kernels.cu.  Reference call stack:
+//   UniDepthV2old.infer              unidepth/models/unidepthv2/unidepthv2_old.py:198-282 (_shapes/_preprocess/_postprocess :33-116)
+//     pixel_encoder = DINOv2         backbones/dinov2.py:324-347 (use_norm: every block output through the final norm)
+//     pixel_decoder = Decoder        unidepthv2/decoder_old.py:428-522 (CameraHead :32-86, GlobalHead :89-146,
+//                                    DepthHead :149-343), layers/{attention,nystrom_attention,mlp,upsample,convnext}.py
+#include "engine_common.h"
+
+struct udb_engine_v2old : udb::EngineBase {
+  udb_v2old_config_t cfg;
+};
+
+namespace udb {
+
+constexpr int RAY_K = 128;          // 99 ray features (96 Fourier + the ray) zero-extended to the GEMM's K step
+constexpr int RAY_BANDS = 32;       // camera_dim 96 / 3 axes
+
+// unidepthv2_old.py:45-92 (Python float == C double; ceil(x - 0.5))
+static udb_v2old_geometry_t v2old_geometry(int H, int W, int level, int lo, int hi) {
+  udb_v2old_geometry_t g;
+  const int lv = level < 0 ? 0 : (level > 10 ? 10 : level);
+  g.pixels = lo + static_cast<int>(ceil(static_cast<double>(hi - lo) * lv / 10));
+  const double ratio = static_cast<double>(W) / H;
+  const double n = fmax(fmin((static_cast<double>(H) / 14) * (static_cast<double>(W) / 14), g.pixels), g.pixels);
+  const int gh = static_cast<int>(ceil(sqrt(n / ratio) - 0.5));
+  const int gw = static_cast<int>(ceil(gh * ratio - 0.5));
+  g.net_h = gh * 14;
+  g.net_w = gw * 14;
+  g.ratio = static_cast<double>(gh) / H * 14;
+  return g;
+}
+
+// AttentionBlock with one head over a long f16 context and at most four queries (decoder_old.py:72-77, 142-143): the camera
+// head's and the global head's aggregate blocks, on V1's split-key cross attention.  x f32 [B*nq, hid] -> new f32 rows.
+static float* small_cross_block(Ctx& c, const std::string& p, const float* x, int B, int nq, const void* ctx, long long nk,
+                                const float* q_pos, int hid, int expansion) {
+  Arena& ar = *c.ar;
+  const int R = B * nq;
+  const long long Rc = static_cast<long long>(B) * nk;
+  float* xn = ar.f(static_cast<size_t>(R) * hid);
+  float* q = ar.f(static_cast<size_t>(R) * hid);
+  float* at = ar.f(static_cast<size_t>(R) * hid);
+  float* scratch = ar.f(static_cast<size_t>(B) * 16 * 4 * (hid + 2));
+  c.layernorm(x, 1, xn, 1, c.F(p + "nxw"), c.F(p + "nxb"), R, hid, 1e-5f);
+  c.small_linear(xn, R, hid, c.F(p + "q_w"), hid, c.F(p + "q_b"), UDB_ACT_NONE, nullptr, nullptr, q);
+  const size_t m = ar.mark();          // the normalised context and its (k | v) rows: dead once the attention has run
+  __half* cn = ar.h(Rc * hid);
+  ln16(c, ctx, 0, cn, p + "ncw", p + "ncb", Rc, hid, 1e-5f);
+  __half* kv = ar.h(Rc * 2 * hid);
+  { Ctx::G g{cn, c.H(p + "kv_w"), static_cast<int>(Rc), 2 * hid, hid}; g.bias = c.F(p + "kv_b"); g.out = kv; c.gemm(g); }
+  c.launch([&] {
+    return udb_cross_attn_small(q, q_pos, kv, at, scratch, B, nq, static_cast<int>(nk), hid, 1.0f / sqrtf(static_cast<float>(hid)), c.st);
+  });
+  ar.release(m);
+  float* t2 = xn;
+  c.small_linear(at, R, hid, c.F(p + "out_w"), hid, c.F(p + "out_b"), UDB_ACT_NONE, c.F(p + "ls1"), x, t2);
+  return cam_mlp(c, p + "mlp", t2, R, hid, expansion * hid, hid, t2, c.F(p + "ls2"));
+}
+
+// f32 [R, D] rows of `n` cls tokens -> LN + Linear + GELU per token (ListAdapter, decoder_old.py:13-29) -> f32 [B, n, hid]
+static float* token_adapter(Ctx& c, const std::string& p, float* const* cls, int n, int B, int D, int hid) {
+  float* toks = c.ar->f(static_cast<size_t>(B) * n * hid);
+  for (int i = 0; i < n; ++i) {
+    const std::string tk = p + idx("%d.", i);
+    float* t = c.ar->f(static_cast<size_t>(B) * D);
+    c.ln_any(cls[i], 1, t, 1, c.F(tk + "ln_w"), c.F(tk + "ln_b"), B, D, 1e-5f);
+    c.small_linear(t, B, D, c.F(tk + "w"), hid, c.F(tk + "b"), UDB_ACT_GELU, nullptr, nullptr, toks + i * hid, D, n * hid, 0);
+  }
+  return toks;
+}
+
+static int run_v2old(udb_engine_v2old* e, const udb_infer_v2old_args_t& a, Arena& ar, void* st) {
+  const udb_v2old_config_t& cf = e->cfg;
+  Ctx c{e, &ar, st, ar.dry};
+  const int B = a.B, net_h = cf.net_h, net_w = cf.net_w, hid = cf.hidden, D = cf.embed_dim;
+  const int gh = net_h / 14, gw = net_w / 14, N = gh * gw, T = N + 1, nq = N;
+  const size_t BN = static_cast<size_t>(B) * N, BT = static_cast<size_t>(B) * T;
+  const long long Rq = static_cast<long long>(B) * nq;
+  const double ratio = static_cast<double>(gh) / a.H * 14;     // unidepthv2_old.py:88
+  // Nystrom attention with 128 landmarks at the first decoder level needs more tokens than landmarks, and the heads'
+  // cross attention has a shared-memory bound: both named by the dry run before anything is launched
+  if (nq <= 128) {
+    set_error("udb_v2old: network shape %dx%d gives %d tokens; Nystrom attention needs more than its 128 landmarks", net_h, net_w, nq);
+    return 1;
+  }
+  if (cross_attn_small_check("udb_v2old: camera head cross attention", 4, 4 * nq + 4, hid)) return 1;
+  Stage stage;
+
+  // ---- pre-processing + patch embedding (unidepthv2_old.py:211-230: /255, ImageNet normalisation, antialiased resize)
+  stage.next("udb_v2old:encoder");
+  __half* feats[4];
+  for (int l = 0; l < 4; ++l) feats[l] = ar.h(BN * D);
+  // normed cls rows of the last three blocks (cls[-3..-1]) and of the third output block (the stacked tokens[-2])
+  float* cls[4];
+  for (int k = 0; k < 4; ++k) cls[k] = ar.f(static_cast<size_t>(B) * D);
+  {
+    const size_t m = ar.mark();
+    __half* patches = ar.h(BN * 640);
+    {
+      udb_v1_preprocess_t p;
+      memset(&p, 0, sizeof(p));
+      p.rgb = a.rgb; p.rgb_is_u8 = a.rgb_is_u8; p.scale255 = a.scale255; p.normalize = a.normalize; p.B = B; p.H = a.H; p.W = a.W;
+      p.rh = net_h; p.rw = net_w; p.net_h = net_h; p.net_w = net_w; p.patches = patches; p.patch = 14;
+      c.launch([&] { return udb_v1_preprocess(&p, st); });
+    }
+    float* x = ar.f(BT * D);
+    c.expect2("patch_w", D, 640);
+    c.expect2("pos", T, D);
+    {
+      const float* pos = c.F("pos");
+      const float* clsw = c.F("cls");
+      Ctx::G q{patches, c.H("patch_w"), static_cast<int>(BN), D, 640};
+      q.bias = c.F("patch_b"); q.resid = pos; q.resid_f32 = 1; q.ldr = D; q.out = x; q.out_f32 = 1;
+      q.rows_per_group = N; q.group_stride = T; q.row_offset = 1; q.resid_mod = N; q.resid_row_offset = 1;
+      c.gemm(q);
+      c.launch([&] { return udb_set_cls_rows(x, clsw, pos, B, T, D, st); });
+    }
+    VitBlocks v{B, T, D, cf.enc_heads, cf.enc_depth};
+    int tap = 0;
+    vit_blocks(c, "blocks.", x, v, [&](int i) {
+      if (tap < 4 && i + 1 == cf.output_idx[tap]) {
+        c.layernorm(x, 1, feats[tap], 0, c.F("norm_w"), c.F("norm_b"), static_cast<int>(BN), D, 1e-5f, N, T, 1);
+        ++tap;
+      }
+      const int from_end = cf.enc_depth - 1 - i;
+      if (from_end < 3) c.layernorm(x, 1, cls[2 - from_end], 1, c.F("norm_w"), c.F("norm_b"), B, D, 1e-5f, 1, T, 0);
+      if (i + 1 == cf.output_idx[2]) c.layernorm(x, 1, cls[3], 1, c.F("norm_w"), c.F("norm_b"), B, D, 1e-5f, 1, T, 0);
+    });
+    ar.release(m);
+  }
+
+  // ---- adapters (decoder_old.py:448-461): tokens [B, 4*nq, hid] for the context and featcat [B*nq, 4*hid] for the latents
+  stage.next("udb_v2old:adapters");
+  __half* featcat = ar.h(Rq * 4 * hid);
+  __half* tokens = ar.h((Rq * 4 + 64) * hid);
+  for (int l = 0; l < 4; ++l) {
+    const size_t m = ar.mark();
+    const std::string ad = idx("adapt.%d.", l);
+    __half* an = ar.h(Rq * D);
+    ln16(c, feats[l], 0, an, ad + "ln_w", ad + "ln_b", Rq, D, 1e-5f);
+    { Ctx::G q{an, c.H(ad + "w"), static_cast<int>(Rq), hid, D}; q.bias = c.F(ad + "b"); q.act = UDB_ACT_GELU; q.out = tokens;
+      q.rows_per_group = nq; q.group_stride = 4 * nq; q.row_offset = l * nq; c.gemm(q); }
+    { Ctx::G q{an, c.H(ad + "w"), static_cast<int>(Rq), hid, D}; q.bias = c.F(ad + "b"); q.act = UDB_ACT_GELU;
+      q.out = featcat + l * hid; q.ldc = 4 * hid; c.gemm(q); }
+    ar.release(m);
+  }
+  const float* tokens_pos = c.F("tokens_pos");         // [4*nq, hid]: sine position + level embedding (decoder_old.py:463-479)
+  c.expect2("tokens_pos", 4LL * nq, hid);
+
+  // ---- camera head (decoder_old.py:378-406, 66-83)
+  stage.next("udb_v2old:camera_head");
+  float* intr4 = ar.f(static_cast<size_t>(B) * 4);
+  float* k4_points = ar.f(static_cast<size_t>(B) * 4);
+  {
+    const size_t m = ar.mark();
+    const int R4 = B * 4;
+    float* toks = token_adapter(c, "ctok.", cls, 4, B, D, hid);
+    float* cl = cam_mlp(c, "cam.cls", toks, R4, hid, 4 * hid, hid, nullptr, nullptr);
+    const long long Rc = static_cast<long long>(B) * (4 * nq + 4);
+    __half* ctx = ar.h(Rc * hid);
+    {
+      const size_t m2 = ar.mark();
+      __half* a1 = ar.h(Rq * 4 * hid);
+      __half* m1 = ar.h(Rq * 4 * 2 * hid);
+      c.ln_any(tokens, 0, a1, 0, c.F("cam.inf.nw"), c.F("cam.inf.nb"), Rq * 4, hid, 1e-5f, 0, tokens_pos, 4LL * nq);
+      { Ctx::G q{a1, c.H("cam.inf.w1"), static_cast<int>(Rq * 4), 2 * hid, hid}; q.bias = c.F("cam.inf.b1"); q.act = UDB_ACT_GELU; q.out = m1; c.gemm(q); }
+      { Ctx::G q{m1, c.H("cam.inf.w2"), static_cast<int>(Rq * 4), hid, 2 * hid}; q.bias = c.F("cam.inf.b2"); q.out = ctx;
+        q.rows_per_group = 4 * nq; q.group_stride = 4 * nq + 4; q.row_offset = 0; c.gemm(q); }
+      ar.release(m2);
+    }
+    c.launch([&] { return udb_copy_rows_f32_to_f16(cl, ctx, B, 4, hid, 4LL * nq + 4, 4LL * nq, st); });
+    const float* cam_pos = c.F("cam.pos");
+    float* t = small_cross_block(c, "cam.agg1.", cl, B, 4, ctx, 4LL * nq + 4, cam_pos, hid, cf.expansion);
+    t = small_cross_block(c, "cam.agg2.", t, B, 4, ctx, 4LL * nq + 4, cam_pos, hid, cf.expansion);
+    float* x4 = cam_mlp(c, "cam.out", t, R4, hid, 2 * hid, 1, nullptr, nullptr);     // [B*4, 1] == [B, 4]
+    c.launch([&] {
+      return udb_v2old_camera(x4, a.intrinsics, B, net_h, net_w, static_cast<float>(ratio), intr4, a.out_intrinsics, k4_points, st);
+    });
+    ar.release(m);
+  }
+
+  // ---- ray features at the three decoder grids (GlobalHead / DepthHead.embed_rays, decoder_old.py:111-121,237-255)
+  stage.next("udb_v2old:ray_features");
+  __half* rayf[3];
+  for (int s = 0; s < 3; ++s) {
+    const int lh = gh << s, lw = gw << s;
+    rayf[s] = ar.h(static_cast<size_t>(B) * lh * lw * RAY_K);
+    udb_ray_embed_t p;
+    memset(&p, 0, sizeof(p));
+    p.intr4 = intr4; p.scales = c.F(idx("ray_scales.%d", s)); p.B = B; p.net_h = net_h; p.net_w = net_w; p.gh = lh; p.gw = lw;
+    p.bands = RAY_BANDS; p.out = rayf[s]; p.out_f32 = 0;
+    c.launch([&] { return udb_ray_embed_cat_orig(&p, RAY_K, st); });
+  }
+
+  // ---- global head (decoder_old.py:408-426, 135-146): (scale, shift) of the depth
+  stage.next("udb_v2old:global_head");
+  float* scale_shift = ar.f(static_cast<size_t>(B) * 2);
+  {
+    const size_t m = ar.mark();
+    const int R2 = B * 2;
+    float* gtok[2] = {cls[1], cls[2]};
+    float* toks = token_adapter(c, "gtok.", gtok, 2, B, D, hid);
+    float* gcl = cam_mlp(c, "glob.cls", toks, R2, hid, 4 * hid, hid, nullptr, nullptr);
+    // in_features(features + project_rays(rays)) = W_in features + (W_in project_rays(rays) + b_in), the second term per
+    // token of the grid and shared by the four levels
+    __half* pr = ar.h(Rq * hid);
+    c.expect2("glob.rays_w", hid, RAY_K);
+    { Ctx::G q{rayf[0], c.H("glob.rays_w"), static_cast<int>(Rq), hid, RAY_K}; q.bias = c.F("glob.rays_b"); q.out = pr; c.gemm(q); }
+    float* rr = ar.f(Rq * hid);
+    { Ctx::G q{pr, c.H("glob.in_w"), static_cast<int>(Rq), hid, hid}; q.bias = c.F("glob.in_b"); q.out = rr; q.out_f32 = 1; c.gemm(q); }
+    const long long nk = 4LL * nq + 2;
+    __half* gctx = ar.h(B * nk * hid);
+    for (int b = 0; b < B; ++b) {
+      Ctx::G q{tokens + static_cast<long long>(b) * 4 * nq * hid, c.H("glob.in_w"), 4 * nq, hid, hid};
+      q.resid = rr + static_cast<long long>(b) * nq * hid; q.resid_f32 = 1; q.ldr = hid; q.resid_mod = nq; q.resid_row_offset = 0;
+      q.out = gctx + static_cast<long long>(b) * nk * hid; c.gemm(q);
+    }
+    c.launch([&] { return udb_copy_rows_f32_to_f16(gcl, gctx, B, 2, hid, nk, 4LL * nq, st); });
+    float* t = small_cross_block(c, "glob.agg1.", gcl, B, 2, gctx, nk, nullptr, hid, cf.expansion);
+    t = small_cross_block(c, "glob.agg2.", t, B, 2, gctx, nk, nullptr, hid, cf.expansion);
+    float* x2 = cam_mlp(c, "glob.out", t, R2, hid, 2 * hid, 1, nullptr, nullptr);    // [B*2, 1] == [B, 2]: log scale, shift
+    c.launch([&] {
+      return cuda_rc(cudaMemcpyAsync(scale_shift, x2, sizeof(float) * 2 * B, cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(st)),
+                     "engine_v2old: copying the global head's scale and shift");
+    });
+    ar.release(m);
+  }
+
+  // ---- depth head (decoder_old.py:317-343)
+  stage.next("udb_v2old:depth_head");
+  float* emb[3];
+  for (int s = 0; s < 3; ++s) {
+    const long long R = static_cast<long long>(B) * (gh << s) * (gw << s);
+    const std::string n = idx("rays.%d.", s);
+    emb[s] = ar.f(R * (hid >> s));
+    c.expect2(n + "w", hid >> s, RAY_K);
+    Ctx::G q{rayf[s], c.H(n + "w"), static_cast<int>(R), hid >> s, RAY_K}; q.bias = c.F(n + "b"); q.out = emb[s]; q.out_f32 = 1; c.gemm(q);
+  }
+  float* lat = ar.f(Rq * hid);
+  {
+    const size_t m = ar.mark();
+    __half* f16l = ar.h(Rq * hid);
+    { Ctx::G q{featcat, c.H("fcc_w"), static_cast<int>(Rq), hid, 4 * hid}; q.bias = c.F("fcc_b"); q.out = f16l; c.gemm(q); }
+    __half* hN = ar.h(Rq * hid);
+    __half* md = ar.h(Rq * 2 * hid);
+    ln16(c, f16l, 0, hN, "lat.nw", "lat.nb", Rq, hid, 1e-5f);
+    { Ctx::G q{hN, c.H("lat.w1"), static_cast<int>(Rq), 2 * hid, hid}; q.bias = c.F("lat.b1"); q.act = UDB_ACT_GELU; q.out = md; c.gemm(q); }
+    { Ctx::G q{md, c.H("lat.w2"), static_cast<int>(Rq), hid, 2 * hid}; q.bias = c.F("lat.b2"); q.resid = f16l; q.resid_f32 = 0;
+      q.out = lat; q.out_f32 = 1; c.gemm(q); }
+    ar.release(m);
+  }
+  dense_attn_block(c, "agg16.", lat, B, nq, hid, tokens, 0, 4 * nq, tokens_pos);
+  dense_attn_block(c, "prompt.", lat, B, nq, hid, emb[0], 1, nq, nullptr);
+  for (int i = 0; i < cf.nystrom_depth; ++i) mh_attn_block(c, idx("nys.%d.", i), lat, B, nq, hid, cf.heads, emb[0], true);
+
+  // ConvUpsampleShuffleResidual per level (layers/upsample.py:82-130), then the level's [depth | confidence] MLPs
+  float* heads_in[3];
+  int ch = gh, cw = gw, C = hid;
+  for (int s = 0; s < 3; ++s) {
+    const std::string u = idx("up.%d.", s);
+    const long long R = static_cast<long long>(B) * ch * cw, Rn = 4 * R;
+    const int C2 = C / 2, Cq = C / 4, Cqp = static_cast<int>(rup(Cq, 64));
+    float* nxt = ar.f(Rn * C2);
+    heads_in[s] = ar.f(Rn * 32);
+    const size_t m = ar.mark();
+    float* xs = ar.f(R * C);
+    __half* xs16 = ar.h(R * C);
+    c.launch([&] { return udb_add_f32(lat, emb[s], xs, xs16, R * C, st); });
+    for (int j = 0; j < 2; ++j) cvnxt_block(c, u + (j ? "c1." : "c0."), xs, xs16, B, ch, cw, C, 1e-5f);
+    __half* r1 = ar.h(R * C2);
+    { Ctx::G q{xs16, c.H(u + "res_w"), static_cast<int>(R), C2, C}; q.bias = c.F(u + "res_b"); q.out = r1; c.gemm(q); }
+    __half* res = ar.h(Rn * C2);
+    c.launch([&] { return udb_resize_ac_pad_nhwc_f16(r1, res, B, ch, cw, C2, 2 * ch, 2 * cw, 0, st); });
+    __half* sh = ar.h(Rn * Cqp);
+    const float* dw_w = c.F(u + "dw_w");
+    const float* dw_b = c.F(u + "dw_b");
+    c.launch([&] { return udb_pshuffle_dw7_relu(xs16, dw_w, dw_b, sh, B, ch, cw, C, Cqp, st); });
+    c.expect2(u + "conv_w", C2, 9 * Cqp);
+    __half* nxt16 = ar.h(Rn * C2);
+    c.conv3x3(sh, B, 2 * ch, 2 * cw, Cqp, c.H(u + "conv_w"), C2, c.F(u + "conv_b"), UDB_ACT_NONE, nullptr, res, 0, nxt, 1, nxt16, 0);
+    // depth_mlp / confidence_mlp (LN -> Linear -> GELU -> Linear(-> 16)) side by side: [hd | hc] then one block-diagonal GEMM
+    const std::string hm = idx("hmlp.%d.", s);
+    __half* hn = ar.h(Rn * C2);
+    __half* hm1 = ar.h(Rn * C);
+    for (int k = 0; k < 2; ++k) {
+      const std::string p = hm + (k ? "c." : "d.");
+      ln16(c, nxt, 1, hn, p + "nw", p + "nb", Rn, C2, 1e-5f);
+      Ctx::G q{hn, c.H(p + "w1"), static_cast<int>(Rn), C2, C2}; q.bias = c.F(p + "b1"); q.act = UDB_ACT_GELU; q.out = hm1 + k * C2; q.ldc = C; c.gemm(q);
+    }
+    c.expect2(hm + "w2", 32, C);
+    { Ctx::G q{hm1, c.H(hm + "w2"), static_cast<int>(Rn), 32, C}; q.bias = c.F(hm + "b2"); q.out = heads_in[s]; q.out_f32 = 1; c.gemm(q); }
+    ar.release(m);
+    lat = nxt;
+    ch *= 2; cw *= 2; C = C2;
+  }
+
+  // ---- depth / confidence convolutions at the network shape, the depth tail, output assembly (unidepthv2_old.py:107-116,262-274)
+  stage.next("udb_v2old:heads+postprocess");
+  const long long nhw = static_cast<long long>(net_h) * net_w;
+  float* dmap = ar.f(B * nhw);
+  float* cmap = ar.f(B * nhw);
+  {
+    udb_v2old_heads_t p;
+    memset(&p, 0, sizeof(p));
+    for (int s = 0; s < 3; ++s) p.levels[s] = heads_in[s];
+    p.w = c.F("head_w"); p.bias_depth = static_cast<float>(c.S("head_b_depth")); p.bias_conf = static_cast<float>(c.S("head_b_conf"));
+    p.B = B; p.gh = gh; p.gw = gw; p.net_h = net_h; p.net_w = net_w; p.logdepth = dmap; p.confidence = cmap;
+    c.launch([&] { return udb_v2old_heads(&p, st); });
+  }
+  c.launch([&] { return udb_v2old_depth_tail(dmap, scale_shift, B, nhw, st); });
+  {
+    udb_v2old_postprocess_t p;
+    memset(&p, 0, sizeof(p));
+    p.depth = dmap; p.confidence = cmap; p.k4 = k4_points; p.B = B; p.net_h = net_h; p.net_w = net_w; p.H = a.H; p.W = a.W;
+    p.mode = a.interpolation; p.out_depth = a.out_depth; p.out_confidence = a.out_confidence; p.out_points = a.out_points;
+    c.launch([&] { return udb_v2old_postprocess(&p, st); });
+  }
+  if (!c.rc && ar.overflow) { set_error("engine_v2old: workspace too small (%zu bytes needed)", ar.peak); return 1; }
+  return c.rc;
+}
+
+static size_t dry_run(udb_engine_v2old* e, int B, int H, int W) {
+  if (!e || B <= 0 || H <= 0 || W <= 0) { set_error("udb_v2old_workspace_bytes: bad argument"); return 0; }
+  udb_infer_v2old_args_t a;
+  memset(&a, 0, sizeof(a));
+  a.B = B; a.H = H; a.W = W;
+  Arena ar(nullptr, 0);
+  if (run_v2old(e, a, ar, nullptr)) return 0;
+  return ar.peak + 256;
+}
+
+}  // namespace udb
+
+using namespace udb;
+
+extern "C" {
+
+int udb_v2old_create(const udb_v2old_config_t* cfg, udb_engine_v2old** out) {
+  if (!cfg || !out) { set_error("udb_v2old_create: null argument"); return 1; }
+  if (cfg->embed_dim <= 0 || cfg->embed_dim % 128 || cfg->embed_dim > 1024 || cfg->enc_heads <= 0 || cfg->embed_dim / cfg->enc_heads != 64) {
+    set_error("udb_v2old_create: encoder width %d / heads %d: 64-wide heads and a width that is a multiple of 128 up to 1024",
+              cfg->embed_dim, cfg->enc_heads);
+    return 1;
+  }
+  for (int i = 0; i < 4; ++i)
+    if (cfg->output_idx[i] < 1 || cfg->output_idx[i] > cfg->enc_depth || (i && cfg->output_idx[i] <= cfg->output_idx[i - 1])) {
+      set_error("udb_v2old_create: output_idx must be four increasing block indices in [1, %d]", cfg->enc_depth);
+      return 1;
+    }
+  if (cfg->enc_depth < 3) { set_error("udb_v2old_create: the camera head reads the cls tokens of the last three blocks (depth %d)", cfg->enc_depth); return 1; }
+  if (cfg->hidden != 512 || cfg->heads != 8 || cfg->expansion != 4) {
+    set_error("udb_v2old_create: decoder hidden %d / heads %d / expansion %d not supported (512 / 8 / 4)", cfg->hidden, cfg->heads, cfg->expansion);
+    return 1;
+  }
+  if (cfg->nystrom_depth < 0) { set_error("udb_v2old_create: nystrom_depth %d must be >= 0", cfg->nystrom_depth); return 1; }
+  if (cfg->net_h < 56 || cfg->net_w < 56 || cfg->net_h % 14 || cfg->net_w % 14) {
+    set_error("udb_v2old_create: network shape %dx%d must be multiples of 14, at least 56", cfg->net_h, cfg->net_w);
+    return 1;
+  }
+  udb_engine_v2old* e = new udb_engine_v2old();
+  e->cfg = *cfg;
+  *out = e;
+  return 0;
+}
+
+void udb_v2old_destroy(udb_engine_v2old* e) { delete e; }
+
+int udb_v2old_geometry(int32_t H, int32_t W, int32_t resolution_level, int32_t pixels_lo, int32_t pixels_hi, udb_v2old_geometry_t* out) {
+  if (!out || H <= 0 || W <= 0 || pixels_lo <= 0 || pixels_hi < pixels_lo) { set_error("udb_v2old_geometry: bad argument"); return 1; }
+  *out = v2old_geometry(H, W, resolution_level, pixels_lo, pixels_hi);       // the function the Python boundary keys engines by
+  return 0;
+}
+
+int udb_v2old_set_weight(udb_engine_v2old* e, const char* name, const void* dev_ptr, const int64_t* shape, int32_t ndim, int32_t dtype) {
+  return EngineBase::set_weight(e, "udb_v2old_set_weight", name, dev_ptr, shape, ndim, dtype);
+}
+
+int udb_v2old_set_scalar(udb_engine_v2old* e, const char* name, double value) {
+  return EngineBase::set_scalar(e, "udb_v2old_set_scalar", name, value);
+}
+
+size_t udb_v2old_schedule_bytes(udb_engine_v2old* e, int32_t B, int32_t H, int32_t W) { return dry_run(e, B, H, W); }
+
+size_t udb_v2old_workspace_bytes(udb_engine_v2old* e, int32_t B, int32_t H, int32_t W) {
+  const size_t n = dry_run(e, B, H, W);
+  return n ? e->prepared(shape_name(B, H, W), n) : 0;
+}
+
+int udb_infer_v2old(udb_engine_v2old* e, const udb_infer_v2old_args_t* a, void* stream) {
+  if (!e || !a || !a->rgb || !a->workspace) { set_error("udb_infer_v2old: null argument"); return 1; }
+  if (!a->out_intrinsics || !a->out_points || !a->out_depth || !a->out_confidence) {
+    set_error("udb_infer_v2old: all four output pointers are required");
+    return 1;
+  }
+  if (a->interpolation != UDB_V2OLD_BILINEAR && a->interpolation != UDB_V2OLD_NEAREST_EXACT) {
+    set_error("udb_infer_v2old: `interpolation` %d is neither UDB_V2OLD_BILINEAR (0) nor UDB_V2OLD_NEAREST_EXACT (1)", a->interpolation);
+    return 1;
+  }
+  if (e->check_workspace("udb_infer_v2old", "udb_v2old_workspace_bytes", shape_name(a->B, a->H, a->W), a->workspace, a->workspace_bytes))
+    return 1;
+  Arena ar(a->workspace, a->workspace_bytes);
+  return run_v2old(e, *a, ar, stream);
+}
+
+}  // extern "C"

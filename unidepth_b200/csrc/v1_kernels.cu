@@ -1536,3 +1536,282 @@ int udb_v1_postprocess(const udb_v1_postprocess_t* p, void* stream) {
 }
 
 }  // extern "C"
+
+// ------------------------------------------------------------------------------------------------------------------
+// UniDepthV2old (unidepthv2/decoder_old.py, unidepthv2_old.py).  CUDA-core kernels for the four steps no existing kernel
+// computes; they sit here to share the antialiased weights above (aa_axis) with V1's post-processing.
+// ------------------------------------------------------------------------------------------------------------------
+namespace udb {
+
+// ConvUpsampleShuffleResidual's up branch before its 3x3 conv (layers/upsample.py:110-121): PixelShuffle(2) of the NHWC
+// f16 map [B,h,w,C] (out channel c of pixel (Y, X) is input channel 4c + 2(Y%2) + X%2 of pixel (Y/2, X/2)), then the
+// depthwise 7x7 (zero padding) on the C/4 shuffled channels, then ReLU.  Written to an f16 map [B,2h,2w,ldo] whose channels
+// C/4..ldo-1 are zero, so that the following 3x3 conv runs on the wgmma path, which needs 64-channel multiples.  No
+// existing kernel reads a pixel-shuffled operand: udb_dwconv7_nhwc_f16 needs C % 64 == 0 and a plain NHWC map.
+// One thread per output (pixel, channel); taps tap-major [49, C/4] f32 as the ConvNeXt depthwise weights.
+__global__ void __launch_bounds__(256) pshuffle_dw7_relu_kernel(const __half* __restrict__ x, const float* __restrict__ w,
+                                                                const float* __restrict__ bias, __half* __restrict__ out, int B,
+                                                                int h, int wd, int C, int ldo) {
+  const int Cq = C / 4, H2 = 2 * h, W2 = 2 * wd;
+  const long long total = (long long)B * H2 * W2 * ldo;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % ldo);
+    const long long px = i / ldo;
+    if (c >= Cq) { out[i] = __float2half_rn(0.f); continue; }
+    const int X = (int)(px % W2), Y = (int)((px / W2) % H2), b = (int)(px / ((long long)W2 * H2));
+    float acc = bias[c];
+    for (int dy = 0; dy < 7; ++dy) {
+      const int yy = Y + dy - 3;
+      if (yy < 0 || yy >= H2) continue;
+      for (int dx = 0; dx < 7; ++dx) {
+        const int xx = X + dx - 3;
+        if (xx < 0 || xx >= W2) continue;
+        const int ch = 4 * c + 2 * (yy & 1) + (xx & 1);
+        const float v = __half2float(x[(((long long)b * h + (yy >> 1)) * wd + (xx >> 1)) * C + ch]);
+        acc = fmaf(w[(dy * 7 + dx) * Cq + c], v, acc);
+      }
+    }
+    out[i] = __float2half_rn(fmaxf(acc, 0.f));
+  }
+}
+
+// The depth and confidence convolutions of DepthHead.decode_depth (decoder_old.py:282-304): each level's 32-channel MLP
+// output ([depth 16 | confidence 16], f32 NHWC at (2gh, 2gw) << i) is bilinearly resized (align_corners=False, no
+// antialias) to the network shape and concatenated finest level first (channel block 2 - i), and a 7x7 reflect-padded
+// conv maps the 48 channels to one.  The resized maps are never stored: each of the 49 taps samples the levels where it
+// lands.  Writes the log-depth and the sigmoid of the confidence logit.  One thread per network pixel; weights in shared
+// memory ([2][48][49]: depth then confidence).
+__device__ __forceinline__ int reflect_idx(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i); }
+
+__global__ void __launch_bounds__(256) v2old_heads_kernel(const udb_v2old_heads_t p) {
+  __shared__ float ws[2 * 48 * 49];
+  for (int i = threadIdx.x; i < 2 * 48 * 49; i += blockDim.x) ws[i] = p.w[i];
+  __syncthreads();
+  const long long total = (long long)p.B * p.net_h * p.net_w;
+  for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
+    const int X = (int)(idx % p.net_w), Y = (int)((idx / p.net_w) % p.net_h), b = (int)(idx / ((long long)p.net_w * p.net_h));
+    float ad = p.bias_depth, ac = p.bias_conf;
+    for (int lvl = 0; lvl < 3; ++lvl) {
+      const int lh = (2 * p.gh) << lvl, lw = (2 * p.gw) << lvl;
+      const float sy = (float)lh / (float)p.net_h, sx = (float)lw / (float)p.net_w;
+      const float* src = p.levels[lvl] + (long long)b * lh * lw * 32;
+      const float* wd = ws + (2 - lvl) * 16 * 49;
+      const float* wc = ws + 48 * 49 + (2 - lvl) * 16 * 49;
+      for (int dy = 0; dy < 7; ++dy) {
+        const int yy = reflect_idx(Y + dy - 3, p.net_h);
+        const float fy = fmaxf(sy * ((float)yy + 0.5f) - 0.5f, 0.f);
+        const int y0 = (int)fy, y1 = y0 + (y0 < lh - 1 ? 1 : 0);
+        const float ly = fy - (float)y0;
+        for (int dx = 0; dx < 7; ++dx) {
+          const int xx = reflect_idx(X + dx - 3, p.net_w);
+          const float fx = fmaxf(sx * ((float)xx + 0.5f) - 0.5f, 0.f);
+          const int x0 = (int)fx, x1 = x0 + (x0 < lw - 1 ? 1 : 0);
+          const float lx = fx - (float)x0;
+          const float4* r00 = reinterpret_cast<const float4*>(src + ((long long)y0 * lw + x0) * 32);
+          const float4* r01 = reinterpret_cast<const float4*>(src + ((long long)y0 * lw + x1) * 32);
+          const float4* r10 = reinterpret_cast<const float4*>(src + ((long long)y1 * lw + x0) * 32);
+          const float4* r11 = reinterpret_cast<const float4*>(src + ((long long)y1 * lw + x1) * 32);
+          const float w00 = (1.f - ly) * (1.f - lx), w01 = (1.f - ly) * lx, w10 = ly * (1.f - lx), w11 = ly * lx;
+          const int tap = dy * 7 + dx;
+#pragma unroll
+          for (int q = 0; q < 8; ++q) {
+            const float4 a = __ldg(r00 + q), bb = __ldg(r01 + q), cc = __ldg(r10 + q), d = __ldg(r11 + q);
+            const float v[4] = {w00 * a.x + w01 * bb.x + w10 * cc.x + w11 * d.x, w00 * a.y + w01 * bb.y + w10 * cc.y + w11 * d.y,
+                                w00 * a.z + w01 * bb.z + w10 * cc.z + w11 * d.z, w00 * a.w + w01 * bb.w + w10 * cc.w + w11 * d.w};
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const int ch = q * 4 + e;
+              if (ch < 16) ad = fmaf(wd[ch * 49 + tap], v[e], ad);
+              else ac = fmaf(wc[(ch - 16) * 49 + tap], v[e], ac);
+            }
+          }
+        }
+      }
+    }
+    p.logdepth[idx] = ad;
+    p.confidence[idx] = 1.f / (1.f + expf(-ac));
+  }
+}
+
+// The decoder's tail (decoder_old.py:505-514) in place on the log-depth map of one image per block: LayerNorm over the whole
+// H x W map (no affine, eps 1e-5; mean then variance, two passes, double accumulation), exp, (x + shift) * scale with
+// (log scale, shift) from the global head, softplus with beta 10 (threshold 20, as torch).  A per-map reduction fused
+// with its pointwise tail: no existing LayerNorm kernel normalises over a whole map.
+__global__ void __launch_bounds__(1024) v2old_depth_tail_kernel(float* __restrict__ d, const float* __restrict__ scale_shift, long long hw) {
+  __shared__ double red[32];
+  __shared__ double bc;
+  float* m = d + blockIdx.x * hw;
+  auto block_sum = [&](double v) {
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+      double t = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.0;
+      for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+      if (threadIdx.x == 0) bc = t;
+    }
+    __syncthreads();
+    const double r = bc;
+    __syncthreads();
+    return r;
+  };
+  double s = 0.0;
+  for (long long i = threadIdx.x; i < hw; i += blockDim.x) s += m[i];
+  const float mean = (float)(block_sum(s) / (double)hw);
+  double v = 0.0;
+  for (long long i = threadIdx.x; i < hw; i += blockDim.x) { const double t = (double)m[i] - mean; v += t * t; }
+  const float rstd = rsqrtf((float)(block_sum(v) / (double)hw) + 1e-5f);
+  const float sc = expf(scale_shift[blockIdx.x * 2]), sh = scale_shift[blockIdx.x * 2 + 1];
+  for (long long i = threadIdx.x; i < hw; i += blockDim.x) {
+    const float z = (expf((m[i] - mean) * rstd) + sh) * sc;
+    m[i] = 10.f * z > 20.f ? z : log1pf(expf(10.f * z)) / 10.f;
+  }
+}
+
+// Output assembly at the input size (unidepthv2_old.py:107-116,267-274): depth resized from the network shape with
+// bilinear (align_corners=False, no antialias) or nearest-exact, confidence with antialiased bilinear (aa_axis), and the
+// points z * (tan(theta), 1 / tan(phi) / cos(theta), 1) of the unit ray of each input pixel through k4 (fx, fy, cx, cy).
+// V1's post-processing crops paddings and resizes depth with antialias only; V2's assembles radius-based points from
+// padded maps; neither resizes with these two modes.
+__global__ void __launch_bounds__(256) v2old_postprocess_kernel(const udb_v2old_postprocess_t p) {
+  const long long total = (long long)p.B * p.H * p.W;
+  const float sh = (float)p.net_h / (float)p.H, sw = (float)p.net_w / (float)p.W;
+  for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
+    const int X = (int)(idx % p.W), Y = (int)((idx / p.W) % p.H), b = (int)(idx / ((long long)p.W * p.H));
+    const long long nhw = (long long)p.net_h * p.net_w;
+    const float* dm = p.depth + b * nhw;
+    float z;
+    if (p.mode == UDB_V2OLD_NEAREST_EXACT) {
+      const int yi = min((int)floorf(((float)Y + 0.5f) * sh), p.net_h - 1), xi = min((int)floorf(((float)X + 0.5f) * sw), p.net_w - 1);
+      z = dm[(long long)yi * p.net_w + xi];
+    } else {
+      const float fy = fmaxf(sh * ((float)Y + 0.5f) - 0.5f, 0.f), fx = fmaxf(sw * ((float)X + 0.5f) - 0.5f, 0.f);
+      const int y0 = (int)fy, x0 = (int)fx;
+      const int y1 = y0 + (y0 < p.net_h - 1 ? 1 : 0), x1 = x0 + (x0 < p.net_w - 1 ? 1 : 0);
+      const float ly = fy - (float)y0, lx = fx - (float)x0;
+      z = (1.f - ly) * ((1.f - lx) * dm[(long long)y0 * p.net_w + x0] + lx * dm[(long long)y0 * p.net_w + x1]) +
+          ly * ((1.f - lx) * dm[(long long)y1 * p.net_w + x0] + lx * dm[(long long)y1 * p.net_w + x1]);
+    }
+    const AAxis ay = aa_axis(Y, p.net_h, sh), ax = aa_axis(X, p.net_w, sw);
+    const float* cm = p.confidence + b * nhw;
+    float conf = 0.f;
+    for (int jy = 0; jy < ay.xsize; ++jy) {
+      float r = 0.f;
+      for (int jx = 0; jx < ax.xsize; ++jx) r += ax.w(jx) * cm[(long long)(ay.xmin + jy) * p.net_w + ax.xmin + jx];
+      conf += ay.w(jy) * r;
+    }
+    const float* k = p.k4 + b * 4;
+    const float dx = ((float)X + 0.5f - k[2]) / k[0], dy = ((float)Y + 0.5f - k[3]) / k[1];
+    const float inv = 1.0f / fmaxf(sqrtf(dx * dx + dy * dy + 1.0f), 1e-12f);
+    const float rx = dx * inv, ry = dy * inv, rz = inv;
+    const float theta = atan2f(rx, rz), phi = acosf(ry);
+    const long long hw = (long long)p.H * p.W, pix = (long long)Y * p.W + X;
+    p.out_depth[b * hw + pix] = z;
+    p.out_confidence[b * hw + pix] = conf;
+    p.out_points[(b * 3 + 0) * hw + pix] = z * tanf(theta);
+    p.out_points[(b * 3 + 1) * hw + pix] = z / tanf(phi) / cosf(theta);
+    p.out_points[(b * 3 + 2) * hw + pix] = z;
+  }
+}
+
+// The camera of UniDepthV2old (decoder_old.py:55-64,396-399; unidepthv2_old.py:95-104,112-115,268): the predicted K at the
+// network shape (focal max(h, w)/2 exp(x), principal point sigmoid(x) times the side) and at the input size (divided
+// by `ratio`: out_k, always the prediction), the K of the rays (the caller's K times `ratio`, else the prediction) and
+// the K of the points (the caller's K, else the prediction at the input size).
+__global__ void v2old_camera_kernel(const float* __restrict__ x4, const float* __restrict__ gt_k, int B, int net_h, int net_w,
+                                    float ratio, float* intr4_rays, float* k_out, float* k4_points) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const float half = (float)(net_h > net_w ? net_h : net_w) / 2.f;
+  const float* x = x4 + b * 4;
+  const float fx = half * expf(x[0]), fy = half * expf(x[1]);
+  const float cx = (1.f / (1.f + expf(-x[2]))) * (float)net_w, cy = (1.f / (1.f + expf(-x[3]))) * (float)net_h;
+  const float kf[4] = {fx / ratio, fy / ratio, cx / ratio, cy / ratio};
+  float* o = k_out + b * 9;
+  o[0] = kf[0]; o[1] = 0.f; o[2] = kf[2]; o[3] = 0.f; o[4] = kf[1]; o[5] = kf[3]; o[6] = 0.f; o[7] = 0.f; o[8] = 1.f;
+  if (gt_k) {
+    const float* g = gt_k + b * 9;
+    const float gk[4] = {g[0], g[4], g[2], g[5]};
+    for (int i = 0; i < 4; ++i) { intr4_rays[b * 4 + i] = gk[i] * ratio; k4_points[b * 4 + i] = gk[i]; }
+  } else {
+    const float pk[4] = {fx, fy, cx, cy};
+    for (int i = 0; i < 4; ++i) { intr4_rays[b * 4 + i] = pk[i]; k4_points[b * 4 + i] = kf[i]; }
+  }
+}
+
+}  // namespace udb
+
+extern "C" {
+
+int udb_pshuffle_dw7_relu(const void* x, const float* w, const float* bias, void* out, int32_t B, int32_t h, int32_t wd, int32_t C,
+                          int32_t ldo, void* stream) {
+  const struct { int v; const char* name; } dims[] = {{B, "B"}, {h, "h"}, {wd, "w"}, {C, "C"}};
+  for (const auto& d : dims)
+    if (d.v < 1) { set_error("udb_pshuffle_dw7_relu: %s=%d must be >= 1", d.name, d.v); return 1; }
+  if (C % 4) { set_error("udb_pshuffle_dw7_relu: C=%d must be a multiple of 4 (PixelShuffle(2))", C); return 1; }
+  if (ldo < C / 4) { set_error("udb_pshuffle_dw7_relu: ldo=%d must be >= C/4=%d", ldo, C / 4); return 1; }
+  const struct { const void* p; const char* name; } ptrs[] = {{x, "x"}, {w, "w"}, {bias, "bias"}, {out, "out"}};
+  for (const auto& a : ptrs)
+    if (!a.p) { set_error("udb_pshuffle_dw7_relu: `%s` must be non-null", a.name); return 1; }
+  const long long total = 4LL * B * h * wd * ldo;
+  note_work(2.0 * 49 * 4.0 * B * h * wd * (C / 4), 2.0 * B * h * wd * C + 2.0 * total);
+  pshuffle_dw7_relu_kernel<<<grid_1d(total), 256, 0, ST(stream)>>>(reinterpret_cast<const __half*>(x), w, bias,
+                                                                    reinterpret_cast<__half*>(out), B, h, wd, C, ldo);
+  return check_launch("pshuffle_dw7_relu_kernel");
+}
+
+int udb_v2old_heads(const udb_v2old_heads_t* p, void* stream) {
+  if (!p) { set_error("udb_v2old_heads: null argument"); return 1; }
+  const struct { int v; const char* name; } dims[] = {{p->B, "B"}, {p->gh, "gh"}, {p->gw, "gw"}, {p->net_h, "net_h"}, {p->net_w, "net_w"}};
+  for (const auto& d : dims)
+    if (d.v < 1) { set_error("udb_v2old_heads: %s=%d must be >= 1", d.name, d.v); return 1; }
+  if (p->net_h < 4 || p->net_w < 4) { set_error("udb_v2old_heads: net_h=%d net_w=%d: the 7x7 reflect padding needs >= 4", p->net_h, p->net_w); return 1; }
+  const struct { const void* q; const char* name; } ptrs[] = {{p->levels[0], "levels[0]"}, {p->levels[1], "levels[1]"},
+                                                             {p->levels[2], "levels[2]"}, {p->w, "w"}, {p->logdepth, "logdepth"},
+                                                             {p->confidence, "confidence"}};
+  for (const auto& a : ptrs)
+    if (!a.q || (reinterpret_cast<uintptr_t>(a.q) & 15)) { set_error("udb_v2old_heads: `%s` must be a non-null, 16-byte aligned pointer", a.name); return 1; }
+  const long long px = (long long)p->B * p->net_h * p->net_w;
+  note_work(px * 49.0 * 3 * (8.0 * 32 + 2.0 * 32), px * 8.0);
+  v2old_heads_kernel<<<grid_1d(px), 256, 0, ST(stream)>>>(*p);
+  return check_launch("v2old_heads_kernel");
+}
+
+int udb_v2old_depth_tail(float* depth, const float* scale_shift, int32_t B, int64_t hw, void* stream) {
+  if (B < 1 || hw < 1) { set_error("udb_v2old_depth_tail: B=%d hw=%lld must be >= 1", B, (long long)hw); return 1; }
+  if (!depth || !scale_shift) { set_error("udb_v2old_depth_tail: `%s` must be non-null", depth ? "scale_shift" : "depth"); return 1; }
+  note_work(12.0 * B * hw, 16.0 * B * hw);
+  v2old_depth_tail_kernel<<<B, 1024, 0, ST(stream)>>>(depth, scale_shift, hw);
+  return check_launch("v2old_depth_tail_kernel");
+}
+
+int udb_v2old_postprocess(const udb_v2old_postprocess_t* p, void* stream) {
+  if (!p) { set_error("udb_v2old_postprocess: null argument"); return 1; }
+  const struct { int v; const char* name; } dims[] = {{p->B, "B"}, {p->H, "H"}, {p->W, "W"}, {p->net_h, "net_h"}, {p->net_w, "net_w"}};
+  for (const auto& d : dims)
+    if (d.v < 1) { set_error("udb_v2old_postprocess: %s=%d must be >= 1", d.name, d.v); return 1; }
+  if (p->mode != UDB_V2OLD_BILINEAR && p->mode != UDB_V2OLD_NEAREST_EXACT) {
+    set_error("udb_v2old_postprocess: `mode` %d is neither UDB_V2OLD_BILINEAR (0) nor UDB_V2OLD_NEAREST_EXACT (1)", p->mode);
+    return 1;
+  }
+  const struct { const void* q; const char* name; } ptrs[] = {{p->depth, "depth"}, {p->confidence, "confidence"}, {p->k4, "k4"},
+                                                             {p->out_depth, "out_depth"}, {p->out_confidence, "out_confidence"},
+                                                             {p->out_points, "out_points"}};
+  for (const auto& a : ptrs)
+    if (!a.q) { set_error("udb_v2old_postprocess: `%s` must be non-null", a.name); return 1; }
+  v2old_postprocess_kernel<<<grid_1d((long long)p->B * p->H * p->W), 256, 0, ST(stream)>>>(*p);
+  return check_launch("v2old_postprocess_kernel");
+}
+
+int udb_v2old_camera(const float* x4, const float* gt_k, int32_t B, int32_t net_h, int32_t net_w, float ratio, float* intr4_rays,
+                     float* k_out, float* k4_points, void* stream) {
+  if (B < 1 || net_h < 1 || net_w < 1 || !(ratio > 0.f)) {
+    set_error("udb_v2old_camera: B=%d net_h=%d net_w=%d ratio=%g: all must be > 0", B, net_h, net_w, ratio);
+    return 1;
+  }
+  if (!x4 || !intr4_rays || !k_out || !k4_points) { set_error("udb_v2old_camera: null output or camera-head pointer"); return 1; }
+  v2old_camera_kernel<<<(B + 63) / 64, 64, 0, ST(stream)>>>(x4, gt_k, B, net_h, net_w, ratio, intr4_rays, k_out, k4_points);
+  return check_launch("v2old_camera_kernel");
+}
+
+}  // extern "C"

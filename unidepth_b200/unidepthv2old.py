@@ -1,0 +1,324 @@
+"""UniDepthV2old (DINOv2 ViT-L/14 or ViT-S/14 encoder) -- drop-in for the reference's inference API, running on libudb.so
+(sm_90a).
+
+Mirrors `unidepth.models.unidepthv2.unidepthv2_old.UniDepthV2old` for the inference path only (reference:
+unidepth/models/unidepthv2/unidepthv2_old.py:126-132 constructor, :198-282 `infer`, :284-300 `load_pretrained`,
+:302-304 `device`, :343-349 the `shape_constraints` / `interpolation_mode` / `resolution_level` attributes; HF-hub mixin
+`from_pretrained`):
+
+    model = UniDepthV2old.from_pretrained(dir_with_config_json_and_safetensors)     # or UniDepthV2old(config)
+    model = model.to("cuda").eval()
+    model.resolution_level = 5                                                       # None: the maximum (10), with a warning
+    out = model.infer(rgb_uint8, intrinsics=None)       # dict: intrinsics points depth confidence
+
+The module owns `nn.Parameter`s under exactly the reference's state-dict names (unidepth_b200/spec_v2old.py), so
+reference checkpoints load unchanged.  `infer` packs the weights once and makes ONE C call (`udb_infer_v2old`,
+include/udb.h) that enqueues the hand-written kernels on torch's current stream, replayed as a CUDA graph per input
+shape.  No CPU / eager fallback.  The network shape follows the input's aspect ratio and the resolution level, so the
+engine (one per network shape, as UniDepthV1's) is rebuilt when that shape changes.
+
+The first decoder level uses Nystrom attention (reference: xformers NystromAttention, absent here); this implementation
+follows the published algorithm as restated in oracle/unidepth_v1_oracle.py, as UniDepthV1 does -- parity for that one
+function is unpinned (see DESIGN.md).
+"""
+from __future__ import annotations
+
+import ctypes as C
+import math
+from typing import Dict, Optional, Tuple
+
+import torch
+import torch.nn.functional as F
+
+from . import _cabi as cabi
+from ._engine_model import HUB_KWARGS, EngineModel, PyTorchModelHubMixin, f16, f32
+from .spec import PATCH
+from .spec_v2old import RAY_K, V2oldSpec, check_ratio, check_resolution, param_shapes
+from .unidepthv1 import _sine_position_embedding
+from .unidepthv2 import pack_vit_encoder
+
+INTERPOLATION_MODES = {"bilinear": 0, "nearest-exact": 1}     # include/udb.h UDB_V2OLD_*
+
+
+def v2old_geometry(H: int, W: int, level: int, pixels_bounds) -> Tuple[Tuple[int, int], float]:
+    """((net_h, net_w), ratio) of an H x W input at the (clipped) resolution level: the engine's own arithmetic
+    (udb_v2old_geometry, unidepthv2_old.py:45-92)."""
+    g = cabi.V2oldGeometry()
+    lo, hi = sorted(pixels_bounds)
+    cabi.check(cabi.lib().udb_v2old_geometry(int(H), int(W), int(level), int(lo), int(hi), C.byref(g)), "udb_v2old_geometry")
+    return (g.net_h, g.net_w), g.ratio
+
+
+class UniDepthV2old(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
+    _ENGINE_FNS = ("udb_v2old_create", "udb_v2old_destroy", "udb_v2old_set_weight", "udb_v2old_set_scalar")
+
+    def __init__(self, config: dict, eps: float = 1e-6, **kwargs):
+        super().__init__(config, eps, max_cached_workspaces=4)
+        self.spec = V2oldSpec(config)
+        self._add_params(param_shapes(config))
+        # the reference's attributes (unidepthv2_old.py:343-349), read on every call
+        sc = dict(config["data"]["shape_constraints"])
+        sc["pixels_bounds_ori"] = list(sc.get("pixels_bounds", [1400, 2400]))
+        self.shape_constraints = sc
+        self.interpolation_mode = "bilinear"
+        self.resolution_level = None
+
+    # ------------------------------------------------------------------ weight packing
+    def _pack_tensors(self, dev, shape: Optional[Tuple[int, int]] = None):
+        """({engine tensor name: tensor on `dev`}, {scalar name: float}) of the weights and of the operands of the
+        network shape `shape` (default: the shape of a 480 x 640 input at the maximum level).  The product packs the
+        two parts separately (`_weights`, `_shape_operands`); tests/test_v2old_cpu.py runs this on the CPU to check,
+        through the engine's dry run, that the packer registers exactly the operands the C schedule asks for."""
+        T, S = self._pack_weights(dev)
+        if shape is None:
+            shape, _ = v2old_geometry(480, 640, 10, self.shape_constraints["pixels_bounds_ori"])
+        T.update(self._shape_operands(shape, dev))
+        return T, S
+
+    def _shape_operands(self, shape: Tuple[int, int], dev) -> Dict[str, torch.Tensor]:
+        """The operands that depend on the network shape: "pos", the DINOv2 position table resized (bicubic, to the
+        patch grid's size: interpolate_offset 0, dinov2.py:267-304); "tokens_pos", the sine position embedding of the
+        patch grid plus the level embedding MLP of the four learned level vectors (decoder_old.py:463-479); and
+        "ray_scales.{i}", the 32 Fourier frequencies 2^linspace(0, log2(max(grid_i) // 2)) of the three decoder grids
+        (positional_embedding.py:230-233), computed on the CPU as the reference computes them."""
+        s = self.spec
+        sd = self.state_dict()
+        pd = "pixel_decoder."
+        hid, D = s.hidden, s.embed_dim
+        gh, gw = shape[0] // PATCH, shape[1] // PATCH
+        c32 = lambda t: t.to(dev, f32).contiguous()
+        T: Dict[str, torch.Tensor] = {}
+        pos = sd["pixel_encoder.pos_embed"].detach().float().reshape(-1, D)
+        M = math.isqrt(pos.shape[0] - 1)
+        grid = pos[1:].reshape(1, M, M, D).permute(0, 3, 1, 2)
+        g = F.interpolate(grid, size=(gh, gw), mode="bicubic", antialias=False)
+        T["pos"] = c32(torch.cat([pos[:1], g.permute(0, 2, 3, 1).reshape(gh * gw, D)], dim=0))
+        le = F.linear(F.gelu(F.linear(sd[pd + "level_embeds"].float(), sd[pd + "level_embed_layer.0.weight"].float(),
+                                      sd[pd + "level_embed_layer.0.bias"].float())),
+                      sd[pd + "level_embed_layer.2.weight"].float(), sd[pd + "level_embed_layer.2.bias"].float())
+        le = F.layer_norm(le, (hid,), sd[pd + "level_embed_layer.3.weight"].float(), sd[pd + "level_embed_layer.3.bias"].float(), 1e-5)
+        sine = _sine_position_embedding(gh, gw, hid // 2, le.device)
+        T["tokens_pos"] = c32((sine[None, :, :] + le[:, None, :]).reshape(4 * gh * gw, hid))
+        for i in range(3):
+            mf = max(gh << i, gw << i) // 2
+            T[f"ray_scales.{i}"] = c32(2.0 ** torch.linspace(0.0, math.log2(mf), steps=32, dtype=f32))
+        return T
+
+    def _pack_weights(self, dev):
+        s = self.spec
+        sd = {k: v.detach() for k, v in self.state_dict().items()}
+        h16 = lambda t: t.to(dev, f16).contiguous()
+        c32 = lambda t: t.to(dev, f32).contiguous()
+        T: Dict[str, torch.Tensor] = {}
+        S: Dict[str, float] = {}
+        pd, dl = "pixel_decoder.", "pixel_decoder.depth_layer."
+        hid, D = s.hidden, s.embed_dim
+
+        def kpad(w, k):
+            out = torch.zeros((w.shape[0], k), dtype=f32, device=w.device)
+            out[:, :w.shape[1]] = w.float()
+            return out
+
+        # ---- encoder: the shared DINOv2 packing; its "pos" is the checkpoint's grid, which the shape's table replaces
+        T.update({k: v.to(dev) for k, v in pack_vit_encoder(sd, D, s.enc_depth, dev).items()})
+        del T["pos"]
+        T["norm_w"], T["norm_b"] = c32(sd["pixel_encoder.norm.weight"]), c32(sd["pixel_encoder.norm.bias"])
+
+        # ---- adapters
+        for l in range(4):
+            a = f"{pd}input_adapter.input_adapters.{l}"
+            T[f"adapt.{l}.ln_w"], T[f"adapt.{l}.ln_b"] = c32(sd[a + ".0.weight"]), c32(sd[a + ".0.bias"])
+            T[f"adapt.{l}.w"], T[f"adapt.{l}.b"] = h16(sd[a + ".1.weight"]), c32(sd[a + ".1.bias"])
+        for dst, src, n in (("ctok", "camera_token_adapter", 4), ("gtok", "global_token_adapter", 2)):
+            for i in range(n):
+                a = f"{pd}{src}.input_adapters.{i}"
+                T[f"{dst}.{i}.ln_w"], T[f"{dst}.{i}.ln_b"] = c32(sd[a + ".0.weight"]), c32(sd[a + ".0.bias"])
+                T[f"{dst}.{i}.w"], T[f"{dst}.{i}.b"] = c32(sd[a + ".1.weight"]), c32(sd[a + ".1.bias"])
+
+        def mlp32(dst, src):
+            T[dst + ".nw"], T[dst + ".nb"] = c32(sd[src + ".norm.weight"]), c32(sd[src + ".norm.bias"])
+            T[dst + ".w1"], T[dst + ".b1"] = c32(sd[src + ".proj1.weight"]), c32(sd[src + ".proj1.bias"])
+            T[dst + ".w2"], T[dst + ".b2"] = c32(sd[src + ".proj2.weight"]), c32(sd[src + ".proj2.bias"])
+
+        def cross_block(dst, src):
+            """a single-head AttentionBlock of the camera / global head: f32 operands of the CUDA-core path, the (k | v)
+            weight f16 for the GEMM over the long context"""
+            for a, b in (("nxw", "norm_attnx.weight"), ("nxb", "norm_attnx.bias"), ("ncw", "norm_attnctx.weight"),
+                         ("ncb", "norm_attnctx.bias"), ("q_w", "q.weight"), ("q_b", "q.bias"), ("kv_b", "kv.bias"),
+                         ("out_w", "out.weight"), ("out_b", "out.bias"), ("ls1", "ls1.gamma"), ("ls2", "ls2.gamma")):
+                T[dst + a] = c32(sd[src + b])
+            T[dst + "kv_w"] = h16(sd[src + "kv.weight"])
+            mlp32(dst + "mlp", src + "mlp")
+
+        # ---- camera head
+        cl = pd + "camera_layer."
+        mlp32("cam.cls", cl + "project_cls")
+        T["cam.inf.nw"], T["cam.inf.nb"] = c32(sd[cl + "in_features.norm.weight"]), c32(sd[cl + "in_features.norm.bias"])
+        T["cam.inf.w1"], T["cam.inf.b1"] = h16(sd[cl + "in_features.proj1.weight"]), c32(sd[cl + "in_features.proj1.bias"])
+        T["cam.inf.w2"], T["cam.inf.b2"] = h16(sd[cl + "in_features.proj2.weight"]), c32(sd[cl + "in_features.proj2.bias"])
+        T["cam.pos"] = c32(sd[cl + "latents_pos"].reshape(4, hid))
+        cross_block("cam.agg1.", cl + "aggregate1.")
+        cross_block("cam.agg2.", cl + "aggregate2.")
+        mlp32("cam.out", cl + "out")
+
+        # ---- global head
+        gl = pd + "global_layer."
+        mlp32("glob.cls", gl + "project_cls")
+        T["glob.rays_w"], T["glob.rays_b"] = h16(kpad(sd[gl + "project_rays.weight"], RAY_K)), c32(sd[gl + "project_rays.bias"])
+        T["glob.in_w"], T["glob.in_b"] = h16(sd[gl + "in_features.weight"]), c32(sd[gl + "in_features.bias"])
+        cross_block("glob.agg1.", gl + "aggregate1.")
+        cross_block("glob.agg2.", gl + "aggregate2.")
+        mlp32("glob.out", gl + "out")
+
+        # ---- depth head
+        for i in range(3):
+            T[f"rays.{i}.w"], T[f"rays.{i}.b"] = h16(kpad(sd[f"{dl}rays_layers.{i}.weight"], RAY_K)), c32(sd[f"{dl}rays_layers.{i}.bias"])
+        T["fcc_w"], T["fcc_b"] = h16(sd[dl + "features_channel_cat.weight"]), c32(sd[dl + "features_channel_cat.bias"])
+        T["lat.nw"], T["lat.nb"] = c32(sd[dl + "to_latents.norm.weight"]), c32(sd[dl + "to_latents.norm.bias"])
+        T["lat.w1"], T["lat.b1"] = h16(sd[dl + "to_latents.proj1.weight"]), c32(sd[dl + "to_latents.proj1.bias"])
+        T["lat.w2"], T["lat.b2"] = h16(sd[dl + "to_latents.proj2.weight"]), c32(sd[dl + "to_latents.proj2.bias"])
+
+        def attn_block(dst, src, split_kv):
+            """V1's packing of the decoder's AttentionBlock / NystromBlock (engine_common.h dense_attn_block, mh_attn_block)"""
+            for a, b in (("nxw", "norm_attnx.weight"), ("nxb", "norm_attnx.bias"), ("ncw", "norm_attnctx.weight"),
+                         ("ncb", "norm_attnctx.bias"), ("q_b", "q.bias"), ("out_b", "out.bias"), ("ls1", "ls1.gamma"),
+                         ("ls2", "ls2.gamma"), ("mnw", "mlp.norm.weight"), ("mnb", "mlp.norm.bias"), ("mb1", "mlp.proj1.bias"),
+                         ("mb2", "mlp.proj2.bias")):
+                T[dst + a] = c32(sd[src + b])
+            for a, b in (("q_w", "q.weight"), ("out_w", "out.weight"), ("mw1", "mlp.proj1.weight"), ("mw2", "mlp.proj2.weight")):
+                T[dst + a] = h16(sd[src + b])
+            kvw, kvb = sd[src + "kv.weight"], sd[src + "kv.bias"]
+            d = kvw.shape[1]
+            if split_kv:
+                T[dst + "k_w"], T[dst + "k_b"] = h16(kvw[:d]), c32(kvb[:d])
+                T[dst + "v_w"], T[dst + "v_b"] = h16(kvw[d:]), c32(kvb[d:])
+            else:
+                T[dst + "kv_w"], T[dst + "kv_b"] = h16(kvw), c32(kvb)
+
+        attn_block("agg16.", dl + "aggregate_16.", True)
+        attn_block("prompt.", dl + "prompt_camera.", True)
+        for j in range(s.dec_depths[0]):
+            attn_block(f"nys.{j}.", f"{dl}process_layers.0.{j}.", False)
+        for i in range(3):
+            c = hid >> i
+            cq, c2 = c // 4, c // 2
+            cqp = -(-cq // 64) * 64
+            u, dst = f"{dl}ups.{i}.", f"up.{i}."
+            for j in range(2):
+                b = f"{u}convs.{j}."
+                w = sd[b + "dwconv.weight"]
+                T[f"{dst}c{j}.dw_w"], T[f"{dst}c{j}.dw_b"] = c32(w.reshape(c, 49).t()), c32(sd[b + "dwconv.bias"])
+                T[f"{dst}c{j}.ln_w"], T[f"{dst}c{j}.ln_b"] = c32(sd[b + "norm.weight"]), c32(sd[b + "norm.bias"])
+                T[f"{dst}c{j}.w1"], T[f"{dst}c{j}.b1"] = h16(sd[b + "pwconv1.weight"]), c32(sd[b + "pwconv1.bias"])
+                T[f"{dst}c{j}.w2"], T[f"{dst}c{j}.b2"] = h16(sd[b + "pwconv2.weight"]), c32(sd[b + "pwconv2.bias"])
+                T[f"{dst}c{j}.gamma"] = c32(sd[b + "gamma"])
+            T[dst + "dw_w"], T[dst + "dw_b"] = c32(sd[u + "up.1.weight"].reshape(cq, 49).t()), c32(sd[u + "up.1.bias"])
+            cw = torch.zeros((c2, 3, 3, cqp), dtype=f32, device=sd[u + "up.3.weight"].device)
+            cw[..., :cq] = sd[u + "up.3.weight"].float().permute(0, 2, 3, 1)         # [C/2, C/4, 3, 3] -> [C/2, (ky, kx, ci)]
+            T[dst + "conv_w"], T[dst + "conv_b"] = h16(cw.reshape(c2, 9 * cqp)), c32(sd[u + "up.3.bias"])
+            T[dst + "res_w"], T[dst + "res_b"] = h16(sd[u + "residual.0.weight"].reshape(c2, c)), c32(sd[u + "residual.0.bias"])
+            # depth_mlp / confidence_mlp: first layers apart, second layers as one block-diagonal [32, 2 * C/2] GEMM weight
+            hm = f"hmlp.{i}."
+            w2 = torch.zeros((32, c), dtype=f32, device=sd[u + "up.3.weight"].device)
+            for k, nm in enumerate(("depth_mlp", "confidence_mlp")):
+                src, p = f"{dl}{nm}.{i}.", hm + ("c." if k else "d.")
+                T[p + "nw"], T[p + "nb"] = c32(sd[src + "norm.weight"]), c32(sd[src + "norm.bias"])
+                T[p + "w1"], T[p + "b1"] = h16(sd[src + "proj1.weight"]), c32(sd[src + "proj1.bias"])
+                w2[16 * k:16 * (k + 1), c2 * k:c2 * (k + 1)] = sd[src + "proj2.weight"].float()
+            T[hm + "w2"] = h16(w2)
+            T[hm + "b2"] = c32(torch.cat([sd[f"{dl}depth_mlp.{i}.proj2.bias"], sd[f"{dl}confidence_mlp.{i}.proj2.bias"]]))
+        T["head_w"] = c32(torch.stack([sd[dl + "to_depth.weight"].reshape(48, 49), sd[dl + "to_confidence.weight"].reshape(48, 49)]))
+        S["head_b_depth"] = float(sd[dl + "to_depth.bias"].item())
+        S["head_b_conf"] = float(sd[dl + "to_confidence.bias"].item())
+        return T, S
+
+    # ------------------------------------------------------------------ engine
+    def _engine_config(self, shape: Tuple[int, int]) -> "cabi.V2oldConfig":
+        """udb_v2old_config_t of this model at the network shape `shape` (include/udb.h)."""
+        s = self.spec
+        cfg = cabi.V2oldConfig()
+        cfg.embed_dim, cfg.enc_depth, cfg.enc_heads = s.embed_dim, s.enc_depth, s.enc_heads
+        for i in range(4):
+            cfg.output_idx[i] = s.output_idx[i]
+        cfg.hidden, cfg.heads, cfg.expansion = s.hidden, s.heads, s.expansion
+        cfg.nystrom_depth = s.dec_depths[0]
+        cfg.net_h, cfg.net_w = shape
+        return cfg
+
+    def _get_engine(self, shape: Tuple[int, int]):
+        """The engine of the network shape `shape`; a new shape makes a new engine with the packed weights and the shape's
+        own operands, and drops the previous one with its workspaces and graphs."""
+        T, _ = self._weights()
+        if self._engine is not None and self._engine_key == shape:
+            return self._engine
+        ops = self._shape_operands(shape, self.device)
+        handle = self._create_engine(self._engine_config(shape), shape, tensors={**T, **ops})
+        self._shape_ops = ops              # the engine borrows their pointers
+        return handle
+
+    def _forward_engine(self, rgb: torch.Tensor, K: Optional[torch.Tensor], scale255: bool, normalize: bool, mode: int):
+        eng = self._engine
+        lib = cabi.lib()
+        dev = rgb.device
+        B, _, H, W = rgb.shape
+        ws = self._workspace((self._engine_key, B, H, W), lambda: lib.udb_v2old_workspace_bytes(eng, B, H, W))
+        out = {"intrinsics": torch.empty((B, 3, 3), device=dev, dtype=f32),
+               "points": torch.empty((B, 3, H, W), device=dev, dtype=f32),
+               "depth": torch.empty((B, 1, H, W), device=dev, dtype=f32),
+               "confidence": torch.empty((B, 1, H, W), device=dev, dtype=f32)}
+        a = cabi.InferV2oldArgs()
+        a.rgb, a.rgb_is_u8, a.scale255, a.normalize = rgb.data_ptr(), int(rgb.dtype == torch.uint8), int(scale255), int(normalize)
+        a.B, a.H, a.W = B, H, W
+        a.intrinsics = K.data_ptr() if K is not None else None
+        a.interpolation = mode
+        a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
+        a.out_intrinsics, a.out_points = out["intrinsics"].data_ptr(), out["points"].data_ptr()
+        a.out_depth, a.out_confidence = out["depth"].data_ptr(), out["confidence"].data_ptr()
+        cabi.check(lib.udb_infer_v2old(eng, C.byref(a), C.c_void_p(torch.cuda.current_stream().cuda_stream)), "udb_infer_v2old")
+        return out
+
+    # ------------------------------------------------------------------ infer
+    @torch.no_grad()
+    def infer(self, rgbs: torch.Tensor, intrinsics=None):
+        """Same contract as the reference `UniDepthV2old.infer` (unidepthv2_old.py:198-282)."""
+        if self.interpolation_mode not in INTERPOLATION_MODES:
+            raise NotImplementedError(f"interpolation_mode {self.interpolation_mode!r}: only 'bilinear' and 'nearest-exact' "
+                                      "are implemented")
+        mode = INTERPOLATION_MODES[self.interpolation_mode]
+        if rgbs.ndim == 3:
+            rgbs = rgbs.unsqueeze(0)
+        if intrinsics is not None and intrinsics.ndim == 2:
+            intrinsics = intrinsics.unsqueeze(0)
+        dev = self.device
+        if dev.type != "cuda":
+            raise RuntimeError("unidepth_b200 has no CPU path: move the model to a CUDA device")
+        B, _, H, W = rgbs.shape
+        level = check_resolution(self.resolution_level)
+        check_ratio((H, W), self.shape_constraints["ratio_bounds"])
+        shape, _ = v2old_geometry(H, W, level, self.shape_constraints["pixels_bounds_ori"])
+        with torch.cuda.device(dev):
+            rgbs = rgbs.to(dev)
+            # unidepthv2_old.py:211-218: "/255" when the data looks like 0..255, ImageNet normalisation when it then lies in [0, 1]
+            if rgbs.dtype == torch.uint8:
+                scale255, normalize = True, True
+            else:
+                rgbs = rgbs.float()
+                mx, mn = float(rgbs.max()), float(rgbs.min())
+                scale255 = mx > 5
+                if scale255:
+                    mx, mn = mx / 255.0, mn / 255.0
+                normalize = mn >= 0.0 and mx <= 1.0
+            rgbs = rgbs.contiguous()
+            K = None
+            if intrinsics is not None:
+                K = intrinsics.to(dev, f32).reshape(-1, 3, 3)
+                if K.shape[0] != B:
+                    raise ValueError(f"intrinsics holds {K.shape[0]} matrices for a batch of {B} images")
+                K = K.contiguous()
+            self._get_engine(shape)
+            run = lambda x, inputs: self._forward_engine(x, inputs.get("K"), scale255, normalize, mode)
+            key = (shape, tuple(rgbs.shape), rgbs.dtype, scale255, normalize, K is not None, mode)
+            return self._run_graphed(run, rgbs, {} if K is None else {"K": K}, key)
+
+    def forward(self, *args, **kwargs):
+        raise NotImplementedError("training / validation forward of UniDepthV2old is out of scope; use .infer()")
