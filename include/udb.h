@@ -666,8 +666,9 @@ int udb_infer_v2(udb_engine* e, const udb_infer_args_t* a, void* stream);
 /* ---------------------------------------------------------------------------------------------
  * UniDepthV1 engine: the whole `UniDepthV1.infer` path (ConvNeXt or DINOv2 encoder) as one call (SURVEY.md section 8b
  * `udb_infer_v1`; reference unidepth/models/unidepthv1/unidepthv1.py:288-373).  Same contract as the V2 engine: the
- * caller owns packed weights (names listed in unidepth_b200/unidepthv1.py::_pack), workspace and outputs; nothing is
- * allocated, copied or synchronised inside udb_infer_v1.
+ * caller owns packed weights (names listed by unidepth_b200/unidepthv1.py UniDepthV1._pack_tensors, with the packers
+ * the V1-family decoders share in unidepth_b200/_pack.py), workspace and outputs; nothing is allocated, copied or
+ * synchronised inside udb_infer_v1.
  * ------------------------------------------------------------------------------------------- */
 typedef struct udb_engine_v1 udb_engine_v1;
 
@@ -735,8 +736,9 @@ int udb_infer_v1(udb_engine_v1* e, const udb_infer_v1_args_t* a, void* stream);
  * UniDepthV2old engine: the whole `UniDepthV2old.infer` path (DINOv2 ViT-L/14 or ViT-S/14) as one call (reference
  * unidepth/models/unidepthv2/unidepthv2_old.py:198-282, decoder_old.py).  One engine per network shape (net_h, net_w),
  * which `udb_v2old_geometry` derives from the input size and the resolution level; otherwise the contract of the V1 engine:
- * the caller owns the packed weights (names in unidepth_b200/unidepthv2old.py::_pack_tensors), workspace and outputs, and
- * nothing is allocated, copied or synchronised inside udb_infer_v2old.
+ * the caller owns the packed weights (names listed by unidepth_b200/unidepthv2old.py UniDepthV2old._pack_tensors, with
+ * the packers the V1-family decoders share in unidepth_b200/_pack.py), workspace and outputs, and nothing is allocated,
+ * copied or synchronised inside udb_infer_v2old.
  * ------------------------------------------------------------------------------------------- */
 typedef struct udb_engine_v2old udb_engine_v2old;
 

@@ -20,7 +20,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 from fixture import make_state_dict  # noqa: E402
 from unidepth_b200 import UniDepthV2, _cabi  # noqa: E402
-from unidepth_b200.unidepthv2 import pack_e4m3  # noqa: E402
+from unidepth_b200._pack import pack_e4m3  # noqa: E402
 
 CPU = torch.device("cpu")
 E4M3 = torch.float8_e4m3fn

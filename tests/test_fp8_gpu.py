@@ -76,7 +76,7 @@ def test_e4m3_gemm_against_fp64(M, N, K):
     a8, sa = _quant_ref(a)
     a8p = torch.zeros((M, lda), dtype=E4M3)
     a8p[:, :K] = a8
-    from unidepth_b200.unidepthv2 import pack_e4m3
+    from unidepth_b200._pack import pack_e4m3
     w8, sw = pack_e4m3(w)
     w8p = torch.zeros((N, lda), dtype=E4M3)
     w8p[:, :K] = w8

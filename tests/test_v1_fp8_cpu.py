@@ -15,7 +15,7 @@ import torch.nn.functional as F
 from test_fp8_cpu import fp8_encoder
 from unidepth_b200 import UniDepthV1, _cabi
 from unidepth_b200.unidepthv1 import FP8_STAGES
-from unidepth_b200.unidepthv2 import pack_e4m3
+from unidepth_b200._pack import pack_e4m3
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden")

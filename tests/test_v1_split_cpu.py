@@ -5,7 +5,7 @@ import pytest
 import torch
 
 from test_v1_fp8_cpu import SMALL, _bytes, _model
-from unidepth_b200.unidepthv1 import split_weight
+from unidepth_b200._pack import split_weight
 
 CPU = torch.device("cpu")
 CASES = [("config_v1_cnvnxtl.json", SMALL), ("config_v1_cnvnxtl.json", None), ("config_v1_vitl14.json", None)]

@@ -14,6 +14,8 @@ ACT_NONE, ACT_GELU, ACT_LEAKY = 0, 1, 2
 STORE_ROWS, STORE_CONVT, STORE_CONVTILE, STORE_HEAD = 0, 1, 2, 3
 INTERP_BILINEAR, INTERP_BICUBIC = 0, 1
 INTERP_MODES = {"bilinear": INTERP_BILINEAR, "bicubic": INTERP_BICUBIC}
+V2OLD_BILINEAR, V2OLD_NEAREST_EXACT = 0, 1      # udb.h UDB_V2OLD_*: UniDepthV2old's depth resize
+V2OLD_INTERP_MODES = {"bilinear": V2OLD_BILINEAR, "nearest-exact": V2OLD_NEAREST_EXACT}
 CAM_NONE, CAM_PINHOLE, CAM_EUCM, CAM_SPHERICAL, CAM_OPENCV, CAM_FISHEYE624, CAM_MEI = range(7)
 CAM_STRIDE = 20      # floats per packed camera row (udb.h UDB_CAM_STRIDE)
 

@@ -1,8 +1,11 @@
-"""Host runtime shared by UniDepthV1 and UniDepthV2: parameters under the reference's state-dict names, checkpoint
-loading, weight packing per weight version, the C engine's lifetime, and the workspace and CUDA-graph caches.
+"""Host runtime shared by UniDepthV1, UniDepthV2 and UniDepthV2old: parameters under the reference's state-dict names,
+checkpoint loading, weight packing per weight version, the C engine's lifetime, the engine of a network shape, the input
+block of `infer`, and the workspace and CUDA-graph caches.
 
-A model class supplies its packer (`_pack_tensors` -> ({engine tensor name: tensor}, {scalar name: float})), its engine
-(`_get_engine`, `_forward_engine`) and the names of its engine's C entry points (`_ENGINE_FNS`)."""
+A model class supplies its packer (`_pack_tensors` -> ({engine tensor name: tensor}, {scalar name: float}); the shared
+packing code is `_pack.py`), its engine (`_forward_engine`, and the lookup of the current engine: `_shape_engine` with the
+model's `_shape_operands` for one engine per network shape) and the names of its engine's C entry points
+(`_ENGINE_FNS`)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -32,6 +35,32 @@ HUB_KWARGS = dict(library_name="UniDepth", repo_url="https://github.com/lpiccine
 
 f16, f32 = torch.float16, torch.float32
 _DTYPES = {f16: cabi.DT_F16, f32: cabi.DT_F32, torch.float8_e4m3fn: cabi.DT_E4M3}   # udb.h UDB_DT_*
+
+
+def infer_inputs(rgbs: torch.Tensor, intrinsics, dev):
+    """The input block of UniDepthV1.infer and UniDepthV2old.infer (unidepthv1.py:301-308, unidepthv2_old.py:211-218)
+    -> (rgbs, K, scale255, normalize): the batch on `dev`, uint8 or f32, contiguous; "/255" when the data looks like
+    0..255, ImageNet normalisation when it then lies in [0, 1] (uint8: both); K the intrinsics as [B, 3, 3] f32, one
+    matrix per image, or None."""
+    rgbs = rgbs.to(dev)
+    B = rgbs.shape[0]
+    if rgbs.dtype == torch.uint8:
+        scale255, normalize = True, True
+    else:
+        rgbs = rgbs.float()
+        mx, mn = float(rgbs.max()), float(rgbs.min())
+        scale255 = mx > 5
+        if scale255:
+            mx, mn = mx / 255.0, mn / 255.0
+        normalize = mn >= 0.0 and mx <= 1.0
+    rgbs = rgbs.contiguous()
+    K = None
+    if intrinsics is not None:
+        K = intrinsics.to(dev, f32).reshape(-1, 3, 3)
+        if K.shape[0] != B:
+            raise ValueError(f"intrinsics holds {K.shape[0]} matrices for a batch of {B} images")
+        K = K.contiguous()
+    return rgbs, K, scale255, normalize
 
 
 class _Node(nn.Module):
@@ -78,6 +107,13 @@ class EngineModel(nn.Module):
     @property
     def device(self):
         return next(self.parameters()).device
+
+    def _cuda_device(self):
+        """The model's device, which `infer` needs to be a CUDA device."""
+        dev = self.device
+        if dev.type != "cuda":
+            raise RuntimeError("unidepth_b200 has no CPU path: move the model to a CUDA device")
+        return dev
 
     def load_pretrained(self, model_file: str):
         """unidepthv2.py:381-394 / unidepthv1.py:375-392: torch checkpoint, optional 'model' key, strip 'module.'."""
@@ -158,6 +194,19 @@ class EngineModel(nn.Module):
             raise
         self._drop_engine()
         self._engine, self._engine_key, self._engine_device = handle, key, self.device
+        return handle
+
+    def _shape_engine(self, shape, cfg, check=None):
+        """The engine of the network shape `shape` (UniDepthV1, UniDepthV2old: one engine per shape).  A new shape makes
+        a new engine for the config struct `cfg` with the packed weights and the shape's own operands
+        (`_shape_operands`); `_create_engine` drops the previous one, with its workspaces and graphs, only once the new
+        one has passed `check`."""
+        T, _ = self._weights()
+        if self._engine is not None and self._engine_key == shape:
+            return self._engine
+        ops = self._shape_operands(shape, self.device)
+        handle = self._create_engine(cfg, shape, tensors={**T, **ops}, check=check)
+        self._shape_ops = ops              # the engine borrows their pointers
         return handle
 
     def _drop_engine(self):

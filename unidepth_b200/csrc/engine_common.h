@@ -478,7 +478,7 @@ static inline void vit_block_e4m3(Ctx& c, const std::string& b, float* x, const 
 }
 
 // `depth` pre-norm transformer blocks (metadinov2/block.py:84-109, LayerNorm eps 1e-6) on the f32 residual stream
-// x [B*T, D], weights "<prefix><i>.<operand>" as unidepthv2.pack_vit_encoder packs them.  after_block(i) runs once block
+// x [B*T, D], weights "<prefix><i>.<operand>" as _pack.pack_vit_encoder packs them.  after_block(i) runs once block
 // i has updated x (the engines read their encoder outputs there).  The scratch it allocates is released on return.
 template <class Hook>
 static inline void vit_blocks(Ctx& c, const std::string& prefix, float* x, const VitBlocks& v, Hook&& after_block) {

@@ -110,6 +110,34 @@ def vit_encoder_shapes(out: "OrderedDict[str, tuple]", d: int, depth: int, pe: s
     out[pe + "norm.bias"] = (d,)
 
 
+def attn_decoder_shapes(out: "OrderedDict[str, tuple]", ex: int):
+    """(ln, lin, mlp, attn_block): functions that append the state-dict entries of a LayerNorm, a Linear, an Mlp and an
+    AttentionBlock with biases and layer scales (MLP expansion `ex`) to `out`, in the reference's order; the decoder of
+    UniDepthV1 (spec_v1.param_shapes) and UniDepthV2old (spec_v2old.param_shapes) is built from them."""
+
+    def ln(p, c):
+        out[p + ".weight"], out[p + ".bias"] = (c,), (c,)
+
+    def lin(p, cout, cin):
+        out[p + ".weight"], out[p + ".bias"] = (cout, cin), (cout,)
+
+    def mlp(p, c, expansion, outd=None):
+        ln(p + ".norm", c)
+        lin(p + ".proj1", int(c * expansion), c)
+        lin(p + ".proj2", outd if outd is not None else c, int(c * expansion))
+
+    def attn_block(p, c):
+        mlp(p + ".mlp", c, ex)
+        lin(p + ".kv", 2 * c, c)
+        lin(p + ".q", c, c)
+        ln(p + ".norm_attnx", c)
+        ln(p + ".norm_attnctx", c)
+        lin(p + ".out", c, c)
+        out[p + ".ls1.gamma"], out[p + ".ls2.gamma"] = (c,), (c,)
+
+    return ln, lin, mlp, attn_block
+
+
 def param_shapes(config: dict) -> "OrderedDict[str, tuple]":
     """key -> shape of every tensor in the reference UniDepthV2 `state_dict()` (same names, same
     order of magnitude as SURVEY.md section 8b), so reference checkpoints load unchanged."""

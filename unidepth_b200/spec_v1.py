@@ -8,7 +8,7 @@ import math
 from collections import OrderedDict
 from typing import Dict, Tuple
 
-from .spec import PATCH, vit_encoder_shapes
+from .spec import PATCH, attn_decoder_shapes, vit_encoder_shapes
 
 CONVNEXT_ARCHS = {
     # encoder.py:127-136 (`convnext_large`): depths / dims / per-stage end indices used as `output_idx`
@@ -127,26 +127,7 @@ def param_shapes(config: dict) -> "OrderedDict[str, tuple]":
 
     pd = "pixel_decoder."
     hid, ex = s.hidden, s.expansion
-
-    def ln(p, c):
-        out[p + ".weight"], out[p + ".bias"] = (c,), (c,)
-
-    def lin(p, cout, cin):
-        out[p + ".weight"], out[p + ".bias"] = (cout, cin), (cout,)
-
-    def mlp(p, c, expansion, outd=None):
-        ln(p + ".norm", c)
-        lin(p + ".proj1", int(c * expansion), c)
-        lin(p + ".proj2", outd if outd is not None else c, int(c * expansion))
-
-    def attn_block(p, c):
-        mlp(p + ".mlp", c, ex)
-        lin(p + ".kv", 2 * c, c)
-        lin(p + ".q", c, c)
-        ln(p + ".norm_attnx", c)
-        ln(p + ".norm_attnctx", c)
-        lin(p + ".out", c, c)
-        out[p + ".ls1.gamma"], out[p + ".ls2.gamma"] = (c,), (c,)
+    ln, lin, mlp, attn_block = attn_decoder_shapes(out, ex)
 
     def conv_upsample(p, c):
         for j in range(2):

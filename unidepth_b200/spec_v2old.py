@@ -9,7 +9,7 @@ import warnings
 from collections import OrderedDict
 from typing import Tuple
 
-from .spec import PATCH, vit_encoder_shapes
+from .spec import PATCH, attn_decoder_shapes, vit_encoder_shapes
 
 # encoder.py:139-193 (`dinov2_vits14`, `dinov2_vitl14`): width, blocks, heads
 DINO_ARCHS = {
@@ -91,26 +91,7 @@ def param_shapes(config: dict) -> "OrderedDict[str, tuple]":
     vit_encoder_shapes(out, s.embed_dim, s.enc_depth)
     pd = "pixel_decoder."
     hid, ex, D = s.hidden, s.expansion, s.embed_dim
-
-    def ln(p, c):
-        out[p + ".weight"], out[p + ".bias"] = (c,), (c,)
-
-    def lin(p, cout, cin):
-        out[p + ".weight"], out[p + ".bias"] = (cout, cin), (cout,)
-
-    def mlp(p, c, expansion, outd=None):
-        ln(p + ".norm", c)
-        lin(p + ".proj1", int(c * expansion), c)
-        lin(p + ".proj2", outd if outd is not None else c, int(c * expansion))
-
-    def attn_block(p, c):
-        mlp(p + ".mlp", c, ex)
-        lin(p + ".kv", 2 * c, c)
-        lin(p + ".q", c, c)
-        ln(p + ".norm_attnx", c)
-        ln(p + ".norm_attnctx", c)
-        lin(p + ".out", c, c)
-        out[p + ".ls1.gamma"], out[p + ".ls2.gamma"] = (c,), (c,)
+    ln, lin, mlp, attn_block = attn_decoder_shapes(out, ex)
 
     cl = pd + "camera_layer"
     attn_block(cl + ".aggregate1", hid)

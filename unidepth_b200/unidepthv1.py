@@ -19,61 +19,22 @@ function is unpinned (see DESIGN.md).
 from __future__ import annotations
 
 import ctypes as C
-import math
 import operator
 from typing import Dict, Optional, Tuple
 
 import torch
-import torch.nn.functional as F
 
 from . import _cabi as cabi
+from ._pack import (adapter, attn_block, c32, convnext_block, cross_block, h16, latents, mlp, pack_vit_encoder,
+                    pos_table_by_scale, split_weight, tokens_pos)
 from .spec import PATCH
 from .spec_v1 import (ENCODER_CONVNEXT, ENCODER_DINOV2, V1_INTERPOLATE_OFFSET, V1Spec, param_shapes, v1_paddings,
                       v1_shapes)
-from ._engine_model import HUB_KWARGS, EngineModel, PyTorchModelHubMixin, f16, f32
-from .unidepthv2 import pack_e4m3, pack_vit_encoder
+from ._engine_model import HUB_KWARGS, EngineModel, PyTorchModelHubMixin, f32, infer_inputs
 
 # ConvNeXt stages whose blocks run on e4m3 operands in precision "fp8" (engine_v1.cu kFp8Stage, the same fixed rule: a
 # stage runs e4m3 only where that is measured faster, which on an H100 is none of them, DESIGN.md section 8)
 FP8_STAGES = (False, False, False, False)
-
-
-def split_weight(w: torch.Tensor) -> torch.Tensor:
-    """GEMM weight [N, K] of the split-precision mode: [N, 3K] = [hi | hi | lo] f16 with hi = f16(w), lo = f16(w - hi)
-    (include/udb.h udb_gemm_t.a_split_k; the layout unidepthv2.pack_vit_encoder(split=True) packs)."""
-    w = w.to(f32)
-    hi = w.to(f16)
-    lo = (w - hi.to(f32)).to(f16)
-    return torch.cat([hi, hi, lo], dim=1).contiguous()
-
-
-def _offset_pos_embed(pos: torch.Tensor, gh: int, gw: int, offset: float) -> torch.Tensor:
-    """DINOv2 position table of a gh x gw patch grid with a nonzero interpolate_offset (dinov2.py:267-304): bicubic
-    resize of the M x M grid with scale factors ((gh + offset) / M, (gw + offset) / M), height first, so the sampling
-    positions use 1 / scale_factor rather than M / gh.  pos [1 + M*M, D] -> [1 + gh*gw, D], cls row first.  A constant
-    of the weights and the network shape, evaluated when the engine for that shape is made."""
-    D = pos.shape[1]
-    M = math.isqrt(pos.shape[0] - 1)
-    grid = pos[1:].float().reshape(1, M, M, D).permute(0, 3, 1, 2)
-    g = F.interpolate(grid, scale_factor=((gh + offset) / M, (gw + offset) / M), mode="bicubic", antialias=False)
-    if tuple(g.shape[-2:]) != (gh, gw):
-        raise ValueError(f"position grid resized to {tuple(g.shape[-2:])}, expected {(gh, gw)}")
-    return torch.cat([pos[:1].float(), g.permute(0, 2, 3, 1).reshape(gh * gw, D)], dim=0)
-
-
-def _sine_position_embedding(h: int, w: int, num_pos_feats: int, device) -> torch.Tensor:
-    """PositionEmbeddingSine(num_pos_feats, normalize=True) of an all-valid h x w grid -> [h*w, 2*num_pos_feats]
-    (layers/positional_encoding.py:15-59: y features then x features, sin on even / cos on odd feature indices).
-    Evaluated on the host side when the engine for a network shape is made (a constant of the shape)."""
-    eps, scale = 1e-6, 2 * math.pi
-    y = torch.arange(1, h + 1, dtype=f32, device=device)[:, None].expand(h, w) / (h + eps) * scale
-    x = torch.arange(1, w + 1, dtype=f32, device=device)[None, :].expand(h, w) / (w + eps) * scale
-    dim_t = torch.arange(num_pos_feats, dtype=f32, device=device)
-    dim_t = 10000.0 ** (2 * torch.div(dim_t, 2, rounding_mode="floor") / num_pos_feats)
-    px, py = x[..., None] / dim_t, y[..., None] / dim_t
-    px = torch.stack((px[..., 0::2].sin(), px[..., 1::2].cos()), dim=3).flatten(2)
-    py = torch.stack((py[..., 0::2].sin(), py[..., 1::2].cos()), dim=3).flatten(2)
-    return torch.cat((py, px), dim=2).reshape(h * w, 2 * num_pos_feats)
 
 
 class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
@@ -138,20 +99,12 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         "pos", the patch grid's position table (dinov2.py:267-304)."""
         s = self.spec
         sd = self.state_dict()
-        pd = "pixel_decoder."
-        hid = s.hidden
         hc, wc = s.common_grid(shape)
-        c32 = lambda t: t.to(f32).contiguous()
         T: Dict[str, torch.Tensor] = {}
         if s.encoder == ENCODER_DINOV2:
             pos = c32(sd["pixel_encoder.pos_embed"].detach().reshape(-1, s.embed_dim))
-            T["pos"] = c32(_offset_pos_embed(pos, hc, wc, V1_INTERPOLATE_OFFSET))
-        le = F.linear(F.gelu(F.linear(sd[pd + "level_embeds"].float(), sd[pd + "level_embed_layer.0.weight"].float(),
-                                      sd[pd + "level_embed_layer.0.bias"].float())),
-                      sd[pd + "level_embed_layer.2.weight"].float(), sd[pd + "level_embed_layer.2.bias"].float())
-        le = F.layer_norm(le, (hid,), sd[pd + "level_embed_layer.3.weight"].float(), sd[pd + "level_embed_layer.3.bias"].float(), 1e-5)
-        pos = _sine_position_embedding(hc, wc, hid // 2, dev)
-        T["tokens_pos"] = c32((pos[None, :, :] + le[:, None, :]).reshape(4 * hc * wc, hid))
+            T["pos"] = c32(pos_table_by_scale(pos, hc, wc, V1_INTERPOLATE_OFFSET))
+        T["tokens_pos"] = tokens_pos(sd, hc, wc, s.hidden, dev)
         return T
 
     def _pack_weights(self, dev):
@@ -162,10 +115,8 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
             raise ValueError(f"precision must be 'split', 'f16' or 'fp8', not {self.precision!r}")
         split, fp8 = self.precision == "split", self.precision == "fp8"
         sd = {k: v.detach() for k, v in self.state_dict().items()}
-        h16 = lambda t: t.to(f16).contiguous()
-        c32 = lambda t: t.to(f32).contiguous()
         # GEMM weight of the split-precision mode's operands: [N, 3K] = [hi | hi | lo], or f16 in the other modes
-        s16 = lambda t: split_weight(t) if split else h16(t)
+        s16 = split_weight if split else h16
         T: Dict[str, torch.Tensor] = {}
         # an engine without "precision" runs the f16 mode, so the f16 packing registers exactly the scalars it always has
         S: Dict[str, float] = {"precision": 2.0} if fp8 else ({"precision": 1.0} if split else {})
@@ -182,29 +133,11 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
             out[:t.shape[0]] = t
             return out
 
-        def block(dst, src, conv_names, e4m3=False, enc16=h16):
-            """ConvNeXt block operands: depthwise weights tap-major [49, C] f32, MLP weights f16 (`enc16`: split in the
-            encoder's split mode), or e4m3 with per-output-channel scales (`w1_8` / `w1_8s`, `w2_8` / `w2_8s`; pack_e4m3) for
-            a block of the fp8 mode."""
-            dw, norm, fc1, fc2 = conv_names
-            w = sd[f"{src}{dw}.weight"]
-            T[dst + "dw_w"] = c32(w.reshape(w.shape[0], 49).t())
-            T[dst + "dw_b"] = c32(sd[f"{src}{dw}.bias"])
-            T[dst + "ln_w"], T[dst + "ln_b"] = c32(sd[f"{src}{norm}.weight"]), c32(sd[f"{src}{norm}.bias"])
-            T[dst + "b1"], T[dst + "b2"] = c32(sd[f"{src}{fc1}.bias"]), c32(sd[f"{src}{fc2}.bias"])
-            if e4m3:
-                T[dst + "w1_8"], T[dst + "w1_8s"] = pack_e4m3(sd[f"{src}{fc1}.weight"])
-                T[dst + "w2_8"], T[dst + "w2_8s"] = pack_e4m3(sd[f"{src}{fc2}.weight"])
-            else:
-                T[dst + "w1"], T[dst + "w2"] = enc16(sd[f"{src}{fc1}.weight"]), enc16(sd[f"{src}{fc2}.weight"])
-            T[dst + "gamma"] = c32(sd[f"{src}gamma"])
-
         # ---- encoder
         if s.encoder == ENCODER_DINOV2:
-            # the V2 encoder's f16 or fp8 packing; the final norm, mask token and register tokens are never read
-            # (use_norm=False, dinov2.py:173-178).  Its "pos" is the checkpoint's grid: the shape's table replaces it.
+            # the V2 encoder's packing; the final norm, mask token and register tokens are never read (use_norm=False,
+            # dinov2.py:173-178), and the position table is a shape operand
             T.update(pack_vit_encoder(sd, s.embed_dim, s.enc_depth, dev, split=split, fp8=fp8))
-            del T["pos"]
         for i, depth in enumerate(s.depths if s.encoder == ENCODER_CONVNEXT else ()):
             if i == 0:
                 T["stem_w"] = s16(zpad(sd[pe + "stem.0.weight"].reshape(s.dims[0], 48), s.dims[0], 64))
@@ -216,45 +149,27 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
                 T[f"ds{i}.ln_w"], T[f"ds{i}.ln_b"] = c32(sd[st + "downsample.0.weight"]), c32(sd[st + "downsample.0.bias"])
                 T[f"ds{i}.w"], T[f"ds{i}.b"] = s16(w.permute(0, 2, 3, 1).reshape(w.shape[0], -1)), c32(sd[st + "downsample.1.bias"])
             for j in range(depth):
-                block(f"s{i}.b{j}.", f"{st}blocks.{j}.", ("conv_dw", "norm", "mlp.fc1", "mlp.fc2"), fp8 and FP8_STAGES[i], s16)
+                convnext_block(T, sd, f"s{i}.b{j}.", f"{st}blocks.{j}.", ("conv_dw", "norm", "mlp.fc1", "mlp.fc2"),
+                               fp8 and FP8_STAGES[i], s16)
 
         # ---- decoder: adapters, embeddings
         for l in range(4):
-            a = f"{pd}input_adapter.input_adapters.{l}"
-            T[f"adapt.{l}.ln_w"], T[f"adapt.{l}.ln_b"] = c32(sd[a + ".0.weight"]), c32(sd[a + ".0.bias"])
-            T[f"adapt.{l}.w"], T[f"adapt.{l}.b"] = h16(sd[a + ".1.weight"]), c32(sd[a + ".1.bias"])
+            a = f"{pd}input_adapter.input_adapters.{l}."
+            adapter(T, sd, f"adapt.{l}.", a, h16)
             if split:       # the adapter's copy for the camera head, which reads it on split operands
-                T[f"adapt.{l}.w_cam"] = split_weight(sd[a + ".1.weight"])
-            t = f"{pd}token_adapter.input_adapters.{l}"
-            T[f"tok.{l}.ln_w"], T[f"tok.{l}.ln_b"] = c32(sd[t + ".0.weight"]), c32(sd[t + ".0.bias"])
-            T[f"tok.{l}.w"], T[f"tok.{l}.b"] = c32(sd[t + ".1.weight"]), c32(sd[t + ".1.bias"])
-
-        def mlp32(dst, src):
-            T[dst + ".nw"], T[dst + ".nb"] = c32(sd[src + ".norm.weight"]), c32(sd[src + ".norm.bias"])
-            T[dst + ".w1"], T[dst + ".b1"] = c32(sd[src + ".proj1.weight"]), c32(sd[src + ".proj1.bias"])
-            T[dst + ".w2"], T[dst + ".b2"] = c32(sd[src + ".proj2.weight"]), c32(sd[src + ".proj2.bias"])
+                T[f"adapt.{l}.w_cam"] = split_weight(sd[a + "1.weight"])
+            adapter(T, sd, f"tok.{l}.", f"{pd}token_adapter.input_adapters.{l}.", c32)
 
         cl = pd + "camera_layer."
         T["cam.cls.nw"], T["cam.cls.nb"] = c32(sd[cl + "cls_project.0.weight"]), c32(sd[cl + "cls_project.0.bias"])
         T["cam.cls.w1"], T["cam.cls.b1"] = c32(sd[cl + "cls_project.1.weight"]), c32(sd[cl + "cls_project.1.bias"])
         T["cam.cls.w2"], T["cam.cls.b2"] = c32(sd[cl + "cls_project.3.weight"]), c32(sd[cl + "cls_project.3.bias"])
-        T["cam.inf.nw"], T["cam.inf.nb"] = c32(sd[cl + "in_features.norm.weight"]), c32(sd[cl + "in_features.norm.bias"])
-        T["cam.inf.w1"], T["cam.inf.b1"] = s16(sd[cl + "in_features.proj1.weight"]), c32(sd[cl + "in_features.proj1.bias"])
-        T["cam.inf.w2"], T["cam.inf.b2"] = s16(sd[cl + "in_features.proj2.weight"]), c32(sd[cl + "in_features.proj2.bias"])
+        mlp(T, sd, "cam.inf", cl + "in_features", s16)
         T["cam.pos"] = c32(sd[cl + "latents_pos"].reshape(4, hid))
-
-        def cam_block(dst, src, kv_half):
-            for a, b in (("nxw", "norm_attnx.weight"), ("nxb", "norm_attnx.bias"), ("ncw", "norm_attnctx.weight"),
-                         ("ncb", "norm_attnctx.bias"), ("q_w", "q.weight"), ("q_b", "q.bias"), ("kv_b", "kv.bias"),
-                         ("out_w", "out.weight"), ("out_b", "out.bias"), ("ls1", "ls1.gamma"), ("ls2", "ls2.gamma")):
-                T[dst + a] = c32(sd[src + b])
-            T[dst + "kv_w"] = s16(sd[src + "kv.weight"]) if kv_half else c32(sd[src + "kv.weight"])
-            mlp32(dst + "mlp", src + "mlp")
-
-        cam_block("cam.agg.", cl + "aggregate.", True)
+        cross_block(T, sd, "cam.agg.", cl + "aggregate.", s16)
         for i in range(2):
-            cam_block(f"cam.l{i}.", f"{cl}layers.{i}.", False)
-        mlp32("cam.out", cl + "out")
+            cross_block(T, sd, f"cam.l{i}.", f"{cl}layers.{i}.", c32)
+        mlp(T, sd, "cam.out", cl + "out", c32)
 
         dl = pd + "depth_layer."
         for name, outd in (("16", hid), ("8", hid // 2), ("4", hid // 4)):
@@ -264,35 +179,15 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
             T[f"rays.{name}.b1"] = zpad1(sd[src + ".proj1.bias"].float(), 384)
             T[f"rays.{name}.w2"] = h16(zpad(sd[src + ".proj2.weight"].float(), outd, 384))
             T[f"rays.{name}.b2"] = c32(sd[src + ".proj2.bias"])
-        T["fcc_w"], T["fcc_b"] = h16(sd[dl + "features_channel_cat.weight"]), c32(sd[dl + "features_channel_cat.bias"])
-        T["lat.nw"], T["lat.nb"] = c32(sd[dl + "to_latents.norm.weight"]), c32(sd[dl + "to_latents.norm.bias"])
-        T["lat.w1"], T["lat.b1"] = h16(sd[dl + "to_latents.proj1.weight"]), c32(sd[dl + "to_latents.proj1.bias"])
-        T["lat.w2"], T["lat.b2"] = h16(sd[dl + "to_latents.proj2.weight"]), c32(sd[dl + "to_latents.proj2.bias"])
-
-        def attn_block(dst, src, split_kv):
-            for a, b in (("nxw", "norm_attnx.weight"), ("nxb", "norm_attnx.bias"), ("ncw", "norm_attnctx.weight"),
-                         ("ncb", "norm_attnctx.bias"), ("q_b", "q.bias"), ("out_b", "out.bias"), ("ls1", "ls1.gamma"),
-                         ("ls2", "ls2.gamma"), ("mnw", "mlp.norm.weight"), ("mnb", "mlp.norm.bias"), ("mb1", "mlp.proj1.bias"),
-                         ("mb2", "mlp.proj2.bias")):
-                T[dst + a] = c32(sd[src + b])
-            for a, b in (("q_w", "q.weight"), ("out_w", "out.weight"), ("mw1", "mlp.proj1.weight"), ("mw2", "mlp.proj2.weight")):
-                T[dst + a] = h16(sd[src + b])
-            kvw, kvb = sd[src + "kv.weight"], sd[src + "kv.bias"]
-            d = kvw.shape[1]
-            if split_kv:       # dense single-head blocks: k and v projections are separate GEMM operands
-                T[dst + "k_w"], T[dst + "k_b"] = h16(kvw[:d]), c32(kvb[:d])
-                T[dst + "v_w"], T[dst + "v_b"] = h16(kvw[d:]), c32(kvb[d:])
-            else:
-                T[dst + "kv_w"], T[dst + "kv_b"] = h16(kvw), c32(kvb)
-
-        attn_block("agg16.", dl + "aggregate_16.", True)
-        attn_block("prompt.", dl + "prompt_camera.", True)
+        latents(T, sd, dl)
+        attn_block(T, sd, "agg16.", dl + "aggregate_16.", True)
+        attn_block(T, sd, "prompt.", dl + "prompt_camera.", True)
         for name, dst, n in (("layers_16", "l16", s.dec_depths[0]), ("layers_8", "l8", s.dec_depths[1]), ("layers_4", "l4", s.dec_depths[2])):
             for i in range(n):
-                attn_block(f"{dst}.{i}.", f"{dl}{name}.{i}.", False)
+                attn_block(T, sd, f"{dst}.{i}.", f"{dl}{name}.{i}.", False)
         for name in ("up8", "up4", "up2"):
             for j in range(2):
-                block(f"{name}.c{j}.", f"{dl}{name}.convs.{j}.", ("dwconv", "norm", "pwconv1", "pwconv2"))
+                convnext_block(T, sd, f"{name}.c{j}.", f"{dl}{name}.convs.{j}.", ("dwconv", "norm", "pwconv1", "pwconv2"))
             uw = sd[f"{dl}{name}.up.0.weight"]
             T[f"{name}.up_w"], T[f"{name}.up_b"] = h16(uw.reshape(uw.shape[0], uw.shape[1])), c32(sd[f"{dl}{name}.up.0.bias"])
             cw = sd[f"{dl}{name}.up.2.weight"]
@@ -319,23 +214,16 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         return cfg
 
     def _get_engine(self):
-        """The engine of the current network shape.  A new shape makes a new engine with the packed weights and the
-        shape's own operands; the previous engine, its workspaces and its graphs are dropped only once the new one has
-        passed a dry run, which names any bound the shape breaks before anything is launched."""
-        T, _ = self._weights()
+        """The engine of the current network shape.  A new engine passes a dry run before it replaces the previous one,
+        which names any bound the shape breaks before anything is launched."""
         shape = self._network_shape()
-        if self._engine is not None and self._engine_key == shape:
-            return self._engine
-        ops = self._shape_operands(shape, self.device)
 
         def check(handle):
             lib = cabi.lib()
             if lib.udb_v1_workspace_bytes(handle, 1, *shape) == 0:
                 raise NotImplementedError(f"UniDepthV1.image_shape {list(shape)}: {lib.udb_last_error().decode()}")
 
-        handle = self._create_engine(self._engine_config(), shape, tensors={**T, **ops}, check=check)
-        self._shape_ops = ops              # the engine borrows their pointers
-        return handle
+        return self._shape_engine(shape, self._engine_config(), check)
 
     def _forward_engine(self, rgb: torch.Tensor, K: Optional[torch.Tensor], skip_camera: bool, scale255: bool, normalize: bool):
         eng = self._get_engine()
@@ -365,29 +253,9 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         if intrinsics is not None and intrinsics.ndim == 2:
             intrinsics = intrinsics.unsqueeze(0)
         shape = self._network_shape()
-        dev = self.device
-        if dev.type != "cuda":
-            raise RuntimeError("unidepth_b200 has no CPU path: move the model to a CUDA device")
+        dev = self._cuda_device()
         with torch.cuda.device(dev):
-            rgbs = rgbs.to(dev)
-            B = rgbs.shape[0]
-            # unidepthv1.py:301-308: "/255" when the data looks like 0..255, ImageNet normalisation when it then lies in [0, 1]
-            if rgbs.dtype == torch.uint8:
-                scale255, normalize = True, True
-            else:
-                rgbs = rgbs.float()
-                mx, mn = float(rgbs.max()), float(rgbs.min())
-                scale255 = mx > 5
-                if scale255:
-                    mx, mn = mx / 255.0, mn / 255.0
-                normalize = mn >= 0.0 and mx <= 1.0
-            rgbs = rgbs.contiguous()
-            K = None
-            if intrinsics is not None:
-                K = intrinsics.to(dev, f32).reshape(-1, 3, 3)
-                if K.shape[0] != B:
-                    raise ValueError(f"intrinsics holds {K.shape[0]} matrices for a batch of {B} images")
-                K = K.contiguous()
+            rgbs, K, scale255, normalize = infer_inputs(rgbs, intrinsics, dev)
             self._get_engine()
             run = lambda x, inputs: self._forward_engine(x, inputs.get("K"), skip_camera, scale255, normalize)
             key = (shape, tuple(rgbs.shape), rgbs.dtype, scale255, normalize, K is not None, bool(skip_camera))

@@ -25,87 +25,11 @@ from typing import Dict, Optional
 import torch
 
 from . import _cabi as cabi
-from ._engine_model import HUB_KWARGS, EngineModel, PyTorchModelHubMixin, f16, f32
+from ._engine_model import HUB_KWARGS, EngineModel, PyTorchModelHubMixin, f32
+from ._pack import c32, h16, pack_vit_encoder
+from ._pack import pack_e4m3  # noqa: F401  -- the fp8 weight quantiser stays importable from here, where callers import it
 from .camera import pack_camera
 from .spec import ModelSpec, PATCH, get_paddings, get_resize_factor, param_shapes, pixel_bounds
-
-
-def pack_e4m3(w: torch.Tensor):
-    """A GEMM weight [N, K] as FP8 E4M3 with one f32 scale per output channel: (w8, s) with s = amax / 448 (1 for an
-    all-zero row) and w8 = e4m3(w * (448 / amax)), rounded to nearest even; w ~= w8 * s.  The same arithmetic as the
-    engine's activation quantisers (include/udb.h udb_quantize_rows_e4m3)."""
-    w = w.to(f32)
-    amax = w.abs().amax(dim=1)
-    nz = amax > 0
-    one = torch.ones_like(amax)
-    # a tensor division (correctly rounded, as on the device): `448.0 / amax` would be computed as amax.reciprocal() * 448
-    inv = torch.where(nz, torch.full_like(amax, 448.0) / torch.where(nz, amax, one), one)
-    s = torch.where(nz, amax / 448.0, one)
-    return (w * inv[:, None]).to(torch.float8_e4m3fn).contiguous(), s.contiguous()
-
-
-def pack_vit_encoder(sd: dict, d: int, depth: int, dev, split: bool = False, fuse: bool = False,
-                     pe: str = "pixel_encoder.", fp8: bool = False) -> Dict[str, torch.Tensor]:
-    """Operands of the DINOv2 encoder (patch embedding, cls token, position grid, `depth` blocks) from the reference
-    state dict `sd`, under their engine names (`patch_w`, `cls`, `pos`, `blocks.{i}.qkv_w`, ...) and in the layouts the
-    engines' shared block loop reads (engine_common.h `vit_blocks`).  UniDepthV2 packs every mode through it; UniDepthV1
-    (ViT-L/14) uses the default f16 mode.  The position grid is returned as stored ([1 + 37*37, d]); how it is resized
-    to the patch grid differs between the two models.  `fp8`: the blocks' four linear layers are packed as e4m3 weights
-    with per-output-channel scales (`blocks.{i}.qkv_w8`, `qkv_w8s`, ...; `pack_e4m3`)."""
-    h16 = lambda t: t.to(f16).contiguous()
-    c32 = lambda t: t.to(f32).contiguous()
-
-    def enc16(w):
-        """Encoder GEMM weight [N, K]: f16, or in split mode [N, 3K] = [hi | hi | lo] with w ~= hi + lo."""
-        w = w.to(f32)
-        hi = w.to(f16)
-        if not split:
-            return hi.contiguous()
-        lo = (w - hi.to(f32)).to(f16)
-        return torch.cat([hi, hi, lo], dim=1).contiguous()
-
-    def ln_fold(w, b, lnw, lnb):
-        """LayerNorm folded into the Linear that follows it:  LN(x) W^T + b = rstd (x W'^T - mean c1) + c2  with
-        W' = W diag(ln_w) (f16, what the MMA multiplies), c1 = row sums of the ROUNDED W', c2 = W ln_b + b."""
-        w, b, lnw, lnb = w.float(), b.float(), lnw.float(), lnb.float()
-        wf = (w * lnw.unsqueeze(0)).to(f16)
-        return wf.contiguous(), wf.float().sum(dim=1).contiguous(), (w @ lnb + b).contiguous()
-
-    T: Dict[str, torch.Tensor] = {}
-    wpe = torch.zeros((d, 640), device=dev, dtype=f32)
-    wpe[:, :588] = sd[pe + "patch_embed.proj.weight"].reshape(d, 588).to(f32)
-    T["patch_w"], T["patch_b"] = enc16(wpe), c32(sd[pe + "patch_embed.proj.bias"])
-    T["cls"] = c32(sd[pe + "cls_token"].reshape(d))
-    T["pos"] = c32(sd[pe + "pos_embed"].reshape(-1, d))
-    for i in range(depth):
-        b = f"{pe}blocks.{i}."
-        if fuse:
-            qw, qc1, qc2 = ln_fold(sd[b + "attn.qkv.weight"], sd[b + "attn.qkv.bias"], sd[b + "norm1.weight"], sd[b + "norm1.bias"])
-            fw, fc1, fc2 = ln_fold(sd[b + "mlp.fc1.weight"], sd[b + "mlp.fc1.bias"], sd[b + "norm2.weight"], sd[b + "norm2.bias"])
-            blk = dict(
-                qkv_wf=qw, qkv_c1=qc1, qkv_c2=qc2, fc1_wf=fw, fc1_c1=fc1, fc1_c2=fc2,
-                proj_w=h16(sd[b + "attn.proj.weight"]), proj_b=c32(sd[b + "attn.proj.bias"]), ls1=c32(sd[b + "ls1.gamma"]),
-                fc2_w=h16(sd[b + "mlp.fc2.weight"]), fc2_b=c32(sd[b + "mlp.fc2.bias"]), ls2=c32(sd[b + "ls2.gamma"]))
-        elif fp8:
-            blk = dict(n1w=c32(sd[b + "norm1.weight"]), n1b=c32(sd[b + "norm1.bias"]), qkv_b=c32(sd[b + "attn.qkv.bias"]),
-                       proj_b=c32(sd[b + "attn.proj.bias"]), ls1=c32(sd[b + "ls1.gamma"]),
-                       n2w=c32(sd[b + "norm2.weight"]), n2b=c32(sd[b + "norm2.bias"]), fc1_b=c32(sd[b + "mlp.fc1.bias"]),
-                       fc2_b=c32(sd[b + "mlp.fc2.bias"]), ls2=c32(sd[b + "ls2.gamma"]))
-            for k, src in (("qkv", "attn.qkv"), ("proj", "attn.proj"), ("fc1", "mlp.fc1"), ("fc2", "mlp.fc2")):
-                blk[k + "_w8"], blk[k + "_w8s"] = pack_e4m3(sd[b + src + ".weight"])
-        else:
-            blk = dict(
-                n1w=c32(sd[b + "norm1.weight"]), n1b=c32(sd[b + "norm1.bias"]),
-                qkv_w=enc16(sd[b + "attn.qkv.weight"]), qkv_b=c32(sd[b + "attn.qkv.bias"]),
-                proj_w=enc16(sd[b + "attn.proj.weight"]), proj_b=c32(sd[b + "attn.proj.bias"]),
-                ls1=c32(sd[b + "ls1.gamma"]),
-                n2w=c32(sd[b + "norm2.weight"]), n2b=c32(sd[b + "norm2.bias"]),
-                fc1_w=enc16(sd[b + "mlp.fc1.weight"]), fc1_b=c32(sd[b + "mlp.fc1.bias"]),
-                fc2_w=enc16(sd[b + "mlp.fc2.weight"]), fc2_b=c32(sd[b + "mlp.fc2.bias"]),
-                ls2=c32(sd[b + "ls2.gamma"]))
-        for k, v in blk.items():
-            T[f"blocks.{i}.{k}"] = v
-    return T
 
 
 class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
@@ -157,8 +81,6 @@ class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
             raise NotImplementedError(f"pixel_decoder.kernel_size={s.kernel_size}: the residual conv units run as 3x3 "
                                       "convolutions (every shipped UniDepthV2 config sets 3)")
         sd = {k: v.detach() for k, v in self.state_dict().items()}
-        h16 = lambda t: t.to(f16).contiguous()
-        c32 = lambda t: t.to(f32).contiguous()
         if self.precision not in ("f16", "split", "fp8"):
             raise ValueError(f"precision must be 'f16', 'split' or 'fp8', not {self.precision!r}")
         split, fp8 = self.precision == "split", self.precision == "fp8"
@@ -184,6 +106,7 @@ class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
             raise NotImplementedError(f"high-resolution feature width {c_hr_real} not supported")
         pe = "pixel_encoder."
         T = pack_vit_encoder(sd, d, s.depth, dev, split, fuse, fp8=fp8)
+        T["pos"] = c32(sd[pe + "pos_embed"].reshape(-1, d))      # the stored grid: the engine resizes it per shape
         S: Dict[str, float] = {"precision": 1.0 if split else (2.0 if fp8 else 0.0), "fuse_ln": 1.0 if fuse else 0.0}
         T["norm_w"], T["norm_b"] = c32(sd[pe + "norm.weight"]), c32(sd[pe + "norm.bias"])
 
@@ -486,10 +409,7 @@ class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         return self.forward_test(inputs, image_metas)
 
     def _to_device_input(self, rgb):
-        dev = self.device
-        if dev.type != "cuda":
-            raise RuntimeError("unidepth_b200 has no CPU path: move the model to a CUDA device")
-        rgb = rgb.to(dev)
+        rgb = rgb.to(self._cuda_device())
         if rgb.dtype not in (torch.uint8, f32):
             rgb = rgb.float()
         return rgb.contiguous()

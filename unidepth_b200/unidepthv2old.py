@@ -28,16 +28,13 @@ import math
 from typing import Dict, Optional, Tuple
 
 import torch
-import torch.nn.functional as F
 
 from . import _cabi as cabi
-from ._engine_model import HUB_KWARGS, EngineModel, PyTorchModelHubMixin, f16, f32
+from ._engine_model import HUB_KWARGS, EngineModel, PyTorchModelHubMixin, f32, infer_inputs
+from ._pack import (adapter, attn_block, c32, convnext_block, cross_block, h16, latents, mlp, pack_vit_encoder,
+                    pos_table_by_size, tokens_pos)
 from .spec import PATCH
 from .spec_v2old import RAY_K, V2oldSpec, check_ratio, check_resolution, param_shapes
-from .unidepthv1 import _sine_position_embedding
-from .unidepthv2 import pack_vit_encoder
-
-INTERPOLATION_MODES = {"bilinear": 0, "nearest-exact": 1}     # include/udb.h UDB_V2OLD_*
 
 
 def v2old_geometry(H: int, W: int, level: int, pixels_bounds) -> Tuple[Tuple[int, int], float]:
@@ -83,32 +80,20 @@ class UniDepthV2old(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         (positional_embedding.py:230-233), computed on the CPU as the reference computes them."""
         s = self.spec
         sd = self.state_dict()
-        pd = "pixel_decoder."
-        hid, D = s.hidden, s.embed_dim
         gh, gw = shape[0] // PATCH, shape[1] // PATCH
-        c32 = lambda t: t.to(dev, f32).contiguous()
+        to_dev = lambda t: t.to(dev, f32).contiguous()
         T: Dict[str, torch.Tensor] = {}
-        pos = sd["pixel_encoder.pos_embed"].detach().float().reshape(-1, D)
-        M = math.isqrt(pos.shape[0] - 1)
-        grid = pos[1:].reshape(1, M, M, D).permute(0, 3, 1, 2)
-        g = F.interpolate(grid, size=(gh, gw), mode="bicubic", antialias=False)
-        T["pos"] = c32(torch.cat([pos[:1], g.permute(0, 2, 3, 1).reshape(gh * gw, D)], dim=0))
-        le = F.linear(F.gelu(F.linear(sd[pd + "level_embeds"].float(), sd[pd + "level_embed_layer.0.weight"].float(),
-                                      sd[pd + "level_embed_layer.0.bias"].float())),
-                      sd[pd + "level_embed_layer.2.weight"].float(), sd[pd + "level_embed_layer.2.bias"].float())
-        le = F.layer_norm(le, (hid,), sd[pd + "level_embed_layer.3.weight"].float(), sd[pd + "level_embed_layer.3.bias"].float(), 1e-5)
-        sine = _sine_position_embedding(gh, gw, hid // 2, le.device)
-        T["tokens_pos"] = c32((sine[None, :, :] + le[:, None, :]).reshape(4 * gh * gw, hid))
+        pos = sd["pixel_encoder.pos_embed"].detach().float().reshape(-1, s.embed_dim)
+        T["pos"] = to_dev(pos_table_by_size(pos, gh, gw))
+        T["tokens_pos"] = tokens_pos(sd, gh, gw, s.hidden, dev)
         for i in range(3):
             mf = max(gh << i, gw << i) // 2
-            T[f"ray_scales.{i}"] = c32(2.0 ** torch.linspace(0.0, math.log2(mf), steps=32, dtype=f32))
+            T[f"ray_scales.{i}"] = to_dev(2.0 ** torch.linspace(0.0, math.log2(mf), steps=32, dtype=f32))
         return T
 
     def _pack_weights(self, dev):
         s = self.spec
         sd = {k: v.detach() for k, v in self.state_dict().items()}
-        h16 = lambda t: t.to(dev, f16).contiguous()
-        c32 = lambda t: t.to(dev, f32).contiguous()
         T: Dict[str, torch.Tensor] = {}
         S: Dict[str, float] = {}
         pd, dl = "pixel_decoder.", "pixel_decoder.depth_layer."
@@ -119,99 +104,50 @@ class UniDepthV2old(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
             out[:, :w.shape[1]] = w.float()
             return out
 
-        # ---- encoder: the shared DINOv2 packing; its "pos" is the checkpoint's grid, which the shape's table replaces
-        T.update({k: v.to(dev) for k, v in pack_vit_encoder(sd, D, s.enc_depth, dev).items()})
-        del T["pos"]
+        # ---- encoder: the shared DINOv2 packing; the position table is a shape operand
+        T.update(pack_vit_encoder(sd, D, s.enc_depth, dev))
         T["norm_w"], T["norm_b"] = c32(sd["pixel_encoder.norm.weight"]), c32(sd["pixel_encoder.norm.bias"])
 
         # ---- adapters
         for l in range(4):
-            a = f"{pd}input_adapter.input_adapters.{l}"
-            T[f"adapt.{l}.ln_w"], T[f"adapt.{l}.ln_b"] = c32(sd[a + ".0.weight"]), c32(sd[a + ".0.bias"])
-            T[f"adapt.{l}.w"], T[f"adapt.{l}.b"] = h16(sd[a + ".1.weight"]), c32(sd[a + ".1.bias"])
+            adapter(T, sd, f"adapt.{l}.", f"{pd}input_adapter.input_adapters.{l}.", h16)
         for dst, src, n in (("ctok", "camera_token_adapter", 4), ("gtok", "global_token_adapter", 2)):
             for i in range(n):
-                a = f"{pd}{src}.input_adapters.{i}"
-                T[f"{dst}.{i}.ln_w"], T[f"{dst}.{i}.ln_b"] = c32(sd[a + ".0.weight"]), c32(sd[a + ".0.bias"])
-                T[f"{dst}.{i}.w"], T[f"{dst}.{i}.b"] = c32(sd[a + ".1.weight"]), c32(sd[a + ".1.bias"])
-
-        def mlp32(dst, src):
-            T[dst + ".nw"], T[dst + ".nb"] = c32(sd[src + ".norm.weight"]), c32(sd[src + ".norm.bias"])
-            T[dst + ".w1"], T[dst + ".b1"] = c32(sd[src + ".proj1.weight"]), c32(sd[src + ".proj1.bias"])
-            T[dst + ".w2"], T[dst + ".b2"] = c32(sd[src + ".proj2.weight"]), c32(sd[src + ".proj2.bias"])
-
-        def cross_block(dst, src):
-            """a single-head AttentionBlock of the camera / global head: f32 operands of the CUDA-core path, the (k | v)
-            weight f16 for the GEMM over the long context"""
-            for a, b in (("nxw", "norm_attnx.weight"), ("nxb", "norm_attnx.bias"), ("ncw", "norm_attnctx.weight"),
-                         ("ncb", "norm_attnctx.bias"), ("q_w", "q.weight"), ("q_b", "q.bias"), ("kv_b", "kv.bias"),
-                         ("out_w", "out.weight"), ("out_b", "out.bias"), ("ls1", "ls1.gamma"), ("ls2", "ls2.gamma")):
-                T[dst + a] = c32(sd[src + b])
-            T[dst + "kv_w"] = h16(sd[src + "kv.weight"])
-            mlp32(dst + "mlp", src + "mlp")
+                adapter(T, sd, f"{dst}.{i}.", f"{pd}{src}.input_adapters.{i}.", c32)
 
         # ---- camera head
         cl = pd + "camera_layer."
-        mlp32("cam.cls", cl + "project_cls")
-        T["cam.inf.nw"], T["cam.inf.nb"] = c32(sd[cl + "in_features.norm.weight"]), c32(sd[cl + "in_features.norm.bias"])
-        T["cam.inf.w1"], T["cam.inf.b1"] = h16(sd[cl + "in_features.proj1.weight"]), c32(sd[cl + "in_features.proj1.bias"])
-        T["cam.inf.w2"], T["cam.inf.b2"] = h16(sd[cl + "in_features.proj2.weight"]), c32(sd[cl + "in_features.proj2.bias"])
+        mlp(T, sd, "cam.cls", cl + "project_cls", c32)
+        mlp(T, sd, "cam.inf", cl + "in_features", h16)
         T["cam.pos"] = c32(sd[cl + "latents_pos"].reshape(4, hid))
-        cross_block("cam.agg1.", cl + "aggregate1.")
-        cross_block("cam.agg2.", cl + "aggregate2.")
-        mlp32("cam.out", cl + "out")
+        cross_block(T, sd, "cam.agg1.", cl + "aggregate1.", h16)
+        cross_block(T, sd, "cam.agg2.", cl + "aggregate2.", h16)
+        mlp(T, sd, "cam.out", cl + "out", c32)
 
         # ---- global head
         gl = pd + "global_layer."
-        mlp32("glob.cls", gl + "project_cls")
+        mlp(T, sd, "glob.cls", gl + "project_cls", c32)
         T["glob.rays_w"], T["glob.rays_b"] = h16(kpad(sd[gl + "project_rays.weight"], RAY_K)), c32(sd[gl + "project_rays.bias"])
         T["glob.in_w"], T["glob.in_b"] = h16(sd[gl + "in_features.weight"]), c32(sd[gl + "in_features.bias"])
-        cross_block("glob.agg1.", gl + "aggregate1.")
-        cross_block("glob.agg2.", gl + "aggregate2.")
-        mlp32("glob.out", gl + "out")
+        cross_block(T, sd, "glob.agg1.", gl + "aggregate1.", h16)
+        cross_block(T, sd, "glob.agg2.", gl + "aggregate2.", h16)
+        mlp(T, sd, "glob.out", gl + "out", c32)
 
         # ---- depth head
         for i in range(3):
             T[f"rays.{i}.w"], T[f"rays.{i}.b"] = h16(kpad(sd[f"{dl}rays_layers.{i}.weight"], RAY_K)), c32(sd[f"{dl}rays_layers.{i}.bias"])
-        T["fcc_w"], T["fcc_b"] = h16(sd[dl + "features_channel_cat.weight"]), c32(sd[dl + "features_channel_cat.bias"])
-        T["lat.nw"], T["lat.nb"] = c32(sd[dl + "to_latents.norm.weight"]), c32(sd[dl + "to_latents.norm.bias"])
-        T["lat.w1"], T["lat.b1"] = h16(sd[dl + "to_latents.proj1.weight"]), c32(sd[dl + "to_latents.proj1.bias"])
-        T["lat.w2"], T["lat.b2"] = h16(sd[dl + "to_latents.proj2.weight"]), c32(sd[dl + "to_latents.proj2.bias"])
-
-        def attn_block(dst, src, split_kv):
-            """V1's packing of the decoder's AttentionBlock / NystromBlock (engine_common.h dense_attn_block, mh_attn_block)"""
-            for a, b in (("nxw", "norm_attnx.weight"), ("nxb", "norm_attnx.bias"), ("ncw", "norm_attnctx.weight"),
-                         ("ncb", "norm_attnctx.bias"), ("q_b", "q.bias"), ("out_b", "out.bias"), ("ls1", "ls1.gamma"),
-                         ("ls2", "ls2.gamma"), ("mnw", "mlp.norm.weight"), ("mnb", "mlp.norm.bias"), ("mb1", "mlp.proj1.bias"),
-                         ("mb2", "mlp.proj2.bias")):
-                T[dst + a] = c32(sd[src + b])
-            for a, b in (("q_w", "q.weight"), ("out_w", "out.weight"), ("mw1", "mlp.proj1.weight"), ("mw2", "mlp.proj2.weight")):
-                T[dst + a] = h16(sd[src + b])
-            kvw, kvb = sd[src + "kv.weight"], sd[src + "kv.bias"]
-            d = kvw.shape[1]
-            if split_kv:
-                T[dst + "k_w"], T[dst + "k_b"] = h16(kvw[:d]), c32(kvb[:d])
-                T[dst + "v_w"], T[dst + "v_b"] = h16(kvw[d:]), c32(kvb[d:])
-            else:
-                T[dst + "kv_w"], T[dst + "kv_b"] = h16(kvw), c32(kvb)
-
-        attn_block("agg16.", dl + "aggregate_16.", True)
-        attn_block("prompt.", dl + "prompt_camera.", True)
+        latents(T, sd, dl)
+        attn_block(T, sd, "agg16.", dl + "aggregate_16.", True)
+        attn_block(T, sd, "prompt.", dl + "prompt_camera.", True)
         for j in range(s.dec_depths[0]):
-            attn_block(f"nys.{j}.", f"{dl}process_layers.0.{j}.", False)
+            attn_block(T, sd, f"nys.{j}.", f"{dl}process_layers.0.{j}.", False)
         for i in range(3):
             c = hid >> i
             cq, c2 = c // 4, c // 2
             cqp = -(-cq // 64) * 64
             u, dst = f"{dl}ups.{i}.", f"up.{i}."
             for j in range(2):
-                b = f"{u}convs.{j}."
-                w = sd[b + "dwconv.weight"]
-                T[f"{dst}c{j}.dw_w"], T[f"{dst}c{j}.dw_b"] = c32(w.reshape(c, 49).t()), c32(sd[b + "dwconv.bias"])
-                T[f"{dst}c{j}.ln_w"], T[f"{dst}c{j}.ln_b"] = c32(sd[b + "norm.weight"]), c32(sd[b + "norm.bias"])
-                T[f"{dst}c{j}.w1"], T[f"{dst}c{j}.b1"] = h16(sd[b + "pwconv1.weight"]), c32(sd[b + "pwconv1.bias"])
-                T[f"{dst}c{j}.w2"], T[f"{dst}c{j}.b2"] = h16(sd[b + "pwconv2.weight"]), c32(sd[b + "pwconv2.bias"])
-                T[f"{dst}c{j}.gamma"] = c32(sd[b + "gamma"])
+                convnext_block(T, sd, f"{dst}c{j}.", f"{u}convs.{j}.", ("dwconv", "norm", "pwconv1", "pwconv2"))
             T[dst + "dw_w"], T[dst + "dw_b"] = c32(sd[u + "up.1.weight"].reshape(cq, 49).t()), c32(sd[u + "up.1.bias"])
             cw = torch.zeros((c2, 3, 3, cqp), dtype=f32, device=sd[u + "up.3.weight"].device)
             cw[..., :cq] = sd[u + "up.3.weight"].float().permute(0, 2, 3, 1)         # [C/2, C/4, 3, 3] -> [C/2, (ky, kx, ci)]
@@ -245,17 +181,6 @@ class UniDepthV2old(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         cfg.net_h, cfg.net_w = shape
         return cfg
 
-    def _get_engine(self, shape: Tuple[int, int]):
-        """The engine of the network shape `shape`; a new shape makes a new engine with the packed weights and the shape's
-        own operands, and drops the previous one with its workspaces and graphs."""
-        T, _ = self._weights()
-        if self._engine is not None and self._engine_key == shape:
-            return self._engine
-        ops = self._shape_operands(shape, self.device)
-        handle = self._create_engine(self._engine_config(shape), shape, tensors={**T, **ops})
-        self._shape_ops = ops              # the engine borrows their pointers
-        return handle
-
     def _forward_engine(self, rgb: torch.Tensor, K: Optional[torch.Tensor], scale255: bool, normalize: bool, mode: int):
         eng = self._engine
         lib = cabi.lib()
@@ -281,41 +206,22 @@ class UniDepthV2old(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
     @torch.no_grad()
     def infer(self, rgbs: torch.Tensor, intrinsics=None):
         """Same contract as the reference `UniDepthV2old.infer` (unidepthv2_old.py:198-282)."""
-        if self.interpolation_mode not in INTERPOLATION_MODES:
+        if self.interpolation_mode not in cabi.V2OLD_INTERP_MODES:
             raise NotImplementedError(f"interpolation_mode {self.interpolation_mode!r}: only 'bilinear' and 'nearest-exact' "
                                       "are implemented")
-        mode = INTERPOLATION_MODES[self.interpolation_mode]
+        mode = cabi.V2OLD_INTERP_MODES[self.interpolation_mode]
         if rgbs.ndim == 3:
             rgbs = rgbs.unsqueeze(0)
         if intrinsics is not None and intrinsics.ndim == 2:
             intrinsics = intrinsics.unsqueeze(0)
-        dev = self.device
-        if dev.type != "cuda":
-            raise RuntimeError("unidepth_b200 has no CPU path: move the model to a CUDA device")
+        dev = self._cuda_device()
         B, _, H, W = rgbs.shape
         level = check_resolution(self.resolution_level)
         check_ratio((H, W), self.shape_constraints["ratio_bounds"])
         shape, _ = v2old_geometry(H, W, level, self.shape_constraints["pixels_bounds_ori"])
         with torch.cuda.device(dev):
-            rgbs = rgbs.to(dev)
-            # unidepthv2_old.py:211-218: "/255" when the data looks like 0..255, ImageNet normalisation when it then lies in [0, 1]
-            if rgbs.dtype == torch.uint8:
-                scale255, normalize = True, True
-            else:
-                rgbs = rgbs.float()
-                mx, mn = float(rgbs.max()), float(rgbs.min())
-                scale255 = mx > 5
-                if scale255:
-                    mx, mn = mx / 255.0, mn / 255.0
-                normalize = mn >= 0.0 and mx <= 1.0
-            rgbs = rgbs.contiguous()
-            K = None
-            if intrinsics is not None:
-                K = intrinsics.to(dev, f32).reshape(-1, 3, 3)
-                if K.shape[0] != B:
-                    raise ValueError(f"intrinsics holds {K.shape[0]} matrices for a batch of {B} images")
-                K = K.contiguous()
-            self._get_engine(shape)
+            rgbs, K, scale255, normalize = infer_inputs(rgbs, intrinsics, dev)
+            self._shape_engine(shape, self._engine_config(shape))
             run = lambda x, inputs: self._forward_engine(x, inputs.get("K"), scale255, normalize, mode)
             key = (shape, tuple(rgbs.shape), rgbs.dtype, scale255, normalize, K is not None, mode)
             return self._run_graphed(run, rgbs, {} if K is None else {"K": K}, key)
