@@ -336,7 +336,10 @@ typedef struct udb_ray_embed_t {
 int udb_ray_embed(const udb_ray_embed_t* p, void* stream);
 /* The same resampled unit rays as UniDepthV2old's ray features (decoder_old.py:111-121, positional_embedding.py:218-256
  * with use_log and cat_orig): sin(pi * scales[k] * axis) for the three axes of the ray (axis-major, 3*bands features),
- * then the ray itself, zero-filled up to the row stride ld_out >= 3*bands + 3 */
+ * then the ray itself, zero-filled up to the row stride ld_out >= 3*bands + 3.
+ * out_f32 = 2: split-f16 rows in the udb_gemm_t.a_split_k layout [hi | lo] of ld_out / 2 features each, hi = f16(y)
+ * (what out_f32 = 0 stores) and lo = f16(y - f32(hi)), both halves zero past the 3*bands + 3 features; ld_out must be
+ * even and ld_out / 2 >= 3*bands + 3. */
 int udb_ray_embed_cat_orig(const udb_ray_embed_t* p, int32_t ld_out, void* stream);
 
 /* x2 bilinear up-sample, align_corners=False (layers/upsample.py:215), NHWC f16 -> f16.

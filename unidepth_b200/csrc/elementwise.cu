@@ -466,15 +466,26 @@ __global__ void __launch_bounds__(256) ray_embed_kernel(const udb_ray_embed_t p,
   ax /= nrm; ay /= nrm; az /= nrm;
   if (ld_cat) {
     // UniDepthV2old (decoder_old.py:111-121 / 237-247, positional_embedding.py:218-256 with use_log, cat_orig): sin of each
-    // axis of the unit ray times the `bands` frequencies and pi (axis-major), then the ray itself, zero up to `ld_cat`
+    // axis of the unit ray times the `bands` frequencies and pi (axis-major), then the ray itself, zero up to `ld_cat`.
+    // out_f32 == 2: split-f16 rows [hi | lo] of ld_cat / 2 features each, hi = f16(v), lo = f16(v - f32(hi))
     const float r3[3] = {ax, ay, az};
     const float pi = 3.14159265358979323846f;
-    for (int f = lane; f < ld_cat; f += 32) {
+    const bool split = p.out_f32 == 2;
+    const int nf = split ? ld_cat / 2 : ld_cat;
+    for (int f = lane; f < nf; f += 32) {
       float v = 0.f;
       if (f < 3 * p.bands) v = sinf(r3[f / p.bands] * __ldg(p.scales + (f % p.bands)) * pi);
       else if (f < 3 * p.bands + 3) v = r3[f - 3 * p.bands];
-      if (p.out_f32) reinterpret_cast<float*>(p.out)[(long long)tok * ld_cat + f] = v;
-      else reinterpret_cast<__half*>(p.out)[(long long)tok * ld_cat + f] = __float2half_rn(v);
+      const long long o = (long long)tok * ld_cat + f;
+      if (split) {
+        const __half hi = __float2half_rn(v);
+        reinterpret_cast<__half*>(p.out)[o] = hi;
+        reinterpret_cast<__half*>(p.out)[o + nf] = __float2half_rn(v - __half2float(hi));
+      } else if (p.out_f32) {
+        reinterpret_cast<float*>(p.out)[o] = v;
+      } else {
+        reinterpret_cast<__half*>(p.out)[o] = __float2half_rn(v);
+      }
     }
     return;
   }
@@ -911,12 +922,17 @@ extern "C" int udb_ray_embed_cat_orig(const udb_ray_embed_t* p, int32_t ld_out, 
     set_error("udb_ray_embed_cat_orig: needs bands >= 1 and ld_out >= 3*bands + 3 (bands=%d ld_out=%d)", p->bands, ld_out);
     return 1;
   }
+  if (p->out_f32 == 2 && (ld_out % 2 || ld_out / 2 < 3 * p->bands + 3)) {
+    set_error("udb_ray_embed_cat_orig: split output needs an even ld_out >= 2*(3*bands + 3) to hold both halves (bands=%d ld_out=%d)",
+              p->bands, ld_out);
+    return 1;
+  }
   if (p->B < 1 || p->gh < 1 || p->gw < 1 || p->net_h < 1 || p->net_w < 1) {
     set_error("udb_ray_embed_cat_orig: B=%d gh=%d gw=%d net_h=%d net_w=%d must all be >= 1", p->B, p->gh, p->gw, p->net_h, p->net_w);
     return 1;
   }
   const int toks = p->B * p->gh * p->gw;
-  note_work(0.0, (double)toks * ld_out * (p->out_f32 ? 4 : 2));
+  note_work(0.0, (double)toks * ld_out * (p->out_f32 == 1 ? 4 : 2));
   ray_embed_kernel<<<(toks + 7) / 8, 256, 0, ST(stream)>>>(*p, ld_out);
   return check_launch("ray_embed_cat_orig_kernel");
 }

@@ -152,6 +152,17 @@ struct Ctx {
     }
   }
 
+  // registered 1-D operand (a per-channel scale or bias vector) must have exactly n entries
+  void expect1(const std::string& name, int64_t n) {
+    const Weight* w = W(name);
+    if (rc) return;
+    if (w->ndim != 1 || w->shape[0] != n) {
+      set_error("engine: packed tensor '%s' has shape [%lld] (ndim %d), expected [%lld]", name.c_str(), (long long)w->shape[0],
+                w->ndim, (long long)n);
+      rc = 1;
+    }
+  }
+
   // registered operand must hold e4m3 bytes (f16 bytes would be read as e4m3 pairs)
   void expect_e4m3(const std::string& name) {
     const Weight* w = W(name);
@@ -462,6 +473,10 @@ static inline void vit_block_e4m3(Ctx& c, const std::string& b, float* x, const 
   c.expect2(b + "fc1_w8", 4 * D, D);
   c.expect2(b + "fc2_w8", D, 4 * D);
   for (const char* n : {"qkv_w8", "proj_w8", "fc1_w8", "fc2_w8"}) c.expect_e4m3(b + n);
+  c.expect1(b + "qkv_w8s", 3 * D);
+  c.expect1(b + "proj_w8s", D);
+  c.expect1(b + "fc1_w8s", 4 * D);
+  c.expect1(b + "fc2_w8s", D);
   c.layernorm_e4m3(x, q8, qs, c.F(b + "n1w"), c.F(b + "n1b"), BT, D, 1e-6f);
   { Ctx::G q{q8, c.W(b + "qkv_w8")->p, BT, 3 * D, D}; q.a_scale = qs; q.w_scale = c.F(b + "qkv_w8s");
     q.bias = c.F(b + "qkv_b"); q.out = qkv; c.gemm(q); }

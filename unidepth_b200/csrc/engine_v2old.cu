@@ -34,8 +34,10 @@ static udb_v2old_geometry_t v2old_geometry(int H, int W, int level, int lo, int 
 
 // AttentionBlock with one head over a long f16 context and at most four queries (decoder_old.py:72-77, 142-143): the camera
 // head's and the global head's aggregate blocks, on V1's split-key cross attention.  x f32 [B*nq, hid] -> new f32 rows.
+// Split mode (`sp`): the context is f32, its LayerNorm writes a split operand for the kv GEMM ([2*hid, 3*hid] weight), and
+// the attention reads f32 (k | v) rows, as V1's split camera head.
 static float* small_cross_block(Ctx& c, const std::string& p, const float* x, int B, int nq, const void* ctx, long long nk,
-                                const float* q_pos, int hid, int expansion) {
+                                const float* q_pos, int hid, int expansion, bool sp) {
   Arena& ar = *c.ar;
   const int R = B * nq;
   const long long Rc = static_cast<long long>(B) * nk;
@@ -46,17 +48,40 @@ static float* small_cross_block(Ctx& c, const std::string& p, const float* x, in
   c.layernorm(x, 1, xn, 1, c.F(p + "nxw"), c.F(p + "nxb"), R, hid, 1e-5f);
   c.small_linear(xn, R, hid, c.F(p + "q_w"), hid, c.F(p + "q_b"), UDB_ACT_NONE, nullptr, nullptr, q);
   const size_t m = ar.mark();          // the normalised context and its (k | v) rows: dead once the attention has run
-  __half* cn = ar.h(Rc * hid);
-  ln16(c, ctx, 0, cn, p + "ncw", p + "ncb", Rc, hid, 1e-5f);
-  __half* kv = ar.h(Rc * 2 * hid);
-  { Ctx::G g{cn, c.H(p + "kv_w"), static_cast<int>(Rc), 2 * hid, hid}; g.bias = c.F(p + "kv_b"); g.out = kv; c.gemm(g); }
+  void* kv;
+  if (sp) {
+    __half* cn = ar.h(Rc * 2 * hid);
+    c.ln_any(ctx, 1, cn, UDB_LN_OUT_SPLIT, c.F(p + "ncw"), c.F(p + "ncb"), Rc, hid, 1e-5f, 2 * hid);
+    kv = ar.f(Rc * 2 * hid);
+    c.expect2(p + "kv_w", 2 * hid, 3 * hid);
+    Ctx::G g{cn, c.H(p + "kv_w"), static_cast<int>(Rc), 2 * hid, 3 * hid}; g.lda = 2 * hid; g.a_split_k = hid;
+    g.bias = c.F(p + "kv_b"); g.out = kv; g.out_f32 = 1; c.gemm(g);
+  } else {
+    __half* cn = ar.h(Rc * hid);
+    ln16(c, ctx, 0, cn, p + "ncw", p + "ncb", Rc, hid, 1e-5f);
+    kv = ar.h(Rc * 2 * hid);
+    Ctx::G g{cn, c.H(p + "kv_w"), static_cast<int>(Rc), 2 * hid, hid}; g.bias = c.F(p + "kv_b"); g.out = kv; c.gemm(g);
+  }
   c.launch([&] {
-    return udb_cross_attn_small(q, q_pos, kv, at, scratch, B, nq, static_cast<int>(nk), hid, 1.0f / sqrtf(static_cast<float>(hid)), c.st);
+    const float scale = 1.0f / sqrtf(static_cast<float>(hid));
+    return sp ? udb_cross_attn_small_f32(q, q_pos, static_cast<const float*>(kv), at, scratch, B, nq, static_cast<int>(nk), hid, scale, c.st)
+              : udb_cross_attn_small(q, q_pos, kv, at, scratch, B, nq, static_cast<int>(nk), hid, scale, c.st);
   });
   ar.release(m);
   float* t2 = xn;
   c.small_linear(at, R, hid, c.F(p + "out_w"), hid, c.F(p + "out_b"), UDB_ACT_NONE, c.F(p + "ls1"), x, t2);
   return cam_mlp(c, p + "mlp", t2, R, hid, expansion * hid, hid, t2, c.F(p + "ls2"));
+}
+
+// The n head tokens x f32 [B*n, hid] into rows [row0, row0 + n) of each image's nk context rows: f16, or f32 in split mode
+static void copy_cls_rows(Ctx& c, const float* x, void* ctx, int B, int n, int hid, long long nk, long long row0, bool sp) {
+  c.launch([&] {
+    if (!sp) return udb_copy_rows_f32_to_f16(x, ctx, B, n, hid, nk, row0, c.st);
+    const size_t row = sizeof(float) * hid;
+    return cuda_rc(cudaMemcpy2DAsync(static_cast<float*>(ctx) + row0 * hid, nk * row, x, n * row, n * row, B,
+                                     cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(c.st)),
+                   "engine_v2old: copying the head tokens into the f32 context");
+  });
 }
 
 // f32 [R, D] rows of `n` cls tokens -> LN + Linear + GELU per token (ListAdapter, decoder_old.py:13-29) -> f32 [B, n, hid]
@@ -86,42 +111,65 @@ static int run_v2old(udb_engine_v2old* e, const udb_infer_v2old_args_t& a, Arena
     return 1;
   }
   if (cross_attn_small_check("udb_v2old: camera head cross attention", 4, 4 * nq + 4, hid)) return 1;
+  // "precision": 0 (absent) = f16 operands; 2 = e4m3 operands for the encoder blocks' four linear layers (the taps, heads
+  // and decoder as in f16); 1 = split-f16 operands (parity mode): every GEMM on the path from the image to the intrinsics
+  // and to the global (scale, shift) -- patch embedding, encoder blocks, the adapters' copy for the two heads, the camera
+  // head's in_features and kv, the global head's project_rays, in_features and kv -- multiplies [hi | lo] operands with
+  // [hi | hi | lo] weights; the taps and the two heads' contexts are f32.  The depth head reads the hi half of the
+  // adapters' LayerNorm and of the first level's ray features and runs as in the f16 mode.
+  const double prec = e->scalars.count("precision") ? e->scalars["precision"] : 0.0;
+  if (prec != 0.0 && prec != 1.0 && prec != 2.0) { set_error("udb_infer_v2old: precision %g unsupported (0 f16, 1 split f16, 2 e4m3)", prec); return 1; }
+  const bool f8 = prec == 2.0, sp = prec == 1.0;
+  const int sx = sp ? 2 : 1;          // columns of a split operand per logical column
+  const int kx = sp ? 3 : 1;          // columns of a split weight per logical column
+  if (sp) {   // an f16 packing registered with precision 1 is named for what it is, not only by its first mis-shaped operand
+    const Weight* w = c.W("patch_w");
+    if (!c.rc && (w->ndim != 2 || w->shape[1] != 3 * 640)) {
+      set_error("udb_infer_v2old: precision 1 (split f16) needs the split packing: 'patch_w' has %lld columns, expected %d",
+                static_cast<long long>(w->shape[1]), 3 * 640);
+      return 1;
+    }
+  }
   Stage stage;
 
   // ---- pre-processing + patch embedding (unidepthv2_old.py:211-230: /255, ImageNet normalisation, antialiased resize)
   stage.next("udb_v2old:encoder");
-  __half* feats[4];
-  for (int l = 0; l < 4; ++l) feats[l] = ar.h(BN * D);
+  // the four tapped final-norm outputs: f16, or f32 in split mode (the adapters' LayerNorm writes their split operands)
+  void* feats[4];
+  for (int l = 0; l < 4; ++l) feats[l] = ar.alloc(BN * D * (sp ? 4 : 2));
   // normed cls rows of the last three blocks (cls[-3..-1]) and of the third output block (the stacked tokens[-2])
   float* cls[4];
   for (int k = 0; k < 4; ++k) cls[k] = ar.f(static_cast<size_t>(B) * D);
   {
     const size_t m = ar.mark();
-    __half* patches = ar.h(BN * 640);
+    __half* patches = ar.h(BN * 640 * sx);
     {
       udb_v1_preprocess_t p;
       memset(&p, 0, sizeof(p));
       p.rgb = a.rgb; p.rgb_is_u8 = a.rgb_is_u8; p.scale255 = a.scale255; p.normalize = a.normalize; p.B = B; p.H = a.H; p.W = a.W;
       p.rh = net_h; p.rw = net_w; p.net_h = net_h; p.net_w = net_w; p.patches = patches; p.patch = 14;
-      c.launch([&] { return udb_v1_preprocess(&p, st); });
+      c.launch([&] { return sp ? udb_v1_preprocess_split(&p, st) : udb_v1_preprocess(&p, st); });
     }
     float* x = ar.f(BT * D);
-    c.expect2("patch_w", D, 640);
+    c.expect2("patch_w", D, 640 * kx);
     c.expect2("pos", T, D);
     {
       const float* pos = c.F("pos");
       const float* clsw = c.F("cls");
-      Ctx::G q{patches, c.H("patch_w"), static_cast<int>(BN), D, 640};
+      Ctx::G q{patches, c.H("patch_w"), static_cast<int>(BN), D, 640 * kx};
+      q.lda = 640 * sx; q.a_split_k = sp ? 640 : 0;
       q.bias = c.F("patch_b"); q.resid = pos; q.resid_f32 = 1; q.ldr = D; q.out = x; q.out_f32 = 1;
       q.rows_per_group = N; q.group_stride = T; q.row_offset = 1; q.resid_mod = N; q.resid_row_offset = 1;
       c.gemm(q);
       c.launch([&] { return udb_set_cls_rows(x, clsw, pos, B, T, D, st); });
     }
     VitBlocks v{B, T, D, cf.enc_heads, cf.enc_depth};
+    v.fp8 = f8;
+    v.split = sp;
     int tap = 0;
     vit_blocks(c, "blocks.", x, v, [&](int i) {
       if (tap < 4 && i + 1 == cf.output_idx[tap]) {
-        c.layernorm(x, 1, feats[tap], 0, c.F("norm_w"), c.F("norm_b"), static_cast<int>(BN), D, 1e-5f, N, T, 1);
+        c.layernorm(x, 1, feats[tap], sp ? 1 : 0, c.F("norm_w"), c.F("norm_b"), static_cast<int>(BN), D, 1e-5f, N, T, 1);
         ++tap;
       }
       const int from_end = cf.enc_depth - 1 - i;
@@ -135,15 +183,30 @@ static int run_v2old(udb_engine_v2old* e, const udb_infer_v2old_args_t& a, Arena
   stage.next("udb_v2old:adapters");
   __half* featcat = ar.h(Rq * 4 * hid);
   __half* tokens = ar.h((Rq * 4 + 64) * hid);
+  // split mode: the two heads' copy of the tokens from split operands, f32 for the camera head's LayerNorm and as a split
+  // operand for the global head's in_features GEMM (the depth head keeps the f16 tokens)
+  float* head_tokens = sp ? ar.f(Rq * 4 * hid) : nullptr;
+  __half* head_tokens2 = sp ? ar.h(Rq * 4 * 2 * hid) : nullptr;
   for (int l = 0; l < 4; ++l) {
     const size_t m = ar.mark();
     const std::string ad = idx("adapt.%d.", l);
-    __half* an = ar.h(Rq * D);
-    ln16(c, feats[l], 0, an, ad + "ln_w", ad + "ln_b", Rq, D, 1e-5f);
-    { Ctx::G q{an, c.H(ad + "w"), static_cast<int>(Rq), hid, D}; q.bias = c.F(ad + "b"); q.act = UDB_ACT_GELU; q.out = tokens;
+    __half* an = ar.h(Rq * D * sx);
+    if (sp) c.ln_any(feats[l], 1, an, UDB_LN_OUT_SPLIT, c.F(ad + "ln_w"), c.F(ad + "ln_b"), Rq, D, 1e-5f, 2 * D);
+    else ln16(c, feats[l], 0, an, ad + "ln_w", ad + "ln_b", Rq, D, 1e-5f);
+    { Ctx::G q{an, c.H(ad + "w"), static_cast<int>(Rq), hid, D}; q.lda = D * sx; q.bias = c.F(ad + "b"); q.act = UDB_ACT_GELU; q.out = tokens;
       q.rows_per_group = nq; q.group_stride = 4 * nq; q.row_offset = l * nq; c.gemm(q); }
-    { Ctx::G q{an, c.H(ad + "w"), static_cast<int>(Rq), hid, D}; q.bias = c.F(ad + "b"); q.act = UDB_ACT_GELU;
+    { Ctx::G q{an, c.H(ad + "w"), static_cast<int>(Rq), hid, D}; q.lda = D * sx; q.bias = c.F(ad + "b"); q.act = UDB_ACT_GELU;
       q.out = featcat + l * hid; q.ldc = 4 * hid; c.gemm(q); }
+    if (sp) {
+      c.expect2(ad + "w_cam", hid, 3 * D);
+      for (int k = 0; k < 2; ++k) {
+        Ctx::G q{an, c.H(ad + "w_cam"), static_cast<int>(Rq), hid, 3 * D}; q.lda = 2 * D; q.a_split_k = D; q.bias = c.F(ad + "b");
+        q.act = UDB_ACT_GELU; q.rows_per_group = nq; q.group_stride = 4 * nq; q.row_offset = l * nq;
+        if (k == 0) { q.out = head_tokens; q.out_f32 = 1; }
+        else { q.out = head_tokens2; q.ldc = 2 * hid; q.out_split = hid; }
+        c.gemm(q);
+      }
+    }
     ar.release(m);
   }
   const float* tokens_pos = c.F("tokens_pos");         // [4*nq, hid]: sine position + level embedding (decoder_old.py:463-479)
@@ -159,21 +222,32 @@ static int run_v2old(udb_engine_v2old* e, const udb_infer_v2old_args_t& a, Arena
     float* toks = token_adapter(c, "ctok.", cls, 4, B, D, hid);
     float* cl = cam_mlp(c, "cam.cls", toks, R4, hid, 4 * hid, hid, nullptr, nullptr);
     const long long Rc = static_cast<long long>(B) * (4 * nq + 4);
-    __half* ctx = ar.h(Rc * hid);
+    void* ctx = ar.alloc(Rc * hid * (sp ? 4 : 2));            // f16, or f32 in split mode
     {
       const size_t m2 = ar.mark();
-      __half* a1 = ar.h(Rq * 4 * hid);
-      __half* m1 = ar.h(Rq * 4 * 2 * hid);
-      c.ln_any(tokens, 0, a1, 0, c.F("cam.inf.nw"), c.F("cam.inf.nb"), Rq * 4, hid, 1e-5f, 0, tokens_pos, 4LL * nq);
-      { Ctx::G q{a1, c.H("cam.inf.w1"), static_cast<int>(Rq * 4), 2 * hid, hid}; q.bias = c.F("cam.inf.b1"); q.act = UDB_ACT_GELU; q.out = m1; c.gemm(q); }
-      { Ctx::G q{m1, c.H("cam.inf.w2"), static_cast<int>(Rq * 4), hid, 2 * hid}; q.bias = c.F("cam.inf.b2"); q.out = ctx;
-        q.rows_per_group = 4 * nq; q.group_stride = 4 * nq + 4; q.row_offset = 0; c.gemm(q); }
+      __half* a1 = ar.h(Rq * 4 * hid * sx);
+      __half* m1 = ar.h(Rq * 4 * 2 * hid * sx);
+      if (sp) {
+        c.expect2("cam.inf.w1", 2 * hid, 3 * hid);
+        c.expect2("cam.inf.w2", hid, 6 * hid);
+        c.ln_any(head_tokens, 1, a1, UDB_LN_OUT_SPLIT, c.F("cam.inf.nw"), c.F("cam.inf.nb"), Rq * 4, hid, 1e-5f, 2 * hid, tokens_pos, 4LL * nq);
+        { Ctx::G q{a1, c.H("cam.inf.w1"), static_cast<int>(Rq * 4), 2 * hid, 3 * hid}; q.lda = 2 * hid; q.a_split_k = hid;
+          q.bias = c.F("cam.inf.b1"); q.act = UDB_ACT_GELU; q.out = m1; q.ldc = 4 * hid; q.out_split = 2 * hid; c.gemm(q); }
+        { Ctx::G q{m1, c.H("cam.inf.w2"), static_cast<int>(Rq * 4), hid, 6 * hid}; q.lda = 4 * hid; q.a_split_k = 2 * hid;
+          q.bias = c.F("cam.inf.b2"); q.out = ctx; q.out_f32 = 1; q.rows_per_group = 4 * nq; q.group_stride = 4 * nq + 4; q.row_offset = 0;
+          c.gemm(q); }
+      } else {
+        c.ln_any(tokens, 0, a1, 0, c.F("cam.inf.nw"), c.F("cam.inf.nb"), Rq * 4, hid, 1e-5f, 0, tokens_pos, 4LL * nq);
+        { Ctx::G q{a1, c.H("cam.inf.w1"), static_cast<int>(Rq * 4), 2 * hid, hid}; q.bias = c.F("cam.inf.b1"); q.act = UDB_ACT_GELU; q.out = m1; c.gemm(q); }
+        { Ctx::G q{m1, c.H("cam.inf.w2"), static_cast<int>(Rq * 4), hid, 2 * hid}; q.bias = c.F("cam.inf.b2"); q.out = ctx;
+          q.rows_per_group = 4 * nq; q.group_stride = 4 * nq + 4; q.row_offset = 0; c.gemm(q); }
+      }
       ar.release(m2);
     }
-    c.launch([&] { return udb_copy_rows_f32_to_f16(cl, ctx, B, 4, hid, 4LL * nq + 4, 4LL * nq, st); });
+    copy_cls_rows(c, cl, ctx, B, 4, hid, 4LL * nq + 4, 4LL * nq, sp);
     const float* cam_pos = c.F("cam.pos");
-    float* t = small_cross_block(c, "cam.agg1.", cl, B, 4, ctx, 4LL * nq + 4, cam_pos, hid, cf.expansion);
-    t = small_cross_block(c, "cam.agg2.", t, B, 4, ctx, 4LL * nq + 4, cam_pos, hid, cf.expansion);
+    float* t = small_cross_block(c, "cam.agg1.", cl, B, 4, ctx, 4LL * nq + 4, cam_pos, hid, cf.expansion, sp);
+    t = small_cross_block(c, "cam.agg2.", t, B, 4, ctx, 4LL * nq + 4, cam_pos, hid, cf.expansion, sp);
     float* x4 = cam_mlp(c, "cam.out", t, R4, hid, 2 * hid, 1, nullptr, nullptr);     // [B*4, 1] == [B, 4]
     c.launch([&] {
       return udb_v2old_camera(x4, a.intrinsics, B, net_h, net_w, static_cast<float>(ratio), intr4, a.out_intrinsics, k4_points, st);
@@ -183,15 +257,20 @@ static int run_v2old(udb_engine_v2old* e, const udb_infer_v2old_args_t& a, Arena
 
   // ---- ray features at the three decoder grids (GlobalHead / DepthHead.embed_rays, decoder_old.py:111-121,237-255)
   stage.next("udb_v2old:ray_features");
+  // split mode: the first level, which the global head reads, as [hi | lo] rows; the depth head reads its hi half
   __half* rayf[3];
+  int ray_ld[3];
   for (int s = 0; s < 3; ++s) {
     const int lh = gh << s, lw = gw << s;
-    rayf[s] = ar.h(static_cast<size_t>(B) * lh * lw * RAY_K);
+    const bool split_rays = sp && s == 0;
+    ray_ld[s] = split_rays ? 2 * RAY_K : RAY_K;
+    rayf[s] = ar.h(static_cast<size_t>(B) * lh * lw * ray_ld[s]);
     udb_ray_embed_t p;
     memset(&p, 0, sizeof(p));
     p.intr4 = intr4; p.scales = c.F(idx("ray_scales.%d", s)); p.B = B; p.net_h = net_h; p.net_w = net_w; p.gh = lh; p.gw = lw;
-    p.bands = RAY_BANDS; p.out = rayf[s]; p.out_f32 = 0;
-    c.launch([&] { return udb_ray_embed_cat_orig(&p, RAY_K, st); });
+    p.bands = RAY_BANDS; p.out = rayf[s]; p.out_f32 = split_rays ? 2 : 0;
+    const int ld = ray_ld[s];
+    c.launch([&] { return udb_ray_embed_cat_orig(&p, ld, st); });
   }
 
   // ---- global head (decoder_old.py:408-426, 135-146): (scale, shift) of the depth
@@ -205,21 +284,27 @@ static int run_v2old(udb_engine_v2old* e, const udb_infer_v2old_args_t& a, Arena
     float* gcl = cam_mlp(c, "glob.cls", toks, R2, hid, 4 * hid, hid, nullptr, nullptr);
     // in_features(features + project_rays(rays)) = W_in features + (W_in project_rays(rays) + b_in), the second term per
     // token of the grid and shared by the four levels
-    __half* pr = ar.h(Rq * hid);
-    c.expect2("glob.rays_w", hid, RAY_K);
-    { Ctx::G q{rayf[0], c.H("glob.rays_w"), static_cast<int>(Rq), hid, RAY_K}; q.bias = c.F("glob.rays_b"); q.out = pr; c.gemm(q); }
+    // split mode: the same three GEMMs on split operands ([N, 3K] weights), project_rays writing a split operand for
+    // in_features, and an f32 context
+    __half* pr = ar.h(Rq * hid * sx);
+    c.expect2("glob.rays_w", hid, RAY_K * kx);
+    c.expect2("glob.in_w", hid, hid * kx);
+    { Ctx::G q{rayf[0], c.H("glob.rays_w"), static_cast<int>(Rq), hid, RAY_K * kx}; q.lda = ray_ld[0]; q.a_split_k = sp ? RAY_K : 0;
+      q.bias = c.F("glob.rays_b"); q.out = pr; q.ldc = hid * sx; q.out_split = sp ? hid : 0; c.gemm(q); }
     float* rr = ar.f(Rq * hid);
-    { Ctx::G q{pr, c.H("glob.in_w"), static_cast<int>(Rq), hid, hid}; q.bias = c.F("glob.in_b"); q.out = rr; q.out_f32 = 1; c.gemm(q); }
+    { Ctx::G q{pr, c.H("glob.in_w"), static_cast<int>(Rq), hid, hid * kx}; q.lda = hid * sx; q.a_split_k = sp ? hid : 0;
+      q.bias = c.F("glob.in_b"); q.out = rr; q.out_f32 = 1; c.gemm(q); }
     const long long nk = 4LL * nq + 2;
-    __half* gctx = ar.h(B * nk * hid);
+    void* gctx = ar.alloc(B * nk * hid * (sp ? 4 : 2));
     for (int b = 0; b < B; ++b) {
-      Ctx::G q{tokens + static_cast<long long>(b) * 4 * nq * hid, c.H("glob.in_w"), 4 * nq, hid, hid};
+      const __half* tb = sp ? head_tokens2 + static_cast<long long>(b) * 4 * nq * 2 * hid : tokens + static_cast<long long>(b) * 4 * nq * hid;
+      Ctx::G q{tb, c.H("glob.in_w"), 4 * nq, hid, hid * kx}; q.lda = hid * sx; q.a_split_k = sp ? hid : 0;
       q.resid = rr + static_cast<long long>(b) * nq * hid; q.resid_f32 = 1; q.ldr = hid; q.resid_mod = nq; q.resid_row_offset = 0;
-      q.out = gctx + static_cast<long long>(b) * nk * hid; c.gemm(q);
+      q.out = static_cast<char*>(gctx) + static_cast<long long>(b) * nk * hid * (sp ? 4 : 2); q.out_f32 = sp ? 1 : 0; c.gemm(q);
     }
-    c.launch([&] { return udb_copy_rows_f32_to_f16(gcl, gctx, B, 2, hid, nk, 4LL * nq, st); });
-    float* t = small_cross_block(c, "glob.agg1.", gcl, B, 2, gctx, nk, nullptr, hid, cf.expansion);
-    t = small_cross_block(c, "glob.agg2.", t, B, 2, gctx, nk, nullptr, hid, cf.expansion);
+    copy_cls_rows(c, gcl, gctx, B, 2, hid, nk, 4LL * nq, sp);
+    float* t = small_cross_block(c, "glob.agg1.", gcl, B, 2, gctx, nk, nullptr, hid, cf.expansion, sp);
+    t = small_cross_block(c, "glob.agg2.", t, B, 2, gctx, nk, nullptr, hid, cf.expansion, sp);
     float* x2 = cam_mlp(c, "glob.out", t, R2, hid, 2 * hid, 1, nullptr, nullptr);    // [B*2, 1] == [B, 2]: log scale, shift
     c.launch([&] {
       return cuda_rc(cudaMemcpyAsync(scale_shift, x2, sizeof(float) * 2 * B, cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(st)),
@@ -236,7 +321,8 @@ static int run_v2old(udb_engine_v2old* e, const udb_infer_v2old_args_t& a, Arena
     const std::string n = idx("rays.%d.", s);
     emb[s] = ar.f(R * (hid >> s));
     c.expect2(n + "w", hid >> s, RAY_K);
-    Ctx::G q{rayf[s], c.H(n + "w"), static_cast<int>(R), hid >> s, RAY_K}; q.bias = c.F(n + "b"); q.out = emb[s]; q.out_f32 = 1; c.gemm(q);
+    Ctx::G q{rayf[s], c.H(n + "w"), static_cast<int>(R), hid >> s, RAY_K}; q.lda = ray_ld[s];
+    q.bias = c.F(n + "b"); q.out = emb[s]; q.out_f32 = 1; c.gemm(q);
   }
   float* lat = ar.f(Rq * hid);
   {

@@ -32,7 +32,7 @@ import torch
 from . import _cabi as cabi
 from ._engine_model import HUB_KWARGS, EngineModel, PyTorchModelHubMixin, f32, infer_inputs
 from ._pack import (adapter, attn_block, c32, convnext_block, cross_block, h16, latents, mlp, pack_vit_encoder,
-                    pos_table_by_size, tokens_pos)
+                    pos_table_by_size, split_weight, tokens_pos)
 from .spec import PATCH
 from .spec_v2old import RAY_K, V2oldSpec, check_ratio, check_resolution, param_shapes
 
@@ -59,6 +59,18 @@ class UniDepthV2old(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         self.shape_constraints = sc
         self.interpolation_mode = "bilinear"
         self.resolution_level = None
+        # "f16" (default), "fp8" or "split", as UniDepthV1's.  "fp8": speed mode -- the encoder blocks' qkv, proj, fc1 and
+        # fc2 multiply FP8 E4M3 operands (include/udb.h udb_gemm_e4m3) with per-output-channel weight scales and per-row
+        # activation scales; the taps, heads and decoder run as in "f16".  "split": parity / debugging mode -- every GEMM
+        # on the path from the image to the intrinsics and to the global (scale, shift) (patch embedding, encoder blocks,
+        # the adapters' copy for the two heads, the camera head's in_features and kv, the global head's project_rays,
+        # in_features and kv) multiplies hi + lo f16 operands (udb_gemm_t.a_split_k), the taps and the heads' contexts
+        # are f32 and the encoder's attention runs in the fp32 kernel.  The depth head runs as in "f16".  Slower; not a
+        # speed mode.  Changing it repacks the weights.
+        self.precision = "f16"
+
+    def _fingerprint(self):
+        return (self.precision,) + super()._fingerprint()
 
     # ------------------------------------------------------------------ weight packing
     def _pack_tensors(self, dev, shape: Optional[Tuple[int, int]] = None):
@@ -93,9 +105,15 @@ class UniDepthV2old(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
 
     def _pack_weights(self, dev):
         s = self.spec
+        if self.precision not in ("split", "f16", "fp8"):
+            raise ValueError(f"precision must be 'split', 'f16' or 'fp8', not {self.precision!r}")
+        split, fp8 = self.precision == "split", self.precision == "fp8"
+        # GEMM weight of the split mode's operands: [N, 3K] = [hi | hi | lo], or f16 in the other modes
+        s16 = split_weight if split else h16
         sd = {k: v.detach() for k, v in self.state_dict().items()}
         T: Dict[str, torch.Tensor] = {}
-        S: Dict[str, float] = {}
+        # an engine without "precision" runs the f16 mode, so the f16 packing registers exactly the scalars it always has
+        S: Dict[str, float] = {"precision": 2.0} if fp8 else ({"precision": 1.0} if split else {})
         pd, dl = "pixel_decoder.", "pixel_decoder.depth_layer."
         hid, D = s.hidden, s.embed_dim
 
@@ -105,12 +123,15 @@ class UniDepthV2old(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
             return out
 
         # ---- encoder: the shared DINOv2 packing; the position table is a shape operand
-        T.update(pack_vit_encoder(sd, D, s.enc_depth, dev))
+        T.update(pack_vit_encoder(sd, D, s.enc_depth, dev, split=split, fp8=fp8))
         T["norm_w"], T["norm_b"] = c32(sd["pixel_encoder.norm.weight"]), c32(sd["pixel_encoder.norm.bias"])
 
         # ---- adapters
         for l in range(4):
-            adapter(T, sd, f"adapt.{l}.", f"{pd}input_adapter.input_adapters.{l}.", h16)
+            a = f"{pd}input_adapter.input_adapters.{l}."
+            adapter(T, sd, f"adapt.{l}.", a, h16)
+            if split:       # the adapter's copy for the camera and global heads, which read it on split operands
+                T[f"adapt.{l}.w_cam"] = split_weight(sd[a + "1.weight"])
         for dst, src, n in (("ctok", "camera_token_adapter", 4), ("gtok", "global_token_adapter", 2)):
             for i in range(n):
                 adapter(T, sd, f"{dst}.{i}.", f"{pd}{src}.input_adapters.{i}.", c32)
@@ -118,19 +139,19 @@ class UniDepthV2old(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         # ---- camera head
         cl = pd + "camera_layer."
         mlp(T, sd, "cam.cls", cl + "project_cls", c32)
-        mlp(T, sd, "cam.inf", cl + "in_features", h16)
+        mlp(T, sd, "cam.inf", cl + "in_features", s16)
         T["cam.pos"] = c32(sd[cl + "latents_pos"].reshape(4, hid))
-        cross_block(T, sd, "cam.agg1.", cl + "aggregate1.", h16)
-        cross_block(T, sd, "cam.agg2.", cl + "aggregate2.", h16)
+        cross_block(T, sd, "cam.agg1.", cl + "aggregate1.", s16)
+        cross_block(T, sd, "cam.agg2.", cl + "aggregate2.", s16)
         mlp(T, sd, "cam.out", cl + "out", c32)
 
         # ---- global head
         gl = pd + "global_layer."
         mlp(T, sd, "glob.cls", gl + "project_cls", c32)
-        T["glob.rays_w"], T["glob.rays_b"] = h16(kpad(sd[gl + "project_rays.weight"], RAY_K)), c32(sd[gl + "project_rays.bias"])
-        T["glob.in_w"], T["glob.in_b"] = h16(sd[gl + "in_features.weight"]), c32(sd[gl + "in_features.bias"])
-        cross_block(T, sd, "glob.agg1.", gl + "aggregate1.", h16)
-        cross_block(T, sd, "glob.agg2.", gl + "aggregate2.", h16)
+        T["glob.rays_w"], T["glob.rays_b"] = s16(kpad(sd[gl + "project_rays.weight"], RAY_K)), c32(sd[gl + "project_rays.bias"])
+        T["glob.in_w"], T["glob.in_b"] = s16(sd[gl + "in_features.weight"]), c32(sd[gl + "in_features.bias"])
+        cross_block(T, sd, "glob.agg1.", gl + "aggregate1.", s16)
+        cross_block(T, sd, "glob.agg2.", gl + "aggregate2.", s16)
         mlp(T, sd, "glob.out", gl + "out", c32)
 
         # ---- depth head
