@@ -607,7 +607,9 @@ int udb_set_weight(udb_engine* e, const char* name, const void* dev_ptr, const i
 /* Host scalars of the packed model (the two 1x1 head biases and their additive constants), and the encoder mode:
  * "precision" 0 = f16 operands, 1 = split-f16 (hi/lo) operands, 2 = FP8 E4M3 operands for the four linear layers of every
  * encoder block (blocks.{i}.{qkv,proj,fc1,fc2}_w8 [N, K] UDB_DT_E4M3 with f32 per-output-channel scales *_w8s [N]; the
- * activations are quantised per row on the fly); "fuse_ln" 1 = fused LayerNorm (precision 0 only). */
+ * activations are quantised per row on the fly); "fuse_ln" 1 = fused LayerNorm (precision 0 only).  The schedule
+ * (udb_workspace_bytes, udb_schedule_bytes, udb_infer_v2) refuses any other "precision", and precision 1 with a patch_w
+ * that is not split-packed ([D, 3*640]), naming the mode. */
 int udb_set_scalar(udb_engine* e, const char* name, double value);
 
 /* Geometry of one call, same arithmetic as get_paddings / get_resize_factor (unidepthv2.py:36-77). */

@@ -34,8 +34,9 @@ def _v2(cfg_name, depth=None, **attrs):
     return m.eval()
 
 
-def _v2_engine(m, drop=(), reshape=None):
+def _v2_engine(m, drop=(), reshape=None, scalars_over=None):
     tensors, scalars = m._pack_tensors(CPU)
+    scalars = dict(scalars, **(scalars_over or {}))
     cfg = m._engine_config(tensors)
     for name in drop:
         del tensors[name]
@@ -97,6 +98,22 @@ def test_v2_schedule_names_the_missing_or_misshapen_operand():
         assert "blocks.0.fc1_w" in msg and "expected" in msg, msg
     finally:
         lib.udb_destroy(h)
+
+
+@pytest.mark.parametrize("precision,want", [
+    (3.0, ("udb_infer_v2", "precision 3 unsupported")),                          # no such mode: refused, not run as f16
+    (1.0, ("udb_infer_v2", "precision 1", "split packing", "'patch_w'")),       # the f16 packing named as such
+])
+def test_v2_schedule_checks_the_precision(precision, want):
+    lib = _cabi.lib()
+    h, keep = _v2_engine(_v2("config_v2_vits14.json"), scalars_over={"precision": precision})
+    try:
+        assert lib.udb_schedule_bytes(h, 1, 240, 320, -1) == 0
+        msg = lib.udb_last_error().decode()
+        assert all(w in msg for w in want), msg
+    finally:
+        lib.udb_destroy(h)
+    del keep
 
 
 def _v1(arch=None):

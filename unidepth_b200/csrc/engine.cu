@@ -1,6 +1,8 @@
-// Whole-path engine behind udb_create / udb_set_weight / udb_workspace_bytes / udb_infer_v2
-// (include/udb.h): the host-side schedule of UniDepthV2.infer as one C call that only enqueues the
-// kernels of this library on the caller's stream.  Reference call stack it replaces:
+// Whole-path engine behind udb_create / udb_set_weight / udb_set_scalar / udb_workspace_bytes / udb_schedule_bytes /
+// udb_infer_v2 (include/udb.h): the host-side schedule of UniDepthV2.infer as one C call that only enqueues the
+// kernels of this library on the caller's stream, on the skeleton it shares with the UniDepthV1 and UniDepthV2old
+// engines (engine_common.h: the "precision" scalar, the DINOv2 patch embedding and block loop).  Reference call stack it
+// replaces:
 //   UniDepthV2.infer            unidepth/models/unidepthv2/unidepthv2.py:239-339
 //     get_paddings / get_resize_factor                                  :36-77
 //     encode_decode -> pixel_encoder (DINOv2)   backbones/metadinov2/*  dinov2.py:306-347, block.py:84-109
@@ -85,22 +87,25 @@ static int run(udb_engine* e, const udb_infer_args_t& a, const udb_geometry_t& g
   // ---- a2/a3/a4: pre-process + patch embedding + cls / position rows
   Stage stage;
   stage.next("udb:preprocess+patch_embed");
-  // Split-f16 precise mode (udb_set_scalar("precision", 1)): every f16 GEMM operand of the ENCODER is a hi/lo pair and
-  // the weights are packed [N, 3K] = [hi | hi | lo] (udb_gemm_t.a_split_k); attention runs in the fp32 kernel.  The
-  // cls tokens / camera head are fp32 anyway, so the intrinsics then carry no f16 operand rounding at all.
-  const bool sp = e->scalars.count("precision") && e->scalars["precision"] == 1.0;
+  // Split-f16 precise mode (precision 1): every f16 GEMM operand of the ENCODER is a hi/lo pair and the weights are
+  // packed [N, 3K] = [hi | hi | lo] (udb_gemm_t.a_split_k); attention runs in the fp32 kernel.  The cls tokens / camera
+  // head are fp32 anyway, so the intrinsics then carry no f16 operand rounding at all.
+  // E4M3 mode (precision 2): the four linear layers of every encoder block run on e4m3 operands (vit_block_e4m3); the
+  // patch embedding, attention and everything after the encoder stay as in the f16 mode.
+  const Precision prec = encoder_precision(c, "udb_infer_v2", "patch_w", 3 * 640);
+  if (prec == PREC_BAD) return 1;
+  const bool sp = prec == PREC_SPLIT;
   const int sx = sp ? 2 : 1;
-  // E4M3 mode (udb_set_scalar("precision", 2)): the four linear layers of every encoder block run on e4m3 operands
-  // (vit_block_e4m3); the patch embedding, attention and everything after the encoder stay as in the f16 mode.
-  const bool f8 = e->scalars.count("precision") && e->scalars["precision"] == 2.0;
-  // Fused LayerNorm (udb_set_scalar("fuse_ln", 1), default f16 mode): norm1 / norm2 never run as their own pass.  The GEMM
+  // Fused LayerNorm (udb_set_scalar("fuse_ln", 1), f16 mode only): norm1 / norm2 never run as their own pass.  The GEMM
   // that updates the residual stream (patch embed, attn.proj, mlp.fc2) also writes the f16 copy of its rows and their
   // per-part statistics; qkv / fc1 read that copy with LayerNorm-folded weights (udb_gemm_t.ln_*; block.py:84-109).
-  const bool fuse = !sp && !f8 && e->scalars.count("fuse_ln") && e->scalars["fuse_ln"] == 1.0;
+  const bool fuse = prec == PREC_F16 && e->scalars.count("fuse_ln") && e->scalars["fuse_ln"] == 1.0;
   const int ln_bn = D % 256 == 0 ? 256 : (D % 192 == 0 ? 192 : (D % 128 == 0 ? 128 : 64));   // udb_gemm_f16's tile width for N = D
-  const int ln_parts = D / ln_bn * 2, ln_pc = ln_bn / 2;
-  __half* x16 = fuse ? ar.h(BT * D) : nullptr;
-  float* stats = fuse ? ar.f(BT * ln_parts * 2) : nullptr;
+  VitBlocks v{B, T, D, cf.enc_heads, cf.depth};
+  v.split = sp; v.fuse = fuse; v.fp8 = prec == PREC_E4M3;
+  v.ln_parts = D / ln_bn * 2; v.ln_pc = ln_bn / 2;
+  v.x16 = fuse ? ar.h(BT * D) : nullptr;
+  v.stats = fuse ? ar.f(BT * v.ln_parts * 2) : nullptr;
   __half* patches = ar.h(BN * 640 * sx);
   {
     udb_preprocess_t p;
@@ -111,20 +116,7 @@ static int run(udb_engine* e, const udb_infer_args_t& a, const udb_geometry_t& g
     c.launch([&] { return udb_preprocess_patchify(&p, st); });
   }
   float* x = ar.f(BT * D);           // fp32 residual stream
-  {
-    Ctx::G q{patches, c.H("patch_w"), static_cast<int>(BN), D, sp ? 3 * 640 : 640};
-    q.lda = 640 * sx; q.a_split_k = sp ? 640 : 0;
-    q.bias = c.F("patch_b"); q.resid = tb.pos; q.resid_f32 = 1; q.ldr = D; q.out = x; q.out_f32 = 1;
-    q.rows_per_group = N; q.group_stride = T; q.row_offset = 1; q.resid_mod = N; q.resid_row_offset = 1;
-    c.expect2("patch_w", D, sp ? 3 * 640 : 640);
-    if (fuse) { q.out2 = x16; q.out2_leaky = 0; q.ln_stats_out = stats; q.ln_parts = ln_parts; q.ln_part_cols = ln_pc; }
-    c.gemm(q);
-    const float* cls = c.F("cls");
-    c.launch([&] {
-      return fuse ? udb_set_cls_rows_ln(x, x16, stats, cls, tb.pos, B, T, D, ln_parts, ln_pc, st)
-                  : udb_set_cls_rows(x, cls, tb.pos, B, T, D, st);
-    });
-  }
+  vit_embed(c, patches, tb.pos, x, v);
 
   // ---- a5-a8: transformer blocks, taps through the final norm
   stage.next("udb:encoder_blocks");
@@ -132,8 +124,6 @@ static int run(udb_engine* e, const udb_infer_args_t& a, const udb_geometry_t& g
   float* clss[4];
   for (int l = 0; l < 4; ++l) { feats[l] = ar.h(BN * D); clss[l] = ar.f(static_cast<size_t>(B) * D); }
   {
-    VitBlocks v{B, T, D, cf.enc_heads, cf.depth};
-    v.split = sp; v.fuse = fuse; v.fp8 = f8; v.x16 = x16; v.stats = stats; v.ln_parts = ln_parts; v.ln_pc = ln_pc;
     int tap = 0;
     vit_blocks(c, "blocks.", x, v, [&](int i) {
       if (tap < 4 && i + 1 == cf.taps[tap]) {

@@ -1,6 +1,7 @@
-// Shared by the whole-path engines (engine.cu: UniDepthV2, engine_v1.cu: UniDepthV1): registered weights and prepared
-// shapes, the bump allocator over the caller's workspace, NVTX stage ranges, the launch gate and thin wrappers that fill
-// the operator argument structs.
+// Shared by the three whole-path engines (engine.cu: UniDepthV2, engine_v1.cu: UniDepthV1, engine_v2old.cu: UniDepthV2old):
+// registered weights and prepared shapes, the bump allocator over the caller's workspace, NVTX stage ranges, the launch
+// gate, thin wrappers that fill the operator argument structs, the "precision" scalar, and the schedule stages more than
+// one engine runs (the DINOv2 patch embedding and block loop, V1's and V2old's decoder blocks, adapters and camera context).
 #pragma once
 #include <cuda_fp16.h>
 #include <math.h>
@@ -293,6 +294,28 @@ struct Ctx {
   }
 };
 
+// The "precision" scalar: 0 (absent) f16 operands; 1 split-f16 operands (parity mode: [hi | lo] operand pairs times
+// [hi | hi | lo] weights, see each engine for the GEMMs it covers); 2 e4m3 operands for the encoder blocks.  Any other
+// value is refused, and so is precision 1 when `weight`, the encoder's first GEMM weight, does not have the split
+// packing's `split_cols` columns: an f16 packing is named for what it is, not only by its first mis-shaped operand.  `fn`,
+// the calling entry point, prefixes the message; PREC_BAD means the error is set.
+enum Precision { PREC_BAD = -1, PREC_F16 = 0, PREC_SPLIT = 1, PREC_E4M3 = 2 };
+static inline Precision encoder_precision(Ctx& c, const char* fn, const char* weight, int64_t split_cols) {
+  const auto it = c.e->scalars.find("precision");
+  const double p = it == c.e->scalars.end() ? 0.0 : it->second;
+  if (p != 0.0 && p != 1.0 && p != 2.0) { set_error("%s: precision %g unsupported (0 f16, 1 split f16, 2 e4m3)", fn, p); return PREC_BAD; }
+  if (p == 1.0) {
+    const Weight* w = c.W(weight);
+    if (c.rc) return PREC_BAD;
+    if (w->ndim != 2 || w->shape[1] != split_cols) {
+      set_error("%s: precision 1 (split f16) needs the split packing: '%s' has %lld columns, expected %lld", fn, weight,
+                static_cast<long long>(w->shape[1]), static_cast<long long>(split_cols));
+      return PREC_BAD;
+    }
+  }
+  return static_cast<Precision>(static_cast<int>(p));
+}
+
 // LN -> Linear -> GELU -> Linear (+ gamma, + residual), fp32, camera head (layers/mlp.py:9-35)
 static inline float* cam_mlp(Ctx& c, const std::string& pre, const float* x, int rows, int hid, int mid, int out_dim,
                       const float* resid, const float* gamma) {
@@ -450,6 +473,146 @@ static inline void mh_attn_block(Ctx& c, const std::string& p, float* x, int B, 
   mlp_resid(c, p + "m", x, R, C, 4 * C, c.F(p + "ls2"));
 }
 
+// The four input adapters (decoder.py:395-408, decoder_old.py:448-461).  Level l, [B, sh[l], sw[l], dims[l]] f16 (f32 in
+// split mode), is resized (antialiased) to the common grid hc x wc when its own grid differs, then LayerNorm -> Linear ->
+// GELU writes it twice: rows [l*nq, (l+1)*nq) of each image in tokens [B, 4*nq, hid] and columns [l*hid, (l+1)*hid) of
+// featcat [B*nq, 4*hid].  Split mode (`sp`): the LayerNorm writes a [hi | lo] operand whose hi half those two GEMMs read,
+// and the heads' copy of the tokens multiplies the whole operand with "adapt.<l>.w_cam" [hid, 3*C], into head_f32 (f32
+// rows) and head_split ([hi | lo] rows), each where non-null.
+static inline void adapters(Ctx& c, void* const* levels, const int* dims, const int* sh, const int* sw, int B, int hc, int wc,
+                            int hid, bool sp, __half* tokens, __half* featcat, float* head_f32, __half* head_split) {
+  Arena& ar = *c.ar;
+  const int nq = hc * wc, sx = sp ? 2 : 1;
+  const long long Rq = static_cast<long long>(B) * nq;
+  for (int l = 0; l < 4; ++l) {
+    const size_t m = ar.mark();
+    const int C = dims[l];
+    const void* src = levels[l];
+    if (sh[l] != hc || sw[l] != wc) {
+      void* r = ar.alloc(Rq * C * (sp ? 4 : 2));
+      c.launch([&] {
+        return sp ? udb_aa_resize_nhwc_f32(static_cast<const float*>(levels[l]), static_cast<float*>(r), B, sh[l], sw[l], C, hc, wc, c.st)
+                  : udb_aa_resize_nhwc_f16(levels[l], r, B, sh[l], sw[l], C, hc, wc, c.st);
+      });
+      src = r;
+    }
+    const std::string ad = idx("adapt.%d.", l);
+    __half* an = ar.h(Rq * C * sx);
+    if (sp) c.ln_any(src, 1, an, UDB_LN_OUT_SPLIT, c.F(ad + "ln_w"), c.F(ad + "ln_b"), Rq, C, 1e-5f, 2 * C);
+    else ln16(c, src, 0, an, ad + "ln_w", ad + "ln_b", Rq, C, 1e-5f);
+    { Ctx::G q{an, c.H(ad + "w"), static_cast<int>(Rq), hid, C}; q.lda = C * sx; q.bias = c.F(ad + "b"); q.act = UDB_ACT_GELU; q.out = tokens;
+      q.rows_per_group = nq; q.group_stride = 4 * nq; q.row_offset = l * nq; c.gemm(q); }
+    { Ctx::G q{an, c.H(ad + "w"), static_cast<int>(Rq), hid, C}; q.lda = C * sx; q.bias = c.F(ad + "b"); q.act = UDB_ACT_GELU;
+      q.out = featcat + l * hid; q.ldc = 4 * hid; c.gemm(q); }
+    void* const head[2] = {head_f32, head_split};
+    if (head[0] || head[1]) c.expect2(ad + "w_cam", hid, 3 * C);
+    for (int k = 0; k < 2; ++k) {
+      if (!head[k]) continue;
+      Ctx::G q{an, c.H(ad + "w_cam"), static_cast<int>(Rq), hid, 3 * C}; q.lda = 2 * C; q.a_split_k = C; q.bias = c.F(ad + "b");
+      q.act = UDB_ACT_GELU; q.rows_per_group = nq; q.group_stride = 4 * nq; q.row_offset = l * nq; q.out = head[k];
+      if (k == 0) q.out_f32 = 1;
+      else { q.ldc = 2 * hid; q.out_split = hid; }
+      c.gemm(q);
+    }
+    ar.release(m);
+  }
+}
+
+// The n cls tokens cls[i], f32 [B, dims[i]] -> LN + Linear + GELU per token (ListAdapter, decoder.py:395-408,
+// decoder_old.py:13-29) -> f32 [B, n, hid]
+static inline float* token_adapter(Ctx& c, const std::string& p, float* const* cls, const int* dims, int n, int B, int hid) {
+  float* toks = c.ar->f(static_cast<size_t>(B) * n * hid);
+  for (int i = 0; i < n; ++i) {
+    const std::string tk = p + idx("%d.", i);
+    const int D = dims[i];
+    float* t = c.ar->f(static_cast<size_t>(B) * D);
+    c.ln_any(cls[i], 1, t, 1, c.F(tk + "ln_w"), c.F(tk + "ln_b"), B, D, 1e-5f);
+    c.small_linear(t, B, D, c.F(tk + "w"), hid, c.F(tk + "b"), UDB_ACT_GELU, nullptr, nullptr, toks + i * hid, D, n * hid, 0);
+  }
+  return toks;
+}
+
+// The n head tokens x f32 [B*n, hid] into rows [row0, row0 + n) of each image's nk context rows: f16, or f32 in split mode
+static inline void copy_cls_rows(Ctx& c, const float* x, void* ctx, int B, int n, int hid, long long nk, long long row0, bool sp) {
+  c.launch([&] {
+    if (!sp) return udb_copy_rows_f32_to_f16(x, ctx, B, n, hid, nk, row0, c.st);
+    const size_t row = sizeof(float) * hid;
+    return cuda_rc(cudaMemcpy2DAsync(static_cast<float*>(ctx) + row0 * hid, nk * row, x, n * row, n * row, B,
+                                     cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(c.st)),
+                   "engine: copying the head tokens into the f32 context");
+  });
+}
+
+// The camera head's context (decoder.py:311-343, decoder_old.py:378-406), 4*nq + n rows per image: in_features (LN ->
+// Linear -> GELU -> Linear) of tokens + tokens_pos [4*nq, hid] into the first 4*nq, then the n head tokens x f32 [B*n, hid]
+// after them.  f16 from the f16 tokens; split mode (`sp`): from the f32 head tokens through [hi | lo] operands and
+// [N, 3K] weights into f32 rows.  The context is allocated before the scratch of in_features, which is released.
+static inline void* camera_context(Ctx& c, const void* tokens, const float* tokens_pos, const float* x, int B, int nq, int n,
+                                   int hid, bool sp) {
+  Arena& ar = *c.ar;
+  const long long Rt = 4LL * B * nq, nk = 4LL * nq + n;
+  const int sx = sp ? 2 : 1, kx = sp ? 3 : 1;
+  void* ctx = ar.alloc(B * nk * hid * (sp ? 4 : 2));
+  const size_t m = ar.mark();
+  __half* a1 = ar.h(Rt * hid * sx);
+  __half* m1 = ar.h(Rt * 2 * hid * sx);
+  if (sp) {
+    c.expect2("cam.inf.w1", 2 * hid, 3 * hid);
+    c.expect2("cam.inf.w2", hid, 6 * hid);
+  }
+  c.ln_any(tokens, sp ? 1 : 0, a1, sp ? UDB_LN_OUT_SPLIT : 0, c.F("cam.inf.nw"), c.F("cam.inf.nb"), Rt, hid, 1e-5f, sp ? 2 * hid : 0,
+           tokens_pos, 4LL * nq);
+  { Ctx::G q{a1, c.H("cam.inf.w1"), static_cast<int>(Rt), 2 * hid, hid * kx}; q.lda = hid * sx; q.a_split_k = sp ? hid : 0;
+    q.bias = c.F("cam.inf.b1"); q.act = UDB_ACT_GELU; q.out = m1; q.ldc = 2 * hid * sx; q.out_split = sp ? 2 * hid : 0; c.gemm(q); }
+  { Ctx::G q{m1, c.H("cam.inf.w2"), static_cast<int>(Rt), hid, 2 * hid * kx}; q.lda = 2 * hid * sx; q.a_split_k = sp ? 2 * hid : 0;
+    q.bias = c.F("cam.inf.b2"); q.out = ctx; q.out_f32 = sp ? 1 : 0; q.rows_per_group = 4 * nq; q.group_stride = static_cast<int>(nk);
+    q.row_offset = 0; c.gemm(q); }
+  ar.release(m);
+  copy_cls_rows(c, x, ctx, B, n, hid, nk, 4LL * nq, sp);
+  return ctx;
+}
+
+// AttentionBlock with one head over a long context and at most four queries (decoder.py:225-236, decoder_old.py:72-77,
+// 142-143): the heads' aggregate blocks, on the split-key cross attention.  x f32 [B*nq, hid] -> new f32 rows.  f16
+// context; split mode (`sp`): the context is f32, its LayerNorm writes a split operand for the kv GEMM ([2*hid, 3*hid]
+// weight), and the attention reads f32 (k | v) rows.
+static inline float* small_cross_block(Ctx& c, const std::string& p, const float* x, int B, int nq, const void* ctx, long long nk,
+                                       const float* q_pos, int hid, int expansion, bool sp) {
+  Arena& ar = *c.ar;
+  const int R = B * nq;
+  const long long Rc = static_cast<long long>(B) * nk;
+  float* xn = ar.f(static_cast<size_t>(R) * hid);
+  float* q = ar.f(static_cast<size_t>(R) * hid);
+  float* at = ar.f(static_cast<size_t>(R) * hid);
+  float* scratch = ar.f(static_cast<size_t>(B) * 16 * 4 * (hid + 2));
+  c.layernorm(x, 1, xn, 1, c.F(p + "nxw"), c.F(p + "nxb"), R, hid, 1e-5f);
+  c.small_linear(xn, R, hid, c.F(p + "q_w"), hid, c.F(p + "q_b"), UDB_ACT_NONE, nullptr, nullptr, q);
+  const size_t m = ar.mark();          // the normalised context and its (k | v) rows: dead once the attention has run
+  void* kv;
+  if (sp) {
+    __half* cn = ar.h(Rc * 2 * hid);
+    c.ln_any(ctx, 1, cn, UDB_LN_OUT_SPLIT, c.F(p + "ncw"), c.F(p + "ncb"), Rc, hid, 1e-5f, 2 * hid);
+    kv = ar.f(Rc * 2 * hid);
+    c.expect2(p + "kv_w", 2 * hid, 3 * hid);
+    Ctx::G g{cn, c.H(p + "kv_w"), static_cast<int>(Rc), 2 * hid, 3 * hid}; g.lda = 2 * hid; g.a_split_k = hid;
+    g.bias = c.F(p + "kv_b"); g.out = kv; g.out_f32 = 1; c.gemm(g);
+  } else {
+    __half* cn = ar.h(Rc * hid);
+    ln16(c, ctx, 0, cn, p + "ncw", p + "ncb", Rc, hid, 1e-5f);
+    kv = ar.h(Rc * 2 * hid);
+    Ctx::G g{cn, c.H(p + "kv_w"), static_cast<int>(Rc), 2 * hid, hid}; g.bias = c.F(p + "kv_b"); g.out = kv; c.gemm(g);
+  }
+  c.launch([&] {
+    const float scale = 1.0f / sqrtf(static_cast<float>(hid));
+    return sp ? udb_cross_attn_small_f32(q, q_pos, static_cast<const float*>(kv), at, scratch, B, nq, static_cast<int>(nk), hid, scale, c.st)
+              : udb_cross_attn_small(q, q_pos, kv, at, scratch, B, nq, static_cast<int>(nk), hid, scale, c.st);
+  });
+  ar.release(m);
+  float* t2 = xn;
+  c.small_linear(at, R, hid, c.F(p + "out_w"), hid, c.F(p + "out_b"), UDB_ACT_NONE, c.F(p + "ls1"), x, t2);
+  return cam_mlp(c, p + "mlp", t2, R, hid, expansion * hid, hid, t2, c.F(p + "ls2"));
+}
+
 // ------------------------------------------------------------------------------------------ DINOv2 blocks
 // Shape and packing mode of the DINOv2 block loop (UniDepthV2 uses every mode; UniDepthV1 ViT-L the f16 and e4m3 ones).
 struct VitBlocks {
@@ -461,6 +624,26 @@ struct VitBlocks {
   float* stats = nullptr;      // GEMMs that write x (the patch embedding included)
   int ln_parts = 0, ln_pc = 0;
 };
+
+// DINOv2 patch embedding (dinov2.py:306-347) in the block loop's mode `v`: the patch GEMM of the B*N pre-processed patch
+// rows (N = T - 1; [hi | lo] rows and a [D, 3*640] weight in split mode) into rows 1..N of each image's T rows of the f32
+// residual stream x, with the position table pos [T, D] (cls row first) as row-mapped residual, then the cls rows
+// (cls + pos[0]).  In the fused mode both also write the f16 copy of x and its LayerNorm statistics.
+static inline void vit_embed(Ctx& c, const __half* patches, const float* pos, float* x, const VitBlocks& v) {
+  const int B = v.B, T = v.T, D = v.D, N = T - 1, K = v.split ? 3 * 640 : 640;
+  c.expect2("patch_w", D, K);
+  Ctx::G q{patches, c.H("patch_w"), B * N, D, K};
+  q.lda = v.split ? 2 * 640 : 640; q.a_split_k = v.split ? 640 : 0;
+  q.bias = c.F("patch_b"); q.resid = pos; q.resid_f32 = 1; q.ldr = D; q.out = x; q.out_f32 = 1;
+  q.rows_per_group = N; q.group_stride = T; q.row_offset = 1; q.resid_mod = N; q.resid_row_offset = 1;
+  if (v.fuse) { q.out2 = v.x16; q.out2_leaky = 0; q.ln_stats_out = v.stats; q.ln_parts = v.ln_parts; q.ln_part_cols = v.ln_pc; }
+  c.gemm(q);
+  const float* cls = c.F("cls");
+  c.launch([&] {
+    return v.fuse ? udb_set_cls_rows_ln(x, v.x16, v.stats, cls, pos, B, T, D, v.ln_parts, v.ln_pc, c.st)
+                  : udb_set_cls_rows(x, cls, pos, B, T, D, c.st);
+  });
+}
 
 // One block in e4m3 mode: each of the four linear layers reads an e4m3 copy of its input (LayerNorm or row quantiser,
 // one scale per row) and e4m3 weights with one scale per output channel; attention and the epilogues are those of the

@@ -189,21 +189,11 @@ static void dino_encoder(Ctx& c, const udb_v1_config_t& cf, const udb_infer_v1_a
   __half* patches = ar.h(BN * 640 * sx);
   preprocess(c, cf, a, g, patches, 14, split);
   float* x = ar.f(BT * D);           // fp32 residual stream [B, 1 + N, D]
-  {
-    c.expect2("patch_w", D, split ? 3 * 640 : 640);
-    c.expect2("pos", T, D);
-    const float* pos = c.F("pos");
-    const float* cls = c.F("cls");     // looked up here so that a dry run names it when it is missing
-    Ctx::G q{patches, c.H("patch_w"), static_cast<int>(BN), D, split ? 3 * 640 : 640};
-    q.lda = 640 * sx; q.a_split_k = split ? 640 : 0;
-    q.bias = c.F("patch_b"); q.resid = pos; q.resid_f32 = 1; q.ldr = D; q.out = x; q.out_f32 = 1;
-    q.rows_per_group = N; q.group_stride = T; q.row_offset = 1; q.resid_mod = N; q.resid_row_offset = 1;
-    c.gemm(q);
-    c.launch([&] { return udb_set_cls_rows(x, cls, pos, B, T, D, c.st); });
-  }
   VitBlocks v{B, T, D, D / 64, depth};
   v.fp8 = fp8;
   v.split = split;
+  c.expect2("pos", T, D);
+  vit_embed(c, patches, c.F("pos"), x, v);
   int slice = 0, start = 0;
   vit_blocks(c, "blocks.", x, v, [&](int i) {
     if (i == start + cf.depths[slice]) { start = i; ++slice; }
@@ -249,19 +239,9 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
   // mode): every GEMM of the encoder and of the camera head's context path (adapters, in_features, the aggregate block's
   // kv) multiplies [hi | lo] operands with [hi | hi | lo] weights, and the encoder levels and camera context are f32;
   // the depth head reads the hi half of the adapters' LayerNorm and runs as in the f16 mode.
-  const double prec = e->scalars.count("precision") ? e->scalars["precision"] : 0.0;
-  if (prec != 0.0 && prec != 1.0 && prec != 2.0) { set_error("udb_infer_v1: precision %g unsupported (0 f16, 1 split f16, 2 e4m3)", prec); return 1; }
-  const bool f8 = prec == 2.0, sp = prec == 1.0;
-  if (sp) {   // an f16 packing registered with precision 1 is named for what it is, not only by its first mis-shaped operand
-    const char* first = dino ? "patch_w" : "stem_w";
-    const int k3 = dino ? 3 * 640 : 3 * 64;
-    const Weight* w = c.W(first);
-    if (!c.rc && (w->ndim != 2 || w->shape[1] != k3)) {
-      set_error("udb_infer_v1: precision 1 (split f16) needs the split packing: '%s' has %lld columns, expected %d", first,
-                static_cast<long long>(w->shape[1]), k3);
-      return 1;
-    }
-  }
+  const Precision prec = encoder_precision(c, "udb_infer_v1", dino ? "patch_w" : "stem_w", dino ? 3 * 640 : 3 * 64);
+  if (prec == PREC_BAD) return 1;
+  const bool f8 = prec == PREC_E4M3, sp = prec == PREC_SPLIT;
 
   // ---- pre-processing + stem (convnext.py:371-383: conv k4 s4 as an im2col GEMM, then LayerNorm2d)
   stage.next("udb_v1:preprocess+stem");
@@ -337,35 +317,7 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
   __half* tokens = ar.h((Rq * 4 + 64) * hid);                    // [B, 4*nq, hid]  (features_tokens,   decoder.py:220)
   // split mode: the camera head's copy of the tokens, f32 from split operands (the depth head keeps the f16 tokens)
   float* cam_tokens = sp ? ar.f(Rq * 4 * hid) : nullptr;
-  for (int l = 0; l < 4; ++l) {
-    const size_t m = ar.mark();
-    const int C = cf.dims[l];
-    const void* src = levels[l];
-    if (sh[l] != hc || sw[l] != wc) {
-      void* r = ar.alloc(Rq * C * (sp ? 4 : 2));
-      c.launch([&] {
-        return sp ? udb_aa_resize_nhwc_f32(static_cast<const float*>(levels[l]), static_cast<float*>(r), B, sh[l], sw[l], C, hc, wc, st)
-                  : udb_aa_resize_nhwc_f16(levels[l], r, B, sh[l], sw[l], C, hc, wc, st);
-      });
-      src = r;
-    }
-    const std::string ad = idx("adapt.%d.", l);
-    const int sx = sp ? 2 : 1;
-    __half* an = ar.h(Rq * C * sx);
-    if (sp) c.ln_any(src, 1, an, UDB_LN_OUT_SPLIT, c.F(ad + "ln_w"), c.F(ad + "ln_b"), Rq, C, 1e-5f, 2 * C);
-    else ln16(c, src, 0, an, ad + "ln_w", ad + "ln_b", Rq, C, 1e-5f);
-    { Ctx::G q{an, c.H(ad + "w"), static_cast<int>(Rq), hid, C}; q.lda = C * sx; q.bias = c.F(ad + "b"); q.act = UDB_ACT_GELU; q.out = tokens;
-      q.rows_per_group = nq; q.group_stride = 4 * nq; q.row_offset = l * nq; c.gemm(q); }
-    { Ctx::G q{an, c.H(ad + "w"), static_cast<int>(Rq), hid, C}; q.lda = C * sx; q.bias = c.F(ad + "b"); q.act = UDB_ACT_GELU;
-      q.out = featcat + l * hid; q.ldc = 4 * hid; c.gemm(q); }
-    if (sp) {
-      c.expect2(ad + "w_cam", hid, 3 * C);
-      Ctx::G q{an, c.H(ad + "w_cam"), static_cast<int>(Rq), hid, 3 * C}; q.lda = 2 * C; q.a_split_k = C; q.bias = c.F(ad + "b");
-      q.act = UDB_ACT_GELU; q.out = cam_tokens; q.out_f32 = 1; q.rows_per_group = nq; q.group_stride = 4 * nq; q.row_offset = l * nq;
-      c.gemm(q);
-    }
-    ar.release(m);
-  }
+  adapters(c, levels, cf.dims, sh, sw, B, hc, wc, hid, sp, tokens, featcat, cam_tokens, nullptr);
   const float* tokens_pos = c.F("tokens_pos");                     // [4*nq, hid]: sine position + level embedding (decoder.py:410-433)
   {
     const Weight* tp = c.W("tokens_pos");
@@ -376,88 +328,16 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
   stage.next("udb_v1:camera_head");
   float* intr4 = ar.f(static_cast<size_t>(B) * 4);
   float* k4_points = ar.f(static_cast<size_t>(B) * 4);
+  const size_t cam_mark = ar.mark();          // the camera head's scratch: dead once the intrinsics kernel has read x4
   const float* x4 = nullptr;
   if (!(a.skip_camera && a.intrinsics)) {
-    const size_t m = ar.mark();
     const int R4 = B * 4;
-    float* toks = ar.f(static_cast<size_t>(R4) * hid);
-    for (int i = 0; i < 4; ++i) {
-      const std::string tk = idx("tok.%d.", i);
-      float* t = ar.f(static_cast<size_t>(B) * cls_dim[i]);
-      c.ln_any(clsbuf[i], 1, t, 1, c.F(tk + "ln_w"), c.F(tk + "ln_b"), B, cls_dim[i], 1e-5f);
-      c.small_linear(t, B, cls_dim[i], c.F(tk + "w"), hid, c.F(tk + "b"), UDB_ACT_GELU, nullptr, nullptr, toks + i * hid, cls_dim[i], 4 * hid, 0);
-    }
+    float* toks = token_adapter(c, "tok.", clsbuf, cls_dim, 4, B, hid);
     // cls_project: LN -> Linear(hid -> hid/2) -> GELU -> Linear(hid/2 -> hid)
     float* cl = cam_mlp(c, "cam.cls", toks, R4, hid, hid / 2, hid, nullptr, nullptr);
-    // context = in_features(features + pos) ++ cls tokens
-    const long long Rc = static_cast<long long>(B) * (4 * nq + 4);
-    void* ctx = ar.alloc(Rc * hid * (sp ? 4 : 2));            // f16, or f32 in split mode
-    if (sp) {
-      // the same steps on split operands: LayerNorm (f32 tokens + position, split out) -> in_features' two GEMMs -> f32
-      // context rows; the cls rows are copied in f32
-      const size_t m2 = ar.mark();
-      __half* a1 = ar.h(Rq * 4 * 2 * hid);
-      __half* m1 = ar.h(Rq * 4 * 4 * hid);
-      c.expect2("cam.inf.w1", 2 * hid, 3 * hid);
-      c.expect2("cam.inf.w2", hid, 6 * hid);
-      c.ln_any(cam_tokens, 1, a1, UDB_LN_OUT_SPLIT, c.F("cam.inf.nw"), c.F("cam.inf.nb"), Rq * 4, hid, 1e-5f, 2 * hid, tokens_pos, 4LL * nq);
-      { Ctx::G q{a1, c.H("cam.inf.w1"), static_cast<int>(Rq * 4), 2 * hid, 3 * hid}; q.lda = 2 * hid; q.a_split_k = hid;
-        q.bias = c.F("cam.inf.b1"); q.act = UDB_ACT_GELU; q.out = m1; q.ldc = 4 * hid; q.out_split = 2 * hid; c.gemm(q); }
-      { Ctx::G q{m1, c.H("cam.inf.w2"), static_cast<int>(Rq * 4), hid, 6 * hid}; q.lda = 4 * hid; q.a_split_k = 2 * hid;
-        q.bias = c.F("cam.inf.b2"); q.out = ctx; q.out_f32 = 1; q.rows_per_group = 4 * nq; q.group_stride = 4 * nq + 4; q.row_offset = 0;
-        c.gemm(q); }
-      ar.release(m2);
-      c.launch([&] {
-        const size_t row = sizeof(float) * hid;
-        return cuda_rc(cudaMemcpy2DAsync(static_cast<float*>(ctx) + 4LL * nq * hid, (4 * nq + 4) * row, cl, 4 * row, 4 * row, B,
-                                         cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(st)),
-                       "engine_v1: copying the camera tokens into the f32 context");
-      });
-    } else {
-      const size_t m2 = ar.mark();
-      __half* a1 = ar.h(Rq * 4 * hid);
-      __half* m1 = ar.h(Rq * 4 * 2 * hid);
-      c.ln_any(tokens, 0, a1, 0, c.F("cam.inf.nw"), c.F("cam.inf.nb"), Rq * 4, hid, 1e-5f, 0, tokens_pos, 4LL * nq);
-      { Ctx::G q{a1, c.H("cam.inf.w1"), static_cast<int>(Rq * 4), 2 * hid, hid}; q.bias = c.F("cam.inf.b1"); q.act = UDB_ACT_GELU; q.out = m1; c.gemm(q); }
-      { Ctx::G q{m1, c.H("cam.inf.w2"), static_cast<int>(Rq * 4), hid, 2 * hid}; q.bias = c.F("cam.inf.b2"); q.out = ctx;
-        q.rows_per_group = 4 * nq; q.group_stride = 4 * nq + 4; q.row_offset = 0; c.gemm(q); }
-      ar.release(m2);
-      c.launch([&] { return udb_copy_rows_f32_to_f16(cl, ctx, B, 4, hid, 4LL * nq + 4, 4LL * nq, st); });
-    }
+    const void* ctx = camera_context(c, sp ? static_cast<const void*>(cam_tokens) : tokens, tokens_pos, cl, B, nq, 4, hid, sp);
     // aggregate: the 4 tokens attend to the context (single head of width hid, position term on q)
-    float* t;
-    {
-      const std::string ag = "cam.agg.";
-      float* xn = ar.f(static_cast<size_t>(R4) * hid);
-      c.layernorm(cl, 1, xn, 1, c.F(ag + "nxw"), c.F(ag + "nxb"), R4, hid, 1e-5f);
-      void* kv;
-      if (sp) {         // split LayerNorm -> kv GEMM on split operands -> f32 (k | v)
-        __half* cn = ar.h(Rc * 2 * hid);
-        c.ln_any(ctx, 1, cn, UDB_LN_OUT_SPLIT, c.F(ag + "ncw"), c.F(ag + "ncb"), Rc, hid, 1e-5f, 2 * hid);
-        kv = ar.f(Rc * 2 * hid);
-        c.expect2(ag + "kv_w", 2 * hid, 3 * hid);
-        { Ctx::G q{cn, c.H(ag + "kv_w"), static_cast<int>(Rc), 2 * hid, 3 * hid}; q.lda = 2 * hid; q.a_split_k = hid;
-          q.bias = c.F(ag + "kv_b"); q.out = kv; q.out_f32 = 1; c.gemm(q); }
-      } else {
-        __half* cn = ar.h(Rc * hid);
-        ln16(c, ctx, 0, cn, ag + "ncw", ag + "ncb", Rc, hid, 1e-5f);
-        kv = ar.h(Rc * 2 * hid);
-        { Ctx::G q{cn, c.H(ag + "kv_w"), static_cast<int>(Rc), 2 * hid, hid}; q.bias = c.F(ag + "kv_b"); q.out = kv; c.gemm(q); }
-      }
-      float* q = ar.f(static_cast<size_t>(R4) * hid);
-      c.small_linear(xn, R4, hid, c.F(ag + "q_w"), hid, c.F(ag + "q_b"), UDB_ACT_NONE, nullptr, nullptr, q);
-      float* at = ar.f(static_cast<size_t>(R4) * hid);
-      float* scratch = ar.f(static_cast<size_t>(B) * 16 * 4 * (hid + 2));
-      const float* cam_pos = c.F("cam.pos");
-      c.launch([&] {
-        const float scale = 1.0f / sqrtf(static_cast<float>(hid));
-        return sp ? udb_cross_attn_small_f32(q, cam_pos, static_cast<const float*>(kv), at, scratch, B, 4, 4 * nq + 4, hid, scale, st)
-                  : udb_cross_attn_small(q, cam_pos, kv, at, scratch, B, 4, 4 * nq + 4, hid, scale, st);
-      });
-      float* t2 = ar.f(static_cast<size_t>(R4) * hid);
-      c.small_linear(at, R4, hid, c.F(ag + "out_w"), hid, c.F(ag + "out_b"), UDB_ACT_NONE, c.F(ag + "ls1"), cl, t2);
-      t = cam_mlp(c, ag + "mlp", t2, R4, hid, cf.expansion * hid, hid, t2, c.F(ag + "ls2"));
-    }
+    float* t = small_cross_block(c, "cam.agg.", cl, B, 4, ctx, 4LL * nq + 4, c.F("cam.pos"), hid, cf.expansion, sp);
     for (int i = 0; i < 2; ++i) {
       const std::string ly = idx("cam.l%d.", i);
       float* xn = ar.f(static_cast<size_t>(R4) * hid);
@@ -475,16 +355,13 @@ static int run_v1(udb_engine_v1* e, const udb_infer_v1_args_t& a, Arena& ar, voi
       c.small_linear(a4, R4, hid, c.F(ly + "out_w"), hid, c.F(ly + "out_b"), UDB_ACT_NONE, c.F(ly + "ls1"), t, t2);
       t = cam_mlp(c, ly + "mlp", t2, R4, hid, cf.expansion * hid, hid, t2, c.F(ly + "ls2"));
     }
-    float* xo = cam_mlp(c, "cam.out", t, R4, hid, 2 * hid, 1, nullptr, nullptr);       // [B*4, 1] == [B, 4]
-    // the result must survive the release below: copy into a slot allocated before the mark is not possible with a bump
-    // arena, so keep the camera scratch alive instead (0.3 GB at B=16) -- x4 points into it
-    x4 = xo;
-    (void)m;
+    x4 = cam_mlp(c, "cam.out", t, R4, hid, 2 * hid, 1, nullptr, nullptr);       // [B*4, 1] == [B, 4]
   }
   c.launch([&] {
     return udb_v1_camera_intrinsics(x4, a.intrinsics, B, net_h, net_w, static_cast<float>(g.ratio), g.pad_l, g.pad_t, a.skip_camera,
                                     intr4, a.out_intrinsics, k4_points, st);
   });
+  ar.release(cam_mark);
 
   // ---- ray embeddings at the three decoder levels (decoder.py:203-220)
   stage.next("udb_v1:ray_embeddings");

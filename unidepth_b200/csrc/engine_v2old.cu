@@ -1,7 +1,8 @@
 // Whole-path engine for UniDepthV2old.infer (DINOv2 ViT-L/14 or ViT-S/14) behind udb_v2old_create / udb_v2old_set_weight /
 // udb_v2old_workspace_bytes / udb_infer_v2old (include/udb.h).  Host-side schedule only, on the skeleton of the other two
-// engines (engine_common.h): the shared DINOv2 block loop, V1's decoder blocks (adapters, dense and Nystrom attention,
-// ConvNeXt blocks, the camera head's cross attention) and the V2old kernels of v1_kernels.cu.  Reference call stack:
+// engines (engine_common.h): the shared DINOv2 patch embedding and block loop, V1's decoder stages (adapters, cls-token
+// adapters, camera context, dense and Nystrom attention, ConvNeXt blocks, the heads' cross attention) and the V2old kernels
+// of v1_kernels.cu.  Reference call stack:
 //   UniDepthV2old.infer              unidepth/models/unidepthv2/unidepthv2_old.py:198-282 (_shapes/_preprocess/_postprocess :33-116)
 //     pixel_encoder = DINOv2         backbones/dinov2.py:324-347 (use_norm: every block output through the final norm)
 //     pixel_decoder = Decoder        unidepthv2/decoder_old.py:428-522 (CameraHead :32-86, GlobalHead :89-146,
@@ -32,70 +33,6 @@ static udb_v2old_geometry_t v2old_geometry(int H, int W, int level, int lo, int 
   return g;
 }
 
-// AttentionBlock with one head over a long f16 context and at most four queries (decoder_old.py:72-77, 142-143): the camera
-// head's and the global head's aggregate blocks, on V1's split-key cross attention.  x f32 [B*nq, hid] -> new f32 rows.
-// Split mode (`sp`): the context is f32, its LayerNorm writes a split operand for the kv GEMM ([2*hid, 3*hid] weight), and
-// the attention reads f32 (k | v) rows, as V1's split camera head.
-static float* small_cross_block(Ctx& c, const std::string& p, const float* x, int B, int nq, const void* ctx, long long nk,
-                                const float* q_pos, int hid, int expansion, bool sp) {
-  Arena& ar = *c.ar;
-  const int R = B * nq;
-  const long long Rc = static_cast<long long>(B) * nk;
-  float* xn = ar.f(static_cast<size_t>(R) * hid);
-  float* q = ar.f(static_cast<size_t>(R) * hid);
-  float* at = ar.f(static_cast<size_t>(R) * hid);
-  float* scratch = ar.f(static_cast<size_t>(B) * 16 * 4 * (hid + 2));
-  c.layernorm(x, 1, xn, 1, c.F(p + "nxw"), c.F(p + "nxb"), R, hid, 1e-5f);
-  c.small_linear(xn, R, hid, c.F(p + "q_w"), hid, c.F(p + "q_b"), UDB_ACT_NONE, nullptr, nullptr, q);
-  const size_t m = ar.mark();          // the normalised context and its (k | v) rows: dead once the attention has run
-  void* kv;
-  if (sp) {
-    __half* cn = ar.h(Rc * 2 * hid);
-    c.ln_any(ctx, 1, cn, UDB_LN_OUT_SPLIT, c.F(p + "ncw"), c.F(p + "ncb"), Rc, hid, 1e-5f, 2 * hid);
-    kv = ar.f(Rc * 2 * hid);
-    c.expect2(p + "kv_w", 2 * hid, 3 * hid);
-    Ctx::G g{cn, c.H(p + "kv_w"), static_cast<int>(Rc), 2 * hid, 3 * hid}; g.lda = 2 * hid; g.a_split_k = hid;
-    g.bias = c.F(p + "kv_b"); g.out = kv; g.out_f32 = 1; c.gemm(g);
-  } else {
-    __half* cn = ar.h(Rc * hid);
-    ln16(c, ctx, 0, cn, p + "ncw", p + "ncb", Rc, hid, 1e-5f);
-    kv = ar.h(Rc * 2 * hid);
-    Ctx::G g{cn, c.H(p + "kv_w"), static_cast<int>(Rc), 2 * hid, hid}; g.bias = c.F(p + "kv_b"); g.out = kv; c.gemm(g);
-  }
-  c.launch([&] {
-    const float scale = 1.0f / sqrtf(static_cast<float>(hid));
-    return sp ? udb_cross_attn_small_f32(q, q_pos, static_cast<const float*>(kv), at, scratch, B, nq, static_cast<int>(nk), hid, scale, c.st)
-              : udb_cross_attn_small(q, q_pos, kv, at, scratch, B, nq, static_cast<int>(nk), hid, scale, c.st);
-  });
-  ar.release(m);
-  float* t2 = xn;
-  c.small_linear(at, R, hid, c.F(p + "out_w"), hid, c.F(p + "out_b"), UDB_ACT_NONE, c.F(p + "ls1"), x, t2);
-  return cam_mlp(c, p + "mlp", t2, R, hid, expansion * hid, hid, t2, c.F(p + "ls2"));
-}
-
-// The n head tokens x f32 [B*n, hid] into rows [row0, row0 + n) of each image's nk context rows: f16, or f32 in split mode
-static void copy_cls_rows(Ctx& c, const float* x, void* ctx, int B, int n, int hid, long long nk, long long row0, bool sp) {
-  c.launch([&] {
-    if (!sp) return udb_copy_rows_f32_to_f16(x, ctx, B, n, hid, nk, row0, c.st);
-    const size_t row = sizeof(float) * hid;
-    return cuda_rc(cudaMemcpy2DAsync(static_cast<float*>(ctx) + row0 * hid, nk * row, x, n * row, n * row, B,
-                                     cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(c.st)),
-                   "engine_v2old: copying the head tokens into the f32 context");
-  });
-}
-
-// f32 [R, D] rows of `n` cls tokens -> LN + Linear + GELU per token (ListAdapter, decoder_old.py:13-29) -> f32 [B, n, hid]
-static float* token_adapter(Ctx& c, const std::string& p, float* const* cls, int n, int B, int D, int hid) {
-  float* toks = c.ar->f(static_cast<size_t>(B) * n * hid);
-  for (int i = 0; i < n; ++i) {
-    const std::string tk = p + idx("%d.", i);
-    float* t = c.ar->f(static_cast<size_t>(B) * D);
-    c.ln_any(cls[i], 1, t, 1, c.F(tk + "ln_w"), c.F(tk + "ln_b"), B, D, 1e-5f);
-    c.small_linear(t, B, D, c.F(tk + "w"), hid, c.F(tk + "b"), UDB_ACT_GELU, nullptr, nullptr, toks + i * hid, D, n * hid, 0);
-  }
-  return toks;
-}
-
 static int run_v2old(udb_engine_v2old* e, const udb_infer_v2old_args_t& a, Arena& ar, void* st) {
   const udb_v2old_config_t& cf = e->cfg;
   Ctx c{e, &ar, st, ar.dry};
@@ -117,19 +54,12 @@ static int run_v2old(udb_engine_v2old* e, const udb_infer_v2old_args_t& a, Arena
   // head's in_features and kv, the global head's project_rays, in_features and kv -- multiplies [hi | lo] operands with
   // [hi | hi | lo] weights; the taps and the two heads' contexts are f32.  The depth head reads the hi half of the
   // adapters' LayerNorm and of the first level's ray features and runs as in the f16 mode.
-  const double prec = e->scalars.count("precision") ? e->scalars["precision"] : 0.0;
-  if (prec != 0.0 && prec != 1.0 && prec != 2.0) { set_error("udb_infer_v2old: precision %g unsupported (0 f16, 1 split f16, 2 e4m3)", prec); return 1; }
-  const bool f8 = prec == 2.0, sp = prec == 1.0;
+  const Precision prec = encoder_precision(c, "udb_infer_v2old", "patch_w", 3 * 640);
+  if (prec == PREC_BAD) return 1;
+  const bool sp = prec == PREC_SPLIT;
   const int sx = sp ? 2 : 1;          // columns of a split operand per logical column
   const int kx = sp ? 3 : 1;          // columns of a split weight per logical column
-  if (sp) {   // an f16 packing registered with precision 1 is named for what it is, not only by its first mis-shaped operand
-    const Weight* w = c.W("patch_w");
-    if (!c.rc && (w->ndim != 2 || w->shape[1] != 3 * 640)) {
-      set_error("udb_infer_v2old: precision 1 (split f16) needs the split packing: 'patch_w' has %lld columns, expected %d",
-                static_cast<long long>(w->shape[1]), 3 * 640);
-      return 1;
-    }
-  }
+  const int widths[4] = {D, D, D, D}; // of every tap and cls token
   Stage stage;
 
   // ---- pre-processing + patch embedding (unidepthv2_old.py:211-230: /255, ImageNet normalisation, antialiased resize)
@@ -151,21 +81,11 @@ static int run_v2old(udb_engine_v2old* e, const udb_infer_v2old_args_t& a, Arena
       c.launch([&] { return sp ? udb_v1_preprocess_split(&p, st) : udb_v1_preprocess(&p, st); });
     }
     float* x = ar.f(BT * D);
-    c.expect2("patch_w", D, 640 * kx);
-    c.expect2("pos", T, D);
-    {
-      const float* pos = c.F("pos");
-      const float* clsw = c.F("cls");
-      Ctx::G q{patches, c.H("patch_w"), static_cast<int>(BN), D, 640 * kx};
-      q.lda = 640 * sx; q.a_split_k = sp ? 640 : 0;
-      q.bias = c.F("patch_b"); q.resid = pos; q.resid_f32 = 1; q.ldr = D; q.out = x; q.out_f32 = 1;
-      q.rows_per_group = N; q.group_stride = T; q.row_offset = 1; q.resid_mod = N; q.resid_row_offset = 1;
-      c.gemm(q);
-      c.launch([&] { return udb_set_cls_rows(x, clsw, pos, B, T, D, st); });
-    }
     VitBlocks v{B, T, D, cf.enc_heads, cf.enc_depth};
-    v.fp8 = f8;
+    v.fp8 = prec == PREC_E4M3;
     v.split = sp;
+    c.expect2("pos", T, D);
+    vit_embed(c, patches, c.F("pos"), x, v);
     int tap = 0;
     vit_blocks(c, "blocks.", x, v, [&](int i) {
       if (tap < 4 && i + 1 == cf.output_idx[tap]) {
@@ -187,28 +107,8 @@ static int run_v2old(udb_engine_v2old* e, const udb_infer_v2old_args_t& a, Arena
   // operand for the global head's in_features GEMM (the depth head keeps the f16 tokens)
   float* head_tokens = sp ? ar.f(Rq * 4 * hid) : nullptr;
   __half* head_tokens2 = sp ? ar.h(Rq * 4 * 2 * hid) : nullptr;
-  for (int l = 0; l < 4; ++l) {
-    const size_t m = ar.mark();
-    const std::string ad = idx("adapt.%d.", l);
-    __half* an = ar.h(Rq * D * sx);
-    if (sp) c.ln_any(feats[l], 1, an, UDB_LN_OUT_SPLIT, c.F(ad + "ln_w"), c.F(ad + "ln_b"), Rq, D, 1e-5f, 2 * D);
-    else ln16(c, feats[l], 0, an, ad + "ln_w", ad + "ln_b", Rq, D, 1e-5f);
-    { Ctx::G q{an, c.H(ad + "w"), static_cast<int>(Rq), hid, D}; q.lda = D * sx; q.bias = c.F(ad + "b"); q.act = UDB_ACT_GELU; q.out = tokens;
-      q.rows_per_group = nq; q.group_stride = 4 * nq; q.row_offset = l * nq; c.gemm(q); }
-    { Ctx::G q{an, c.H(ad + "w"), static_cast<int>(Rq), hid, D}; q.lda = D * sx; q.bias = c.F(ad + "b"); q.act = UDB_ACT_GELU;
-      q.out = featcat + l * hid; q.ldc = 4 * hid; c.gemm(q); }
-    if (sp) {
-      c.expect2(ad + "w_cam", hid, 3 * D);
-      for (int k = 0; k < 2; ++k) {
-        Ctx::G q{an, c.H(ad + "w_cam"), static_cast<int>(Rq), hid, 3 * D}; q.lda = 2 * D; q.a_split_k = D; q.bias = c.F(ad + "b");
-        q.act = UDB_ACT_GELU; q.rows_per_group = nq; q.group_stride = 4 * nq; q.row_offset = l * nq;
-        if (k == 0) { q.out = head_tokens; q.out_f32 = 1; }
-        else { q.out = head_tokens2; q.ldc = 2 * hid; q.out_split = hid; }
-        c.gemm(q);
-      }
-    }
-    ar.release(m);
-  }
+  const int grid_h[4] = {gh, gh, gh, gh}, grid_w[4] = {gw, gw, gw, gw};
+  adapters(c, feats, widths, grid_h, grid_w, B, gh, gw, hid, sp, tokens, featcat, head_tokens, head_tokens2);
   const float* tokens_pos = c.F("tokens_pos");         // [4*nq, hid]: sine position + level embedding (decoder_old.py:463-479)
   c.expect2("tokens_pos", 4LL * nq, hid);
 
@@ -219,32 +119,9 @@ static int run_v2old(udb_engine_v2old* e, const udb_infer_v2old_args_t& a, Arena
   {
     const size_t m = ar.mark();
     const int R4 = B * 4;
-    float* toks = token_adapter(c, "ctok.", cls, 4, B, D, hid);
+    float* toks = token_adapter(c, "ctok.", cls, widths, 4, B, hid);
     float* cl = cam_mlp(c, "cam.cls", toks, R4, hid, 4 * hid, hid, nullptr, nullptr);
-    const long long Rc = static_cast<long long>(B) * (4 * nq + 4);
-    void* ctx = ar.alloc(Rc * hid * (sp ? 4 : 2));            // f16, or f32 in split mode
-    {
-      const size_t m2 = ar.mark();
-      __half* a1 = ar.h(Rq * 4 * hid * sx);
-      __half* m1 = ar.h(Rq * 4 * 2 * hid * sx);
-      if (sp) {
-        c.expect2("cam.inf.w1", 2 * hid, 3 * hid);
-        c.expect2("cam.inf.w2", hid, 6 * hid);
-        c.ln_any(head_tokens, 1, a1, UDB_LN_OUT_SPLIT, c.F("cam.inf.nw"), c.F("cam.inf.nb"), Rq * 4, hid, 1e-5f, 2 * hid, tokens_pos, 4LL * nq);
-        { Ctx::G q{a1, c.H("cam.inf.w1"), static_cast<int>(Rq * 4), 2 * hid, 3 * hid}; q.lda = 2 * hid; q.a_split_k = hid;
-          q.bias = c.F("cam.inf.b1"); q.act = UDB_ACT_GELU; q.out = m1; q.ldc = 4 * hid; q.out_split = 2 * hid; c.gemm(q); }
-        { Ctx::G q{m1, c.H("cam.inf.w2"), static_cast<int>(Rq * 4), hid, 6 * hid}; q.lda = 4 * hid; q.a_split_k = 2 * hid;
-          q.bias = c.F("cam.inf.b2"); q.out = ctx; q.out_f32 = 1; q.rows_per_group = 4 * nq; q.group_stride = 4 * nq + 4; q.row_offset = 0;
-          c.gemm(q); }
-      } else {
-        c.ln_any(tokens, 0, a1, 0, c.F("cam.inf.nw"), c.F("cam.inf.nb"), Rq * 4, hid, 1e-5f, 0, tokens_pos, 4LL * nq);
-        { Ctx::G q{a1, c.H("cam.inf.w1"), static_cast<int>(Rq * 4), 2 * hid, hid}; q.bias = c.F("cam.inf.b1"); q.act = UDB_ACT_GELU; q.out = m1; c.gemm(q); }
-        { Ctx::G q{m1, c.H("cam.inf.w2"), static_cast<int>(Rq * 4), hid, 2 * hid}; q.bias = c.F("cam.inf.b2"); q.out = ctx;
-          q.rows_per_group = 4 * nq; q.group_stride = 4 * nq + 4; q.row_offset = 0; c.gemm(q); }
-      }
-      ar.release(m2);
-    }
-    copy_cls_rows(c, cl, ctx, B, 4, hid, 4LL * nq + 4, 4LL * nq, sp);
+    const void* ctx = camera_context(c, sp ? static_cast<const void*>(head_tokens) : tokens, tokens_pos, cl, B, nq, 4, hid, sp);
     const float* cam_pos = c.F("cam.pos");
     float* t = small_cross_block(c, "cam.agg1.", cl, B, 4, ctx, 4LL * nq + 4, cam_pos, hid, cf.expansion, sp);
     t = small_cross_block(c, "cam.agg2.", t, B, 4, ctx, 4LL * nq + 4, cam_pos, hid, cf.expansion, sp);
@@ -280,7 +157,7 @@ static int run_v2old(udb_engine_v2old* e, const udb_infer_v2old_args_t& a, Arena
     const size_t m = ar.mark();
     const int R2 = B * 2;
     float* gtok[2] = {cls[1], cls[2]};
-    float* toks = token_adapter(c, "gtok.", gtok, 2, B, D, hid);
+    float* toks = token_adapter(c, "gtok.", gtok, widths, 2, B, hid);
     float* gcl = cam_mlp(c, "glob.cls", toks, R2, hid, 4 * hid, hid, nullptr, nullptr);
     // in_features(features + project_rays(rays)) = W_in features + (W_in project_rays(rays) + b_in), the second term per
     // token of the grid and shared by the four levels
