@@ -795,6 +795,17 @@ typedef struct udb_infer_v2old_args_t {
   float* out_points;       /* [B,3,H,W] */
   float* out_depth;        /* [B,1,H,W] */
   float* out_confidence;   /* [B,1,H,W] */
+  /* Network-only mode (the reference's `forward(inputs, image_metas)`, unidepthv2_old.py:134-196), selected by
+   * network_only = 1; all zero gives `infer` as above.  `rgb` is the network input itself: f32 (rgb_is_u8, scale255
+   * and normalize 0), already normalised, with (H, W) the engine's network shape, else a named error before any launch.
+   * The ratio is 1: a given K drives the rays as it is, and must then come with (out_h, out_w) == (H, W).  `interpolation`
+   * is not read.  Outputs: out_intrinsics the predicted K (also when K is given); out_depth and out_confidence
+   * [B,1,out_h,out_w], antialiased bilinear from the network shape; out_points [B,3,out_h,out_w] through the predicted K
+   * on the out_h x out_w grid. */
+  int32_t network_only;
+  int32_t out_h, out_w;    /* network-only: size of the depth, confidence and points outputs */
+  float* out_depth_features; /* network-only, optional: [B, (H/14)*(W/14), hidden] f32 latents of the depth head after
+                                aggregate_16 and prompt_camera, before the Nystrom blocks */
 } udb_infer_v2old_args_t;
 
 int udb_infer_v2old(udb_engine_v2old* e, const udb_infer_v2old_args_t* a, void* stream);
@@ -824,6 +835,7 @@ typedef struct udb_v2old_postprocess_t {
   float* out_depth;        /* [B,1,H,W] */
   float* out_confidence;   /* [B,1,H,W] antialiased bilinear */
   float* out_points;       /* [B,3,H,W] */
+  int32_t depth_aa;        /* 1: depth with antialiased bilinear, as the confidence (`mode` is then not read) */
 } udb_v2old_postprocess_t;
 int udb_v2old_postprocess(const udb_v2old_postprocess_t* p, void* stream);
 /* x4 [B,4] camera-head output -> intr4_rays [B,4] (gt_k * ratio, else the prediction at the network shape), k_out [B,3,3]

@@ -193,6 +193,7 @@ class InferV2oldArgs(C.Structure):
         ("rgb", vp), ("rgb_is_u8", i32), ("scale255", i32), ("normalize", i32), ("B", i32), ("H", i32), ("W", i32),
         ("intrinsics", vp), ("interpolation", i32), ("workspace", vp), ("workspace_bytes", C.c_size_t),
         ("out_intrinsics", vp), ("out_points", vp), ("out_depth", vp), ("out_confidence", vp),
+        ("network_only", i32), ("out_h", i32), ("out_w", i32), ("out_depth_features", vp),
     ]
 
 
@@ -203,7 +204,7 @@ class V2oldHeads(C.Structure):
 
 class V2oldPostprocess(C.Structure):
     _fields_ = [("depth", vp), ("confidence", vp), ("k4", vp), ("B", i32), ("net_h", i32), ("net_w", i32), ("H", i32), ("W", i32),
-                ("mode", i32), ("out_depth", vp), ("out_confidence", vp), ("out_points", vp)]
+                ("mode", i32), ("out_depth", vp), ("out_confidence", vp), ("out_points", vp), ("depth_aa", i32)]
 
 
 class NearestNeighbor(C.Structure):

@@ -242,11 +242,12 @@ class EngineModel(nn.Module):
         return ws
 
     # ------------------------------------------------------------------ CUDA graphs
-    def _run_graphed(self, run, rgb: torch.Tensor, inputs: dict, key: tuple, keep=None) -> dict:
+    def _run_graphed(self, run, rgb: torch.Tensor, inputs: dict, key: tuple, keep=None, output_buffers: bool = True) -> dict:
         """`run(rgb, inputs)` -> outputs, eagerly or by replaying a CUDA graph cached under `key`.  The caller packs the
         weights (`_weights()`) before this: a repack drops every graph, so none replays stale weights.  The graph reads
         static copies of `rgb` and of the tensors in `inputs`, refreshed before every replay; `keep` is anything else a
-        captured kernel reads, which the cache entry must own."""
+        captured kernel reads, which the cache entry must own.  `output_buffers=False`: return fresh tensors even when
+        `self.output_buffers` is set (it holds `infer`'s outputs only)."""
         if not self.use_cuda_graph:
             return run(rgb, inputs)
         entry = self._graphs.get(key)
@@ -273,7 +274,7 @@ class EngineModel(nn.Module):
         for k, v in inputs.items():
             entry["inputs"][k].copy_(v, non_blocking=True)
         entry["graph"].replay()
-        bufs = self.output_buffers
+        bufs = self.output_buffers if output_buffers else None
         if bufs is not None:       # caller-provided destinations (e.g. the send slot of parallel.PeerGather): one copy, no clone
             for k, v in entry["out"].items():
                 bufs[k].copy_(v)

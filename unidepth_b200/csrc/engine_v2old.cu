@@ -1,8 +1,8 @@
-// Whole-path engine for UniDepthV2old.infer (DINOv2 ViT-L/14 or ViT-S/14) behind udb_v2old_create / udb_v2old_set_weight /
-// udb_v2old_workspace_bytes / udb_infer_v2old (include/udb.h).  Host-side schedule only, on the skeleton of the other two
-// engines (engine_common.h): the shared DINOv2 patch embedding and block loop, V1's decoder stages (adapters, cls-token
-// adapters, camera context, dense and Nystrom attention, ConvNeXt blocks, the heads' cross attention) and the V2old kernels
-// of v1_kernels.cu.  Reference call stack:
+// Whole-path engine for UniDepthV2old.infer and the evaluation .forward (DINOv2 ViT-L/14 or ViT-S/14) behind
+// udb_v2old_create / udb_v2old_set_weight / udb_v2old_workspace_bytes / udb_infer_v2old (include/udb.h).  Host-side
+// schedule only, on the skeleton of the other two engines (engine_common.h): the shared DINOv2 patch embedding and block
+// loop, V1's decoder stages (adapters, cls-token adapters, camera context, dense and Nystrom attention, ConvNeXt blocks,
+// the heads' cross attention) and the V2old kernels of v1_kernels.cu.  Reference call stack:
 //   UniDepthV2old.infer              unidepth/models/unidepthv2/unidepthv2_old.py:198-282 (_shapes/_preprocess/_postprocess :33-116)
 //     pixel_encoder = DINOv2         backbones/dinov2.py:324-347 (use_norm: every block output through the final norm)
 //     pixel_decoder = Decoder        unidepthv2/decoder_old.py:428-522 (CameraHead :32-86, GlobalHead :89-146,
@@ -40,7 +40,9 @@ static int run_v2old(udb_engine_v2old* e, const udb_infer_v2old_args_t& a, Arena
   const int gh = net_h / 14, gw = net_w / 14, N = gh * gw, T = N + 1, nq = N;
   const size_t BN = static_cast<size_t>(B) * N, BT = static_cast<size_t>(B) * T;
   const long long Rq = static_cast<long long>(B) * nq;
-  const double ratio = static_cast<double>(gh) / a.H * 14;     // unidepthv2_old.py:88
+  // network-only mode (`forward`, unidepthv2_old.py:134-196): the input is the network input and the ratio 1
+  const bool net_only = a.network_only != 0;
+  const double ratio = net_only ? 1.0 : static_cast<double>(gh) / a.H * 14;     // unidepthv2_old.py:88
   // Nystrom attention with 128 landmarks at the first decoder level needs more tokens than landmarks, and the heads'
   // cross attention has a shared-memory bound: both named by the dry run before anything is launched
   if (nq <= 128) {
@@ -126,9 +128,17 @@ static int run_v2old(udb_engine_v2old* e, const udb_infer_v2old_args_t& a, Arena
     float* t = small_cross_block(c, "cam.agg1.", cl, B, 4, ctx, 4LL * nq + 4, cam_pos, hid, cf.expansion, sp);
     t = small_cross_block(c, "cam.agg2.", t, B, 4, ctx, 4LL * nq + 4, cam_pos, hid, cf.expansion, sp);
     float* x4 = cam_mlp(c, "cam.out", t, R4, hid, 2 * hid, 1, nullptr, nullptr);     // [B*4, 1] == [B, 4]
-    c.launch([&] {
-      return udb_v2old_camera(x4, a.intrinsics, B, net_h, net_w, static_cast<float>(ratio), intr4, a.out_intrinsics, k4_points, st);
-    });
+    if (net_only && a.intrinsics) {
+      // `forward` with K: the rays follow the given K, the points the prediction (unidepthv2_old.py:154-159).  At ratio 1
+      // the kernel writes the same values to its rays and points outputs, so each call passes one buffer for both: the
+      // prediction into k4_points, then the given K into intr4.  out_intrinsics is the prediction in both calls.
+      c.launch([&] { return udb_v2old_camera(x4, nullptr, B, net_h, net_w, 1.f, k4_points, a.out_intrinsics, k4_points, st); });
+      c.launch([&] { return udb_v2old_camera(x4, a.intrinsics, B, net_h, net_w, 1.f, intr4, a.out_intrinsics, intr4, st); });
+    } else {
+      c.launch([&] {
+        return udb_v2old_camera(x4, a.intrinsics, B, net_h, net_w, static_cast<float>(ratio), intr4, a.out_intrinsics, k4_points, st);
+      });
+    }
     ar.release(m);
   }
 
@@ -216,6 +226,11 @@ static int run_v2old(udb_engine_v2old* e, const udb_infer_v2old_args_t& a, Arena
   }
   dense_attn_block(c, "agg16.", lat, B, nq, hid, tokens, 0, 4 * nq, tokens_pos);
   dense_attn_block(c, "prompt.", lat, B, nq, hid, emb[0], 1, nq, nullptr);
+  if (a.out_depth_features)          // `forward`'s "depth_features" (decoder_old.py:339-343)
+    c.launch([&] {
+      return cuda_rc(cudaMemcpyAsync(a.out_depth_features, lat, sizeof(float) * Rq * hid, cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(st)),
+                     "engine_v2old: copying the depth features");
+    });
   for (int i = 0; i < cf.nystrom_depth; ++i) mh_attn_block(c, idx("nys.%d.", i), lat, B, nq, hid, cf.heads, emb[0], true);
 
   // ConvUpsampleShuffleResidual per level (layers/upsample.py:82-130), then the level's [depth | confidence] MLPs
@@ -276,8 +291,10 @@ static int run_v2old(udb_engine_v2old* e, const udb_infer_v2old_args_t& a, Arena
   {
     udb_v2old_postprocess_t p;
     memset(&p, 0, sizeof(p));
-    p.depth = dmap; p.confidence = cmap; p.k4 = k4_points; p.B = B; p.net_h = net_h; p.net_w = net_w; p.H = a.H; p.W = a.W;
+    p.depth = dmap; p.confidence = cmap; p.k4 = k4_points; p.B = B; p.net_h = net_h; p.net_w = net_w;
+    p.H = net_only ? a.out_h : a.H; p.W = net_only ? a.out_w : a.W;
     p.mode = a.interpolation; p.out_depth = a.out_depth; p.out_confidence = a.out_confidence; p.out_points = a.out_points;
+    p.depth_aa = net_only ? 1 : 0;
     c.launch([&] { return udb_v2old_postprocess(&p, st); });
   }
   if (!c.rc && ar.overflow) { set_error("engine_v2old: workspace too small (%zu bytes needed)", ar.peak); return 1; }
@@ -357,9 +374,32 @@ int udb_infer_v2old(udb_engine_v2old* e, const udb_infer_v2old_args_t* a, void* 
     set_error("udb_infer_v2old: all four output pointers are required");
     return 1;
   }
-  if (a->interpolation != UDB_V2OLD_BILINEAR && a->interpolation != UDB_V2OLD_NEAREST_EXACT) {
+  if (!a->network_only && a->interpolation != UDB_V2OLD_BILINEAR && a->interpolation != UDB_V2OLD_NEAREST_EXACT) {
     set_error("udb_infer_v2old: `interpolation` %d is neither UDB_V2OLD_BILINEAR (0) nor UDB_V2OLD_NEAREST_EXACT (1)", a->interpolation);
     return 1;
+  }
+  if (a->network_only != 0 && a->network_only != 1) { set_error("udb_infer_v2old: `network_only` %d is neither 0 nor 1", a->network_only); return 1; }
+  if (!a->network_only && (a->out_h || a->out_w || a->out_depth_features)) {
+    set_error("udb_infer_v2old: out_h, out_w and out_depth_features are read in network-only mode only (network_only = 1)");
+    return 1;
+  }
+  if (a->network_only) {
+    const udb_v2old_config_t& cf = e->cfg;
+    if (a->rgb_is_u8 || a->scale255 || a->normalize) {
+      set_error("udb_infer_v2old: network-only input must be f32 and already normalised (rgb_is_u8 %d, scale255 %d, normalize %d must be 0)",
+                a->rgb_is_u8, a->scale255, a->normalize);
+      return 1;
+    }
+    if (a->H != cf.net_h || a->W != cf.net_w) {
+      set_error("udb_infer_v2old: network-only input is %dx%d but the engine's network shape is %dx%d", a->H, a->W, cf.net_h, cf.net_w);
+      return 1;
+    }
+    if (a->out_h < 1 || a->out_w < 1) { set_error("udb_infer_v2old: network-only output size %dx%d must be positive", a->out_h, a->out_w); return 1; }
+    if (a->intrinsics && (a->out_h != a->H || a->out_w != a->W)) {
+      set_error("udb_infer_v2old: a given K needs the output size %dx%d to equal the network input's %dx%d (the reference reshapes "
+                "its rays to the image grid)", a->out_h, a->out_w, a->H, a->W);
+      return 1;
+    }
   }
   if (e->check_workspace("udb_infer_v2old", "udb_v2old_workspace_bytes", shape_name(a->B, a->H, a->W), a->workspace, a->workspace_bytes))
     return 1;

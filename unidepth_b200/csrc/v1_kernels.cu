@@ -1668,11 +1668,27 @@ __global__ void __launch_bounds__(1024) v2old_depth_tail_kernel(float* __restric
   }
 }
 
+// One output pixel of an antialiased bilinear resize of the row-major map m (row length ld) from the axes' weights.  The
+// confidence in v2old_postprocess_kernel keeps its own copy of this loop, so that `infer`'s code is unchanged.
+__device__ __forceinline__ float aa_sample(const float* __restrict__ m, const AAxis& ay, const AAxis& ax, int ld) {
+  float v = 0.f;
+  for (int jy = 0; jy < ay.xsize; ++jy) {
+    float r = 0.f;
+    for (int jx = 0; jx < ax.xsize; ++jx) r += ax.w(jx) * m[(long long)(ay.xmin + jy) * ld + ax.xmin + jx];
+    v += ay.w(jy) * r;
+  }
+  return v;
+}
+
 // Output assembly at the input size (unidepthv2_old.py:107-116,267-274): depth resized from the network shape with
 // bilinear (align_corners=False, no antialias) or nearest-exact, confidence with antialiased bilinear (aa_axis), and the
 // points z * (tan(theta), 1 / tan(phi) / cos(theta), 1) of the unit ray of each input pixel through k4 (fx, fy, cx, cy).
+// DEPTH_AA (depth_aa) resizes the depth with antialiased bilinear too, as the reference's `forward` does
+// (unidepthv2_old.py:166-179); at equal sizes the weights are (1, 0) and the depth is copied bit for bit.  A template
+// argument, so that the code of the two `infer` modes is exactly what it was without it.
 // V1's post-processing crops paddings and resizes depth with antialias only; V2's assembles radius-based points from
 // padded maps; neither resizes with these two modes.
+template <bool DEPTH_AA>
 __global__ void __launch_bounds__(256) v2old_postprocess_kernel(const udb_v2old_postprocess_t p) {
   const long long total = (long long)p.B * p.H * p.W;
   const float sh = (float)p.net_h / (float)p.H, sw = (float)p.net_w / (float)p.W;
@@ -1681,7 +1697,9 @@ __global__ void __launch_bounds__(256) v2old_postprocess_kernel(const udb_v2old_
     const long long nhw = (long long)p.net_h * p.net_w;
     const float* dm = p.depth + b * nhw;
     float z;
-    if (p.mode == UDB_V2OLD_NEAREST_EXACT) {
+    if (DEPTH_AA) {
+      z = aa_sample(dm, aa_axis(Y, p.net_h, sh), aa_axis(X, p.net_w, sw), p.net_w);
+    } else if (p.mode == UDB_V2OLD_NEAREST_EXACT) {
       const int yi = min((int)floorf(((float)Y + 0.5f) * sh), p.net_h - 1), xi = min((int)floorf(((float)X + 0.5f) * sw), p.net_w - 1);
       z = dm[(long long)yi * p.net_w + xi];
     } else {
@@ -1790,7 +1808,8 @@ int udb_v2old_postprocess(const udb_v2old_postprocess_t* p, void* stream) {
   const struct { int v; const char* name; } dims[] = {{p->B, "B"}, {p->H, "H"}, {p->W, "W"}, {p->net_h, "net_h"}, {p->net_w, "net_w"}};
   for (const auto& d : dims)
     if (d.v < 1) { set_error("udb_v2old_postprocess: %s=%d must be >= 1", d.name, d.v); return 1; }
-  if (p->mode != UDB_V2OLD_BILINEAR && p->mode != UDB_V2OLD_NEAREST_EXACT) {
+  if (p->depth_aa != 0 && p->depth_aa != 1) { set_error("udb_v2old_postprocess: `depth_aa` %d is neither 0 nor 1", p->depth_aa); return 1; }
+  if (!p->depth_aa && p->mode != UDB_V2OLD_BILINEAR && p->mode != UDB_V2OLD_NEAREST_EXACT) {
     set_error("udb_v2old_postprocess: `mode` %d is neither UDB_V2OLD_BILINEAR (0) nor UDB_V2OLD_NEAREST_EXACT (1)", p->mode);
     return 1;
   }
@@ -1799,7 +1818,8 @@ int udb_v2old_postprocess(const udb_v2old_postprocess_t* p, void* stream) {
                                                              {p->out_points, "out_points"}};
   for (const auto& a : ptrs)
     if (!a.q) { set_error("udb_v2old_postprocess: `%s` must be non-null", a.name); return 1; }
-  v2old_postprocess_kernel<<<grid_1d((long long)p->B * p->H * p->W), 256, 0, ST(stream)>>>(*p);
+  if (p->depth_aa) v2old_postprocess_kernel<true><<<grid_1d((long long)p->B * p->H * p->W), 256, 0, ST(stream)>>>(*p);
+  else v2old_postprocess_kernel<false><<<grid_1d((long long)p->B * p->H * p->W), 256, 0, ST(stream)>>>(*p);
   return check_launch("v2old_postprocess_kernel");
 }
 

@@ -1,15 +1,16 @@
 """UniDepthV2old (DINOv2 ViT-L/14 or ViT-S/14 encoder) -- drop-in for the reference's inference API, running on libudb.so
 (sm_90a).
 
-Mirrors `unidepth.models.unidepthv2.unidepthv2_old.UniDepthV2old` for the inference path only (reference:
-unidepth/models/unidepthv2/unidepthv2_old.py:126-132 constructor, :198-282 `infer`, :284-300 `load_pretrained`,
-:302-304 `device`, :343-349 the `shape_constraints` / `interpolation_mode` / `resolution_level` attributes; HF-hub mixin
-`from_pretrained`):
+Mirrors `unidepth.models.unidepthv2.unidepthv2_old.UniDepthV2old` for the inference and evaluation paths (reference:
+unidepth/models/unidepthv2/unidepthv2_old.py:126-132 constructor, :134-196 `forward` in eval mode, :198-282 `infer`,
+:284-300 `load_pretrained`, :302-304 `device`, :343-349 the `shape_constraints` / `interpolation_mode` /
+`resolution_level` attributes; HF-hub mixin `from_pretrained`):
 
     model = UniDepthV2old.from_pretrained(dir_with_config_json_and_safetensors)     # or UniDepthV2old(config)
     model = model.to("cuda").eval()
     model.resolution_level = 5                                                       # None: the maximum (10), with a warning
     out = model.infer(rgb_uint8, intrinsics=None)       # dict: intrinsics points depth confidence
+    out = model(inputs, image_metas)                    # the reference's evaluation forward (see `forward`)
 
 The module owns `nn.Parameter`s under exactly the reference's state-dict names (unidepth_b200/spec_v2old.py), so
 reference checkpoints load unchanged.  `infer` packs the weights once and makes ONE C call (`udb_infer_v2old`,
@@ -247,5 +248,74 @@ class UniDepthV2old(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
             key = (shape, tuple(rgbs.shape), rgbs.dtype, scale255, normalize, K is not None, mode)
             return self._run_graphed(run, rgbs, {} if K is None else {"K": K}, key)
 
-    def forward(self, *args, **kwargs):
-        raise NotImplementedError("training / validation forward of UniDepthV2old is out of scope; use .infer()")
+    # ------------------------------------------------------------------ forward
+    def _forward_network(self, image: torch.Tensor, K: Optional[torch.Tensor], out_hw: Tuple[int, int]):
+        """One network-only call of the engine (udb_infer_v2old with network_only = 1) on the normalised f32 network
+        input `image` [B, 3, h, w] -> the outputs of `forward`, maps at `out_hw`."""
+        eng = self._engine
+        lib = cabi.lib()
+        dev = image.device
+        B, _, h, w = image.shape
+        H, W = out_hw
+        ws = self._workspace((self._engine_key, B, h, w), lambda: lib.udb_v2old_workspace_bytes(eng, B, h, w))
+        out = {"K": torch.empty((B, 3, 3), device=dev, dtype=f32),
+               "depth": torch.empty((B, 1, H, W), device=dev, dtype=f32),
+               "confidence": torch.empty((B, 1, H, W), device=dev, dtype=f32),
+               "points": torch.empty((B, 3, H, W), device=dev, dtype=f32),
+               "depth_features": torch.empty((B, (h // PATCH) * (w // PATCH), self.spec.hidden), device=dev, dtype=f32)}
+        a = cabi.InferV2oldArgs()
+        a.rgb, a.B, a.H, a.W = image.data_ptr(), B, h, w
+        a.intrinsics = K.data_ptr() if K is not None else None
+        a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
+        a.out_intrinsics, a.out_points = out["K"].data_ptr(), out["points"].data_ptr()
+        a.out_depth, a.out_confidence = out["depth"].data_ptr(), out["confidence"].data_ptr()
+        a.network_only, a.out_h, a.out_w, a.out_depth_features = 1, H, W, out["depth_features"].data_ptr()
+        cabi.check(lib.udb_infer_v2old(eng, C.byref(a), C.c_void_p(torch.cuda.current_stream().cuda_stream)), "udb_infer_v2old")
+        return out
+
+    @torch.no_grad()
+    def forward(self, inputs, image_metas=None):
+        """The reference's evaluation call `model(inputs, image_metas)` (unidepthv2_old.py:134-196), in eval mode only:
+
+            out = model({"image": x, "depth": gt, "K": K}, image_metas)    # "K" optional; image_metas is not read
+
+        `inputs["image"]` is the network input itself: float [B, 3, h, w], already normalised, both sides multiples of 14
+        (no resize, padding or normalisation here).  `inputs["depth"]` gives only its size (H, W).  A `inputs["K"]`
+        [B, 3, 3] drives the rays as it is, which the reference allows only when (H, W) == (h, w).  Returns
+          "K"              [B, 3, 3]   the predicted K at (h, w), also when K is given (`infer` returns the given K),
+          "depth"          [B, 1, H, W] and "confidence" [B, 1, H, W], antialiased bilinear from (h, w),
+          "points"         [B, 3, H, W] through the predicted K, unscaled, on the (H, W) grid, also when K is given,
+          "depth_features" [B, (h/14)(w/14), 512] f32, the depth head's latents before its Nystrom blocks.
+        Unlike the reference, the caller's `inputs` dict is left as it was: the reference adds "rays", "angles",
+        "features", "tokens", "global_tokens" and "camera_tokens" to it.  `precision` applies as in `infer`; the outputs
+        are new tensors (`output_buffers` holds `infer`'s only).  Training mode raises NotImplementedError: the training
+        forward is out of scope."""
+        if self.training or not isinstance(inputs, dict):
+            raise NotImplementedError("UniDepthV2old.forward runs the evaluation call model(inputs_dict, image_metas) in "
+                                      "eval mode only (model.eval()); the training forward is out of scope")
+        for k in ("image", "depth"):
+            if k not in inputs:
+                raise ValueError(f"inputs needs {k!r}: the network input and the ground truth whose size the outputs take")
+        image = inputs["image"]
+        if image.ndim != 4 or image.shape[1] != 3 or not image.dtype.is_floating_point:
+            raise ValueError(f"inputs['image'] must be a float [B, 3, h, w] tensor, not {image.dtype} {tuple(image.shape)}")
+        B, _, h, w = image.shape
+        if h % PATCH or w % PATCH:
+            raise ValueError(f"inputs['image'] is {h}x{w}: both sides must be multiples of the patch size {PATCH}")
+        H, W = (int(v) for v in inputs["depth"].shape[-2:])
+        K = inputs.get("K")
+        if K is not None:
+            if tuple(K.shape) != (B, 3, 3):
+                raise ValueError(f"inputs['K'] must be [B, 3, 3] = [{B}, 3, 3], not {tuple(K.shape)}")
+            if (H, W) != (h, w):
+                raise ValueError(f"inputs['K'] with a ground truth of {H}x{W} and an image of {h}x{w}: the rays of K are "
+                                 "reshaped to the image grid, so the two sizes must be equal")
+        dev = self._cuda_device()
+        shape = (h, w)
+        with torch.cuda.device(dev):
+            x = image.to(dev, f32).contiguous()
+            Kd = K.to(dev, f32).contiguous() if K is not None else None
+            self._shape_engine(shape, self._engine_config(shape))
+            run = lambda x, ins: self._forward_network(x, ins.get("K"), (H, W))
+            key = ("forward", B, h, w, H, W, K is not None)
+            return self._run_graphed(run, x, {} if Kd is None else {"K": Kd}, key, output_buffers=False)
