@@ -561,6 +561,38 @@ typedef struct udb_postprocess_t {
 } udb_postprocess_t;
 int udb_postprocess(const udb_postprocess_t* p, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Output assembly of the evaluation forward (unidepthv2.py:134-160 `forward_test`, with
+ * utils/misc.py:596-642 `match_gt` and :645-690 `match_intrinsics`), one launch:
+ *   per image b with pads[b] = (l, r, t, b) of the network input, crop the network maps to
+ *   [t, net_h-b) x [l, net_w-r) and resize the crop to H x W with bilinear (align_corners=False, no
+ *   antialias; ATen upsample_bilinear2d's fp32 index arithmetic, scale = crop / out, source clamped
+ *   at 0), taking the taps of points = rays*radius -> out_points [B,3,H,W], out_depth [B,1,H,W] =
+ *   points.z, out_confidence [B,1,H,W];
+ *   out_rays [B,3,net_h,net_w]: the network's rays, normalised twice (max(|r|, 1e-5)), at the
+ *   network size (the reference returns them unmatched);
+ *   intrinsics [B,3,3] IN PLACE: the K of the network input in, match_intrinsics' K out (f32, fx*sx,
+ *   fy*sy, (cx-l)*sx, (cy-t)*sy with sx = f32(W / (net_w-l-r)) rounded from the double ratio).
+ * rays come from rays_in when given, else from intr4 (fx, fy, cx, cy).  pads is DEVICE memory, so a
+ * negative pad or a crop that leaves no row or column cannot be refused before the launch: that
+ * image's maps and K come out NaN, nothing is read out of range.  The caller checks the pads (the
+ * Python boundary class does, before anything runs).
+ * ------------------------------------------------------------------------------------------- */
+typedef struct udb_match_gt_t {
+  const float* radius;       /* [B, net_h, net_w] */
+  const float* confidence;   /* [B, net_h, net_w] */
+  const float* intr4;        /* [B,4], read when rays_in is NULL */
+  const float* rays_in;      /* optional [B, net_h*net_w, 3] */
+  const int32_t* pads;       /* device [B,4] l r t b, each >= 0 */
+  int32_t B, net_h, net_w, H, W;
+  float* intrinsics;         /* [B,3,3] in place */
+  float* out_confidence;
+  float* out_depth;
+  float* out_points;
+  float* out_rays;
+} udb_match_gt_t;
+int udb_match_gt(const udb_match_gt_t* p, void* stream);
+
 /* ======================================================================================
  * Whole-path engine: one handle = one UniDepthV2 model on one device.
  *
@@ -667,6 +699,22 @@ typedef struct udb_infer_args_t {
 } udb_infer_args_t;
 
 int udb_infer_v2(udb_engine* e, const udb_infer_args_t* a, void* stream);
+
+/* Evaluation forward (`forward_test`, unidepthv2.py:134-160): `args` as for udb_infer_v2 with resolution_level
+ * UDB_LEVEL_NETWORK_ONLY, and the output assembly of udb_match_gt selected by match_h, match_w >= 1 and match_pads:
+ * confidence, depth and points are the network maps cropped by match_pads and resized to [B,*,match_h,match_w]
+ * (`match_gt`), intrinsics is `match_intrinsics`' K, rays stay [B,3,H,W] at the network size, and radius is not written
+ * (may be NULL).  All three zero: exactly udb_infer_v2(args).  The engine refuses, before any launch, match fields at
+ * another resolution_level, and a size without pads or pads without a size.  match_pads lives on the device, so the
+ * engine cannot see a crop that leaves no row or column (that image's outputs come out NaN): the caller checks
+ * H - t - b >= 1, W - l - r >= 1 and every pad >= 0.  The matching takes no workspace: udb_workspace_bytes of the
+ * network-only shape applies.  A struct of its own, so that udb_infer_args_t keeps its layout for existing callers. */
+typedef struct udb_infer_match_args_t {
+  udb_infer_args_t args;
+  int32_t match_h, match_w;
+  const int32_t* match_pads;  /* device [B,4] int32: l r t b of each network input */
+} udb_infer_match_args_t;
+int udb_infer_v2_match(udb_engine* e, const udb_infer_match_args_t* a, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * UniDepthV1 engine: the whole `UniDepthV1.infer` path (ConvNeXt or DINOv2 encoder) as one call (SURVEY.md section 8b

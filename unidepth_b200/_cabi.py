@@ -100,6 +100,14 @@ class Postprocess(C.Structure):
     ]
 
 
+class MatchGt(C.Structure):
+    _fields_ = [
+        ("radius", vp), ("confidence", vp), ("intr4", vp), ("rays_in", vp), ("pads", vp),
+        ("B", i32), ("net_h", i32), ("net_w", i32), ("H", i32), ("W", i32),
+        ("intrinsics", vp), ("out_confidence", vp), ("out_depth", vp), ("out_points", vp), ("out_rays", vp),
+    ]
+
+
 class Config(C.Structure):
     _fields_ = [
         ("embed_dim", i32), ("depth", i32), ("enc_heads", i32), ("taps", i32 * 4), ("pos_grid", i32),
@@ -132,6 +140,10 @@ class InferArgs(C.Structure):
         ("confidence", vp), ("intrinsics", vp), ("radius", vp), ("depth", vp), ("points", vp), ("rays", vp),
         ("depth_features", vp),
     ]
+
+
+class InferMatchArgs(C.Structure):
+    _fields_ = [("args", InferArgs), ("match_h", i32), ("match_w", i32), ("match_pads", vp)]
 
 
 class V1Preprocess(C.Structure):
@@ -273,6 +285,7 @@ EXPORTS = {
     "udb_reflect_pad1_nhwc_f16": (i32, [vp, vp, i32, i32, i32, i32, vp]),
     "udb_reflect_border_fill_nhwc_f16": (i32, [vp, i32, i32, i32, i32, vp]),
     "udb_postprocess": (i32, [C.POINTER(Postprocess), vp]),
+    "udb_match_gt": (i32, [C.POINTER(MatchGt), vp]),
     "udb_camera_adjust_k": (i32, [vp, i32, f32, i32, i32, vp, vp]),
     "udb_camera_rays": (i32, [i32, vp, i32, i32, i32, i32, i32, i32, i32, f32, vp, vp]),
     "udb_create": (i32, [C.POINTER(Config), C.POINTER(vp)]),
@@ -283,6 +296,7 @@ EXPORTS = {
     "udb_workspace_bytes": (C.c_size_t, [vp, i32, i32, i32, i32]),
     "udb_schedule_bytes": (C.c_size_t, [vp, i32, i32, i32, i32]),
     "udb_infer_v2": (i32, [vp, C.POINTER(InferArgs), vp]),
+    "udb_infer_v2_match": (i32, [vp, C.POINTER(InferMatchArgs), vp]),
     # UniDepthV1 operators + engine
     "udb_v1_preprocess": (i32, [C.POINTER(V1Preprocess), vp]),
     "udb_v1_preprocess_split": (i32, [C.POINTER(V1Preprocess), vp]),

@@ -695,6 +695,90 @@ __global__ void __launch_bounds__(256) postprocess_bicubic_kernel(const udb_post
   }
 }
 
+// Output assembly of the evaluation forward (udb_match_gt), its own kernel so that postprocess_kernel keeps its code.
+// Matched maps: one thread per output pixel, the four taps of ATen's CUDA upsample_bilinear2d on the crop, combined in its
+// order (h0 * (w0 * v00 + w1 * v01) + h1 * (w0 * v10 + w1 * v11)); a tap of the points is rays * radius rounded once, as
+// network_forward's points are.  Threads below B * net_h * net_w also write one network pixel's rays, threads below B
+// one matched K.  An image whose pads are negative or leave no row or column gets NaN maps and K (no read out of range).
+__device__ __forceinline__ void match_tap(const udb_match_gt_t& p, const float4 k, long long o, int y, int x, float& c,
+                                          float& px, float& py, float& pz) {
+  float3 r;
+  if (p.rays_in) { const float* rp = p.rays_in + o * 3; r = make_float3(rp[0], rp[1], rp[2]); }
+  else r = unit_ray(k, y, x);
+  const float rad = p.radius[o];
+  c = p.confidence[o];
+  px = __fmul_rn(r.x, rad); py = __fmul_rn(r.y, rad); pz = __fmul_rn(r.z, rad);
+}
+
+__global__ void __launch_bounds__(256) match_gt_kernel(const udb_match_gt_t p, long long total) {
+  const long long n_out = (long long)p.B * p.H * p.W, n_net = (long long)p.B * p.net_h * p.net_w;
+  const float nan = __int_as_float(0x7fc00000);
+  for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
+       idx += (long long)gridDim.x * blockDim.x) {
+    if (idx < n_out) {
+      const int x = (int)(idx % p.W), y = (int)((idx / p.W) % p.H), b = (int)(idx / ((long long)p.W * p.H));
+      const int* pd = p.pads + b * 4;
+      const int l = pd[0], r = pd[1], t = pd[2], bo = pd[3];
+      const int ch = p.net_h - t - bo, cw = p.net_w - l - r;
+      const long long plane = (long long)p.H * p.W, pix = (long long)y * p.W + x;
+      float conf = nan, px = nan, py = nan, pz = nan;
+      if (min(min(l, r), min(t, bo)) >= 0 && ch >= 1 && cw >= 1) {
+        int y0, y1, x0, x1;
+        float ly0, ly1, lx0, lx1;
+        bilinear_src((float)ch / (float)p.H, y, ch, y0, y1, ly0, ly1);
+        bilinear_src((float)cw / (float)p.W, x, cw, x0, x1, lx0, lx1);
+        y0 += t; y1 += t; x0 += l; x1 += l;
+        float4 k = make_float4(1.f, 1.f, 0.f, 0.f);
+        if (!p.rays_in) k = *reinterpret_cast<const float4*>(p.intr4 + b * 4);
+        const long long rb = (long long)b * p.net_h;
+        float c[4], X[4], Y[4], Z[4];
+        match_tap(p, k, (rb + y0) * p.net_w + x0, y0, x0, c[0], X[0], Y[0], Z[0]);
+        match_tap(p, k, (rb + y0) * p.net_w + x1, y0, x1, c[1], X[1], Y[1], Z[1]);
+        match_tap(p, k, (rb + y1) * p.net_w + x0, y1, x0, c[2], X[2], Y[2], Z[2]);
+        match_tap(p, k, (rb + y1) * p.net_w + x1, y1, x1, c[3], X[3], Y[3], Z[3]);
+        auto lerp = [&](const float* v) { return ly0 * (lx0 * v[0] + lx1 * v[1]) + ly1 * (lx0 * v[2] + lx1 * v[3]); };
+        conf = lerp(c); px = lerp(X); py = lerp(Y); pz = lerp(Z);
+      }
+      p.out_confidence[b * plane + pix] = conf;
+      p.out_depth[b * plane + pix] = pz;
+      p.out_points[(b * 3 + 0) * plane + pix] = px;
+      p.out_points[(b * 3 + 1) * plane + pix] = py;
+      p.out_points[(b * 3 + 2) * plane + pix] = pz;
+    }
+    if (idx < n_net) {
+      // the rays network_forward returns (one normalisation), normalised once more as forward_test does
+      const int x = (int)(idx % p.net_w), y = (int)((idx / p.net_w) % p.net_h), b = (int)(idx / ((long long)p.net_w * p.net_h));
+      float3 r;
+      if (p.rays_in) { const float* rp = p.rays_in + idx * 3; r = make_float3(rp[0], rp[1], rp[2]); }
+      else r = unit_ray(*reinterpret_cast<const float4*>(p.intr4 + b * 4), y, x);
+      const float n1 = fmaxf(sqrtf(r.x * r.x + r.y * r.y + r.z * r.z), 1e-5f);
+      const float ax = r.x / n1, ay = r.y / n1, az = r.z / n1;
+      const float n2 = fmaxf(sqrtf(ax * ax + ay * ay + az * az), 1e-5f);
+      const long long plane = (long long)p.net_h * p.net_w, pix = (long long)y * p.net_w + x;
+      p.out_rays[(b * 3 + 0) * plane + pix] = ax / n2;
+      p.out_rays[(b * 3 + 1) * plane + pix] = ay / n2;
+      p.out_rays[(b * 3 + 2) * plane + pix] = az / n2;
+    }
+    if (idx < p.B) {
+      // match_intrinsics (misc.py:645-690) in f32 and in its op order; the target has no padding (padding2 = None)
+      const int b = (int)idx;
+      const int* pd = p.pads + b * 4;
+      const int l = pd[0], t = pd[2];
+      const int ch = p.net_h - t - pd[3], cw = p.net_w - l - pd[1];
+      float* K = p.intrinsics + b * 9;
+      if (min(min(l, pd[1]), min(t, pd[3])) >= 0 && ch >= 1 && cw >= 1) {
+        const float sx = (float)((double)p.W / (double)cw), sy = (float)((double)p.H / (double)ch);
+        K[0] = __fmul_rn(K[0], sx);
+        K[4] = __fmul_rn(K[4], sy);
+        K[2] = __fadd_rn(__fmul_rn(__fsub_rn(K[2], (float)l), sx), 0.f);
+        K[5] = __fadd_rn(__fmul_rn(__fsub_rn(K[5], (float)t), sy), 0.f);
+      } else {
+        for (int i = 0; i < 9; ++i) K[i] = nan;
+      }
+    }
+  }
+}
+
 // f16 rows -> e4m3 rows + row scales (udb_quantize_rows_e4m3): one warp per row, lane holds 16-byte chunks
 // lane + 32 i (i < NCH: up to NCH * 256 columns) in registers between the amax reduction and the conversion.  NCH = 16
 // serves up to 4096 columns (the DINOv2 MLP), NCH = 24 up to 6144 (ConvNeXt-L stage 3's 4 x 1536); the amax is a max,
@@ -983,4 +1067,22 @@ extern "C" int udb_postprocess(const udb_postprocess_t* p, void* stream) {
   }
   postprocess_kernel<<<grid, 256, 0, ST(stream)>>>(*p);
   return check_launch("postprocess_kernel");
+}
+
+extern "C" int udb_match_gt(const udb_match_gt_t* p, void* stream) {
+  const struct { int v; const char* name; } dims[] = {{p->B, "B"}, {p->H, "H"}, {p->W, "W"}, {p->net_h, "net_h"}, {p->net_w, "net_w"}};
+  for (const auto& d : dims)
+    if (d.v < 1) { set_error("udb_match_gt: %s=%d must be >= 1", d.name, d.v); return 1; }
+  const struct { const void* q; const char* name; } ptrs[] = {
+      {p->radius, "radius"}, {p->confidence, "confidence"}, {p->pads, "pads"}, {p->intrinsics, "intrinsics"},
+      {p->out_confidence, "out_confidence"}, {p->out_depth, "out_depth"}, {p->out_points, "out_points"}, {p->out_rays, "out_rays"}};
+  for (const auto& a : ptrs)
+    if (!a.q) { set_error("udb_match_gt: `%s` must be non-null", a.name); return 1; }
+  if (!p->rays_in && !p->intr4) { set_error("udb_match_gt: `intr4` must be non-null when `rays_in` is null"); return 1; }
+  if (!p->rays_in && (reinterpret_cast<uintptr_t>(p->intr4) & 15)) { set_error("udb_match_gt: `intr4` must be 16-byte aligned"); return 1; }
+  const long long n_out = (long long)p->B * p->H * p->W, n_net = (long long)p->B * p->net_h * p->net_w;
+  const long long total = n_out > n_net ? n_out : n_net;
+  note_work(0.0, 4.0 * (2.0 * n_net + 5.0 * n_out + 3.0 * n_net));
+  match_gt_kernel<<<grid_for(total), 256, 0, ST(stream)>>>(*p, total);
+  return check_launch("match_gt_kernel");
 }

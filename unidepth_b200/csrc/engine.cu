@@ -1,5 +1,5 @@
 // Whole-path engine behind udb_create / udb_set_weight / udb_set_scalar / udb_workspace_bytes / udb_schedule_bytes /
-// udb_infer_v2 (include/udb.h): the host-side schedule of UniDepthV2.infer as one C call that only enqueues the
+// udb_infer_v2 / udb_infer_v2_match (include/udb.h): the host-side schedule of UniDepthV2.infer (and of forward_test) as one C call that only enqueues the
 // kernels of this library on the caller's stream, on the skeleton it shares with the UniDepthV1 and UniDepthV2old
 // engines (engine_common.h: the "precision" scalar, the DINOv2 patch embedding and block loop).  Reference call stack it
 // replaces:
@@ -77,7 +77,7 @@ static int resize(const udb_config_t& c, int level, udb_geometry_t* g) {
 
 // ------------------------------------------------------------------------------------------ the schedule
 static int run(udb_engine* e, const udb_infer_args_t& a, const udb_geometry_t& g, const ShapeTables& tb, Arena& ar,
-               void* st) {
+               void* st, const udb_infer_match_args_t* mt = nullptr) {
   const udb_config_t& cf = e->cfg;
   Ctx c{e, &ar, st, ar.dry};
   const int B = a.B, nh = g.net_h, nw = g.net_w, gh = g.gh, gw = g.gw;
@@ -311,8 +311,17 @@ static int run(udb_engine* e, const udb_infer_args_t& a, const udb_geometry_t& g
   }
 
   stage.next("udb:postprocess");
-  // ---- a18: output assembly at the original resolution
-  {
+  // ---- a18: output assembly at the original resolution, or matched to the ground truth (`forward_test`); neither
+  //      takes scratch, so the workspace does not depend on the match fields
+  if (mt && mt->match_h) {
+    udb_match_gt_t p;
+    memset(&p, 0, sizeof(p));
+    p.radius = planes[0]; p.confidence = planes[1]; p.intr4 = ray_intr; p.rays_in = rays_in; p.pads = mt->match_pads;
+    p.B = B; p.net_h = nh; p.net_w = nw; p.H = mt->match_h; p.W = mt->match_w;
+    p.intrinsics = a.intrinsics; p.out_confidence = a.confidence; p.out_depth = a.depth; p.out_points = a.points;
+    p.out_rays = a.rays;
+    c.launch([&] { return udb_match_gt(&p, st); });
+  } else {
     udb_postprocess_t p;
     memset(&p, 0, sizeof(p));
     p.radius = planes[0]; p.confidence = planes[1]; p.intr4 = ray_intr; p.rays_in = rays_in;
@@ -462,10 +471,28 @@ size_t udb_workspace_bytes(udb_engine* e, int32_t B, int32_t H, int32_t W, int32
   return n ? e->prepared(shape_name(B, H, W) + idx(" (level %d)", level), n) : 0;
 }
 
-int udb_infer_v2(udb_engine* e, const udb_infer_args_t* a, void* stream) {
+}  // extern "C"
+
+namespace udb {
+
+static int infer(udb_engine* e, const udb_infer_args_t* a, const udb_infer_match_args_t* mt, void* stream) {
   if (!e || !a || !a->rgb || !a->workspace) { set_error("udb_infer_v2: null argument"); return 1; }
-  if (!a->confidence || !a->intrinsics || !a->radius || !a->depth || !a->points || !a->rays || !a->depth_features) {
-    set_error("udb_infer_v2: all seven output pointers are required");
+  const bool match = mt && (mt->match_h || mt->match_w || mt->match_pads);
+  if (match) {
+    if (a->resolution_level != UDB_LEVEL_NETWORK_ONLY) {
+      set_error("udb_infer_v2_match: match_h, match_w and match_pads are read with resolution_level UDB_LEVEL_NETWORK_ONLY "
+                "(-2) only, not %d", a->resolution_level);
+      return 1;
+    }
+    if (mt->match_h < 1 || mt->match_w < 1 || !mt->match_pads) {
+      set_error("udb_infer_v2_match: matching to the ground truth needs match_h, match_w >= 1 and match_pads together "
+                "(match_h %d, match_w %d, match_pads %s)", mt->match_h, mt->match_w, mt->match_pads ? "set" : "NULL");
+      return 1;
+    }
+  }
+  if (!a->confidence || !a->intrinsics || (!a->radius && !match) || !a->depth || !a->points || !a->rays || !a->depth_features) {
+    set_error(match ? "udb_infer_v2: all output pointers but radius are required when matching to the ground truth"
+                    : "udb_infer_v2: all seven output pointers are required");
     return 1;
   }
   if (a->interpolation != UDB_INTERP_BILINEAR && a->interpolation != UDB_INTERP_BICUBIC) {
@@ -498,7 +525,19 @@ int udb_infer_v2(udb_engine* e, const udb_infer_args_t* a, void* stream) {
     return 1;
   }
   Arena ar(a->workspace, a->workspace_bytes);
-  return run(e, *a, g, tb->second, ar, stream);
+  return run(e, *a, g, tb->second, ar, stream, match ? mt : nullptr);
 }
+
+}  // namespace udb
+
+extern "C" {
+
+int udb_infer_v2(udb_engine* e, const udb_infer_args_t* a, void* stream) { return udb::infer(e, a, nullptr, stream); }
+
+int udb_infer_v2_match(udb_engine* e, const udb_infer_match_args_t* a, void* stream) {
+  if (!a) { set_error("udb_infer_v2_match: null argument"); return 1; }
+  return udb::infer(e, &a->args, a, stream);
+}
+
 
 }  // extern "C"

@@ -241,8 +241,10 @@ class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         return self._create_engine(self._engine_config(T), key)
 
     def _forward_engine(self, rgb: torch.Tensor, geom: dict, normalize: bool, level, camera_k=None, rays_in=None,
-                        camera_model=0, camera_params=None):
-        """The whole path as ONE C call (udb_infer_v2): torch only allocates outputs / workspace."""
+                        camera_model=0, camera_params=None, match_pads=None):
+        """The whole path as ONE C call (udb_infer_v2): torch only allocates outputs / workspace.  With `match_pads`
+        (device int32 [B, 4], network-only level, geom["match_hw"]) the engine matches the outputs to the ground truth
+        as `forward_test` returns them."""
         eng = self._get_engine()
         lib = cabi.lib()
         dev = rgb.device
@@ -258,7 +260,13 @@ class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         out = {"confidence": E(B, 1, H, W), "intrinsics": E(B, 3, 3), "radius": E(B, 1, H, W), "depth": E(B, 1, H, W),
                "points": E(B, 3, H, W), "rays": E(B, 3, H, W)}
         feats = E(B, g.gh, g.gw, hid)
-        a = cabi.InferArgs()
+        ma = cabi.InferMatchArgs()
+        a = ma.args                        # a view into `ma`
+        if match_pads is not None:
+            Hm, Wm = geom["match_hw"]
+            out = {"depth": E(B, 1, Hm, Wm), "points": E(B, 3, Hm, Wm), "confidence": E(B, 1, Hm, Wm),
+                   "rays": E(B, 3, H, W), "intrinsics": E(B, 3, 3)}
+            ma.match_h, ma.match_w, ma.match_pads = Hm, Wm, match_pads.data_ptr()
         a.rgb, a.rgb_is_u8, a.normalize = rgb.data_ptr(), int(rgb.dtype == torch.uint8), int(normalize)
         a.B, a.H, a.W, a.resolution_level = B, H, W, lvl
         a.interpolation = cabi.INTERP_MODES[geom.get("interpolation", "bilinear")]
@@ -271,8 +279,13 @@ class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         for k, v in out.items():
             setattr(a, k, v.data_ptr())
         a.depth_features = feats.data_ptr()
-        cabi.check(lib.udb_infer_v2(eng, C.byref(a), C.c_void_p(torch.cuda.current_stream().cuda_stream)), "udb_infer_v2")
-        out["depth_features"] = feats.permute(0, 3, 1, 2)
+        st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+        if match_pads is None:
+            cabi.check(lib.udb_infer_v2(eng, C.byref(a), st), "udb_infer_v2")
+        else:
+            cabi.check(lib.udb_infer_v2_match(eng, C.byref(ma), st), "udb_infer_v2_match")
+        if match_pads is None:
+            out["depth_features"] = feats.permute(0, 3, 1, 2)
         return out
 
     @staticmethod
@@ -381,25 +394,66 @@ class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
             rays_in = rays.to(rgbs.device, f32).permute(0, 2, 3, 1).reshape(B, H * W, 3).contiguous()
         return self._run(rgbs, geom, self.NETWORK_ONLY, False, None, ("network_only",), rays_in=rays_in)
 
+    @staticmethod
+    def _match_paddings(inputs: dict, image_metas, B: int, h: int, w: int) -> torch.Tensor:
+        """The (l, r, t, b) paddings of each network input as a CPU int32 [B, 4] tensor, taken as the reference's
+        `encode_decode` takes them (unidepthv2.py:344-357): the metas' "paddings" (l, t, r, b) reordered to (l, r, t, b)
+        when the first meta has them, else inputs["paddings"] (4-tuples or a [B, 4] tensor), else zeros (where the
+        reference raises KeyError).  Raises ValueError for a count other than B, a negative padding or a crop that
+        leaves no row or column."""
+        if image_metas is not None and len(image_metas) and "paddings" in image_metas[0]:
+            rows = [torch.as_tensor(m["paddings"]).cpu() for m in image_metas]
+            if any(r.shape != (4,) for r in rows):
+                raise ValueError(f"image_metas paddings must be 4 values (l, t, r, b) each, got {[tuple(r.shape) for r in rows]}")
+            pads, src = torch.stack(rows)[:, [0, 2, 1, 3]], "image_metas"
+        elif inputs.get("paddings") is not None:
+            pads, src = torch.as_tensor(inputs["paddings"]).cpu(), "inputs['paddings']"
+        else:
+            return torch.zeros((B, 4), dtype=torch.int32)
+        if pads.ndim != 2 or pads.shape != (B, 4):
+            raise ValueError(f"{src} holds {tuple(pads.shape)} paddings: need one (l, r, t, b) per image, [{B}, 4]")
+        if pads.is_floating_point() and not torch.equal(pads, pads.trunc()):
+            raise ValueError(f"{src}: paddings must be whole pixels, got {pads.tolist()}")
+        pads = pads.to(torch.int64)
+        if bool((pads < 0).any()):
+            raise ValueError(f"{src}: paddings must be >= 0, got {pads.tolist()}")
+        rows_left, cols_left = h - pads[:, 2] - pads[:, 3], w - pads[:, 0] - pads[:, 1]
+        if bool((rows_left < 1).any() or (cols_left < 1).any()):
+            raise ValueError(f"{src}: paddings {pads.tolist()} leave no row or column of the {h}x{w} network input")
+        return pads.to(torch.int32)
+
     @torch.no_grad()
     def forward_test(self, inputs: dict, image_metas=None):
-        """Validation forward of the reference (unidepthv2.py:134-160): `inputs["image"]` is the data
-        pipeline's normalised network input, `inputs["depth"]` the ground truth whose size the predictions
-        are matched to, `inputs["paddings"]` the per-image (l, r, t, b) paddings of the network input,
-        optional `inputs["camera"]` a camera object for GT rays (:361-362)."""
-        from .validation import match_gt, match_intrinsics
-        image = inputs["image"]
-        rays = None
-        cam = inputs.get("camera", None)
-        if cam is not None:
-            B, _, H, W = image.shape
-            rays = cam.get_rays(shapes=(B, H, W))
-        out = self._network_outputs(image, rays)
-        gt, pads = inputs["depth"], inputs.get("paddings", None)
-        res = {k: match_gt(out[k], gt, padding1=pads, padding2=None) for k in ("depth", "points", "confidence")}
-        res["rays"] = out["rays"] / torch.norm(out["rays"], dim=1, keepdim=True).clip(min=1e-5)
-        res["intrinsics"] = match_intrinsics(out["intrinsics"], image, gt, padding1=pads, padding2=None)
-        return res
+        """Validation forward of the reference (unidepthv2.py:134-160), on the engine: `inputs["image"]` is the data
+        pipeline's normalised network input [B, 3, h, w], `inputs["depth"]` the ground truth [B, 1, H, W] whose size the
+        predictions are matched to, the paddings of the network input come from the metas or `inputs["paddings"]`
+        (`_match_paddings`), and an optional `inputs["camera"]` gives the rays (:361-362).  Returns depth, points and
+        confidence at (H, W) (`match_gt`: crop the paddings, bilinear resize), the intrinsics of that frame
+        (`match_intrinsics`) and the renormalised rays at (h, w), all from one udb_infer_v2 call.
+
+        A camera object that `pack_camera` accepts gets its rays from the engine's camera kernel at (h, w), uncropped and
+        unscaled (the reference calls get_rays(shapes=(B, h, w)) on it as given); any other object's own get_rays runs on
+        the host.  CUDA graphs are cached per (B, h, w, H, W, camera source): the paddings are graph inputs, so a new
+        batch with other paddings replays.  The caller's `inputs` is left unchanged."""
+        image, gt = inputs["image"], inputs["depth"]
+        if image.ndim != 4 or image.shape[1] != 3:
+            raise ValueError(f"inputs['image'] must be [B, 3, h, w], not {tuple(image.shape)}")
+        B, _, h, w = image.shape
+        if h % PATCH or w % PATCH:
+            raise ValueError(f"network input {h}x{w} must be a multiple of {PATCH}")
+        if gt.ndim != 4:
+            raise ValueError(f"inputs['depth'] must be a [B, 1, H, W] ground truth, not {tuple(gt.shape)}")
+        pads = self._match_paddings(inputs, image_metas, B, h, w)
+        H, W = int(gt.shape[-2]), int(gt.shape[-1])
+        cam, rays_in = inputs.get("camera", None), None
+        if cam is not None and pack_camera(cam) is None:
+            rays = cam.get_rays(shapes=(B, h, w))
+            rays_in = rays.to(self._cuda_device(), f32).expand(B, 3, h, w).permute(0, 2, 3, 1).reshape(B, h * w, 3).contiguous()
+            cam = None
+        rgb = self._to_device_input(image.float())
+        geom = dict(paddings=(0, 0, 0, 0), padded_hw=(h, w), factor=1.0, net_hw=(h, w), out_hw=(h, w), match_hw=(H, W))
+        return self._run(rgb, geom, self.NETWORK_ONLY, False, cam, ("forward_test", H, W), rays_in=rays_in,
+                         match_pads=pads)
 
     def forward(self, inputs=None, image_metas=None, *args, **kwargs):
         """Evaluation-mode `forward` of the reference dispatches to `forward_test` (unidepthv2.py:162-166);
@@ -414,14 +468,14 @@ class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
             rgb = rgb.float()
         return rgb.contiguous()
 
-    def _run(self, rgb, geom, level, normalize, camera, key_extra, rays_in=None):
-        """Common tail of infer / network_forward: camera handling, the engine call, CUDA graph cache.
+    def _run(self, rgb, geom, level, normalize, camera, key_extra, rays_in=None, match_pads=None):
+        """Common tail of infer / network_forward / forward_test: camera handling, the engine call, CUDA graph cache.
         Everything runs with the model's device current (streams, cudaMalloc of the engine tables, the per-device
         kernel attributes on the C side), so a model on cuda:1 works while cuda:0 is the process default."""
         with torch.cuda.device(self.device):
-            return self._run_on_device(rgb, geom, level, normalize, camera, key_extra, rays_in)
+            return self._run_on_device(rgb, geom, level, normalize, camera, key_extra, rays_in, match_pads)
 
-    def _run_on_device(self, rgb, geom, level, normalize, camera, key_extra, rays_in=None):
+    def _run_on_device(self, rgb, geom, level, normalize, camera, key_extra, rays_in=None, match_pads=None):
         B, _, H, W = rgb.shape
         dev = rgb.device
         nh, nw = geom["net_hw"]
@@ -445,9 +499,12 @@ class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
 
         def run(inp, cam):
             return self._forward_engine(inp, geom, normalize, level, camera_k=cam.get("K"), rays_in=cam.get("rays"),
-                                        camera_model=model, camera_params=cam.get("params"))
+                                        camera_model=model, camera_params=cam.get("params"), match_pads=cam.get("pads"))
 
+        if match_pads is not None:
+            cam["pads"] = match_pads.to(dev)
         # The camera source is part of the key (a graph captured for one source reads other buffers); its values are not:
-        # the entry owns static copies of the camera tensors, refreshed before every replay like the image.
+        # the entry owns static copies of the camera tensors (and of forward_test's paddings), refreshed before every
+        # replay like the image.
         key = (B, H, W, rgb.dtype, bool(normalize)) + tuple(key_extra) + (source,)
         return self._run_graphed(run, rgb, cam, key, keep=scales)
