@@ -37,7 +37,7 @@ def _v2(cfg_name, depth=None, **attrs):
 def _v2_engine(m, drop=(), reshape=None, scalars_over=None):
     tensors, scalars = m._pack_tensors(CPU)
     scalars = dict(scalars, **(scalars_over or {}))
-    cfg = m._engine_config(tensors)
+    cfg = m._engine_config()
     for name in drop:
         del tensors[name]
     if reshape:

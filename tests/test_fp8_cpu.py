@@ -123,7 +123,7 @@ def _v2(cfg_name, depth=None, **attrs):
 
 def _engine(m, tensors, scalars):
     h = C.c_void_p()
-    _cabi.check(_cabi.lib().udb_create(C.byref(m._engine_config(tensors)), C.byref(h)), "udb_create")
+    _cabi.check(_cabi.lib().udb_create(C.byref(m._engine_config()), C.byref(h)), "udb_create")
     m._register(h, tensors, scalars)
     return h
 

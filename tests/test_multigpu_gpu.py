@@ -42,7 +42,7 @@ def same(got, tag):
     return not bad
 
 # order matters: the FIRST call of the model captures the small (B=2) graph, then a gather, then the larger (B=4) graph --
-# the sequence that exposed the use-after-free of the ray-frequency table (unidepthv2.py::_run_on_device)
+# the sequence that exposed the use-after-free of the ray-frequency table (unidepthv2.py::_run)
 full = infer_sharded(m, rgb)
 single = m.infer(rgb)
 ok = same(full, "first synchronous gather")

@@ -107,7 +107,7 @@ def test_engine_refuses_bad_match_fields_and_sizes_no_scratch_for_them():
     m = _model()
     T, S = m._pack_tensors(CPU)
     h = C.c_void_p()
-    _cabi.check(lib.udb_create(C.byref(m._engine_config(T)), C.byref(h)), "udb_create")
+    _cabi.check(lib.udb_create(C.byref(m._engine_config()), C.byref(h)), "udb_create")
     try:
         m._register(h, T, S)
         cases = [

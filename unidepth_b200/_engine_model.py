@@ -2,10 +2,10 @@
 checkpoint loading, weight packing per weight version, the C engine's lifetime, the engine of a network shape, the input
 block of `infer`, and the workspace and CUDA-graph caches.
 
-A model class supplies its packer (`_pack_tensors` -> ({engine tensor name: tensor}, {scalar name: float}); the shared
-packing code is `_pack.py`), its engine (`_forward_engine`, and the lookup of the current engine: `_shape_engine` with the
-model's `_shape_operands` for one engine per network shape) and the names of its engine's C entry points
-(`_ENGINE_FNS`)."""
+A model class supplies its packer (`_pack_weights`, plus `_shape_operands` for an engine per network shape; `_pack_tensors`
+-> ({engine tensor name: tensor}, {scalar name: float}) joins the two; the shared packing code is `_pack.py`), its config
+struct (`_engine_config`), the names of its engine's C entry points (`_ENGINE_FNS`, and `_INFER` for the UniDepthV1
+family's infer call) and the calls that look up its engine and run it."""
 from __future__ import annotations
 
 import ctypes as C
@@ -17,6 +17,7 @@ import torch
 import torch.nn as nn
 
 from . import _cabi as cabi
+from .spec import PATCH
 
 try:  # same mixin as the reference (unidepthv2.py:111-117)
     from huggingface_hub import PyTorchModelHubMixin
@@ -34,6 +35,8 @@ HUB_KWARGS = dict(library_name="UniDepth", repo_url="https://github.com/lpiccine
                   tags=["monocular-metric-depth-estimation"]) if _HAS_HF else {}
 
 f16, f32 = torch.float16, torch.float32
+# the accepted `precision` modes; a mode's index is the engine's "precision" scalar (engine_common.h encoder_precision)
+PRECISIONS = ("f16", "split", "fp8")
 _DTYPES = {f16: cabi.DT_F16, f32: cabi.DT_F32, torch.float8_e4m3fn: cabi.DT_E4M3}   # udb.h UDB_DT_*
 
 
@@ -109,7 +112,7 @@ class EngineModel(nn.Module):
         return next(self.parameters()).device
 
     def _cuda_device(self):
-        """The model's device, which `infer` needs to be a CUDA device."""
+        """The model's device, which packing and every engine call need to be a CUDA device."""
         dev = self.device
         if dev.type != "cuda":
             raise RuntimeError("unidepth_b200 has no CPU path: move the model to a CUDA device")
@@ -139,22 +142,38 @@ class EngineModel(nn.Module):
             return model
 
     # ------------------------------------------------------------------ weight packing
-    def _fingerprint(self):
-        return tuple((p.data_ptr(), p._version) for p in self.parameters())
+    def _precision(self):
+        """(split, fp8, code) of the model's `precision`, one of PRECISIONS: code is the engine's "precision" scalar."""
+        if self.precision not in PRECISIONS:
+            raise ValueError(f"precision must be 'split', 'f16' or 'fp8', not {self.precision!r}; the engine's \"precision\" "
+                             "scalar numbers 'f16', 'split' or 'fp8' as 0, 1 or 2")
+        code = PRECISIONS.index(self.precision)
+        return code == 1, code == 2, code
 
-    def _pack_weights(self, dev):
-        """The operands that depend on the weights alone, packed once per weight version: by default all of
-        `_pack_tensors`."""
-        return self._pack_tensors(dev)
+    def _fingerprint(self):
+        return (self.precision,) + tuple((p.data_ptr(), p._version) for p in self.parameters())
+
+    def _default_shape(self):
+        """The network shape `_pack_tensors` and `_engine_config` take when given none; None: the model has no shape
+        operands (its engine takes every network shape)."""
+        return None
+
+    def _pack_tensors(self, dev, shape=None):
+        """({engine tensor name: tensor on `dev`}, {scalar name: float}): the weight operands (`_pack_weights`) and, for
+        a model with one engine per network shape, the operands of `shape` (default `_default_shape()`).  The product
+        packs the two parts separately (`_weights`, `_shape_engine`); the CPU tests run this to check, through the
+        engine's dry run, that the packer registers exactly the operands the C schedule asks for."""
+        T, S = self._pack_weights(dev)
+        shape = shape or self._default_shape()
+        if shape is not None:
+            T.update(self._shape_operands(shape, dev))
+        return T, S
 
     def _weights(self):
         """The packed (tensors, scalars), repacked once per weight version; a repack drops the engine and its caches."""
         if self._packed is None or self._packed_key != self._fingerprint():
-            dev = self.device
-            if dev.type != "cuda":
-                raise RuntimeError(f"unidepth_b200.{type(self).__name__}.infer needs the model on a CUDA device "
-                                   "(model.to('cuda')); there is no CPU fallback")
-            torch.cuda.set_device(dev)      # callers hold `with torch.cuda.device(self.device)`
+            dev = self._cuda_device()
+            torch.cuda.set_device(dev)      # callers hold the device context of `_run_graphed`
             self._drop_engine()             # it borrows the pointers of the tensors about to be replaced
             self._packed = self._pack_weights(dev)
             self._packed_key = self._fingerprint()
@@ -196,16 +215,16 @@ class EngineModel(nn.Module):
         self._engine, self._engine_key, self._engine_device = handle, key, self.device
         return handle
 
-    def _shape_engine(self, shape, cfg, check=None):
+    def _shape_engine(self, shape, check=None):
         """The engine of the network shape `shape` (UniDepthV1, UniDepthV2old: one engine per shape).  A new shape makes
-        a new engine for the config struct `cfg` with the packed weights and the shape's own operands
+        a new engine for `_engine_config(shape)` with the packed weights and the shape's own operands
         (`_shape_operands`); `_create_engine` drops the previous one, with its workspaces and graphs, only once the new
         one has passed `check`."""
         T, _ = self._weights()
         if self._engine is not None and self._engine_key == shape:
             return self._engine
         ops = self._shape_operands(shape, self.device)
-        handle = self._create_engine(cfg, shape, tensors={**T, **ops}, check=check)
+        handle = self._create_engine(self._engine_config(shape), shape, tensors={**T, **ops}, check=check)
         self._shape_ops = ops              # the engine borrows their pointers
         return handle
 
@@ -241,42 +260,102 @@ class EngineModel(nn.Module):
         self._last_ws = ws
         return ws
 
+    def _infer_call(self, eng, rgb: torch.Tensor, K, scale255: bool = False, normalize: bool = False, **fields) -> dict:
+        """One checked infer call of a UniDepthV1-family engine `eng` (`_INFER`: udb_infer_v1, udb_infer_v2old) on
+        `rgb` [B, 3, H, W] with the intrinsics `K` [B, 3, 3] or None -> {"intrinsics", "points", "depth" and, where the
+        args struct has it, "confidence"}, new tensors with their maps at (H, W), or at (`out_h`, `out_w`) when the
+        caller sets them.  `fields` are the caller's own fields of the args struct (`_INFER`); this fills the ones
+        InferV1Args and InferV2oldArgs share, with the cached workspace of (B, H, W)."""
+        args, infer_fn, workspace_fn = self._INFER
+        lib = cabi.lib()
+        a = args(**fields)
+        B, _, H, W = rgb.shape
+        h, w = fields.get("out_h", H), fields.get("out_w", W)
+        E = lambda *shape: torch.empty(shape, device=rgb.device, dtype=f32)
+        out = {"intrinsics": E(B, 3, 3), "points": E(B, 3, h, w), "depth": E(B, 1, h, w)}
+        if hasattr(a, "out_confidence"):
+            out["confidence"] = E(B, 1, h, w)
+            a.out_confidence = out["confidence"].data_ptr()
+        # the workspaces go with their engine (_drop_engine), so (B, H, W) names one
+        ws = self._workspace((B, H, W), lambda: getattr(lib, workspace_fn)(eng, B, H, W))
+        a.rgb, a.rgb_is_u8, a.scale255, a.normalize = rgb.data_ptr(), int(rgb.dtype == torch.uint8), int(scale255), int(normalize)
+        a.B, a.H, a.W = B, H, W
+        a.intrinsics = K.data_ptr() if K is not None else None
+        a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
+        a.out_intrinsics, a.out_points, a.out_depth = out["intrinsics"].data_ptr(), out["points"].data_ptr(), out["depth"].data_ptr()
+        cabi.check(getattr(lib, infer_fn)(eng, C.byref(a), C.c_void_p(torch.cuda.current_stream().cuda_stream)), infer_fn)
+        return out
+
+    # ------------------------------------------------------------------ entry points
+    def _infer(self, rgbs: torch.Tensor, intrinsics, shape, check=None, **fields) -> dict:
+        """The body of UniDepthV1.infer and UniDepthV2old.infer: `rgbs` [B, 3, H, W] through the engine of the network
+        shape `shape` (`_shape_engine` with `check`), with the class's own args-struct `fields` (`_infer_call`), which
+        also key the CUDA graph."""
+        dev = self._cuda_device()
+        rgbs, K, scale255, normalize = infer_inputs(rgbs, intrinsics, dev)
+        run = lambda eng, x, inputs: self._infer_call(eng, x, inputs.get("K"), scale255, normalize, **fields)
+        key = (shape, tuple(rgbs.shape), rgbs.dtype, scale255, normalize, K is not None) + tuple(fields.values())
+        return self._run_graphed(lambda: self._shape_engine(shape, check), run, rgbs, {} if K is None else {"K": K}, key)
+
+    def _check_eval_call(self, inputs):
+        """The evaluation call `model(inputs_dict, image_metas)` runs in eval mode only."""
+        if self.training or not isinstance(inputs, dict):
+            raise NotImplementedError(f"{type(self).__name__}.forward runs the evaluation call model(inputs_dict, "
+                                      "image_metas) in eval mode only (model.eval()); the training forward is out of scope")
+
+    @staticmethod
+    def _network_input_shape(image: torch.Tensor):
+        """(B, h, w) of a network input `image` [B, 3, h, w] (no resize or padding), whose sides are multiples of the
+        patch size.  Raises before anything touches the device."""
+        if image.ndim != 4 or image.shape[1] != 3:
+            raise ValueError(f"the network input must be [B, 3, h, w], not {tuple(image.shape)}")
+        B, _, h, w = image.shape
+        if h % PATCH or w % PATCH:
+            raise ValueError(f"network input {h}x{w} must be a multiple of {PATCH}: both sides must be multiples of the patch "
+                             "size")
+        return B, h, w
+
     # ------------------------------------------------------------------ CUDA graphs
-    def _run_graphed(self, run, rgb: torch.Tensor, inputs: dict, key: tuple, keep=None, output_buffers: bool = True) -> dict:
-        """`run(rgb, inputs)` -> outputs, eagerly or by replaying a CUDA graph cached under `key`.  The caller packs the
-        weights (`_weights()`) before this: a repack drops every graph, so none replays stale weights.  The graph reads
-        static copies of `rgb` and of the tensors in `inputs`, refreshed before every replay; `keep` is anything else a
-        captured kernel reads, which the cache entry must own.  `output_buffers=False`: return fresh tensors even when
-        `self.output_buffers` is set (it holds `infer`'s outputs only)."""
-        if not self.use_cuda_graph:
-            return run(rgb, inputs)
-        entry = self._graphs.get(key)
-        if entry is None:
-            static_in = rgb.clone()
-            static_inputs = {k: v.clone() for k, v in inputs.items()}
-            # warm-up on a side stream (allocator, per-shape tables, workspace), then capture
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                run(static_in, static_inputs)
-            torch.cuda.current_stream().wait_stream(side)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                static_out = run(static_in, static_inputs)
-            # the entry owns everything whose address the captured kernels read
-            entry = dict(graph=graph, inp=static_in, inputs=static_inputs, out=static_out, ws=self._last_ws, keep=keep)
-            self._graphs[key] = entry
-            while len(self._graphs) > self.max_cached_graphs:
-                self._graphs.popitem(last=False)
-        else:
-            self._graphs.move_to_end(key)
-        entry["inp"].copy_(rgb, non_blocking=True)
-        for k, v in inputs.items():
-            entry["inputs"][k].copy_(v, non_blocking=True)
-        entry["graph"].replay()
-        bufs = self.output_buffers if output_buffers else None
-        if bufs is not None:       # caller-provided destinations (e.g. the send slot of parallel.PeerGather): one copy, no clone
-            for k, v in entry["out"].items():
-                bufs[k].copy_(v)
-            return {k: bufs[k] for k in entry["out"]}
-        return {k: v.clone() for k, v in entry["out"].items()}
+    def _run_graphed(self, engine, run, rgb: torch.Tensor, inputs: dict, key: tuple, keep=None,
+                     output_buffers: bool = True) -> dict:
+        """`run(eng, rgb, inputs)` -> outputs on the engine `engine()` returns, eagerly or by replaying a CUDA graph
+        cached under `key`.  Everything runs with the model's device current (streams, the engine's allocations, the
+        per-device kernel attributes on the C side), so a model on cuda:1 works while cuda:0 is the process default.
+        `engine()` packs the weights (`_weights()`): a repack drops every graph, so none replays stale weights.  The
+        graph reads static copies of `rgb` and of the tensors in `inputs`, refreshed before every replay; `keep` is
+        anything else a captured kernel reads, which the cache entry must own.  `output_buffers=False`: return fresh
+        tensors even when `self.output_buffers` is set (it holds `infer`'s outputs only)."""
+        with torch.cuda.device(self._cuda_device()):
+            eng = engine()
+            if not self.use_cuda_graph:
+                return run(eng, rgb, inputs)
+            entry = self._graphs.get(key)
+            if entry is None:
+                static_in = rgb.clone()
+                static_inputs = {k: v.clone() for k, v in inputs.items()}
+                # warm-up on a side stream (allocator, per-shape tables, workspace), then capture
+                side = torch.cuda.Stream()
+                side.wait_stream(torch.cuda.current_stream())
+                with torch.cuda.stream(side):
+                    run(eng, static_in, static_inputs)
+                torch.cuda.current_stream().wait_stream(side)
+                graph = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(graph):
+                    static_out = run(eng, static_in, static_inputs)
+                # the entry owns everything whose address the captured kernels read
+                entry = dict(graph=graph, inp=static_in, inputs=static_inputs, out=static_out, ws=self._last_ws, keep=keep)
+                self._graphs[key] = entry
+                while len(self._graphs) > self.max_cached_graphs:
+                    self._graphs.popitem(last=False)
+            else:
+                self._graphs.move_to_end(key)
+            entry["inp"].copy_(rgb, non_blocking=True)
+            for k, v in inputs.items():
+                entry["inputs"][k].copy_(v, non_blocking=True)
+            entry["graph"].replay()
+            bufs = self.output_buffers if output_buffers else None
+            if bufs is not None:       # caller-provided destinations (e.g. the send slot of parallel.PeerGather): one copy, no clone
+                for k, v in entry["out"].items():
+                    bufs[k].copy_(v)
+                return {k: bufs[k] for k in entry["out"]}
+            return {k: v.clone() for k, v in entry["out"].items()}

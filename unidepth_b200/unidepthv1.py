@@ -18,9 +18,8 @@ function is unpinned (see DESIGN.md).
 """
 from __future__ import annotations
 
-import ctypes as C
 import operator
-from typing import Dict, Optional, Tuple
+from typing import Dict, Tuple
 
 import torch
 
@@ -30,7 +29,7 @@ from ._pack import (adapter, attn_block, c32, convnext_block, cross_block, h16, 
 from .spec import PATCH
 from .spec_v1 import (ENCODER_CONVNEXT, ENCODER_DINOV2, V1_INTERPOLATE_OFFSET, V1Spec, param_shapes, v1_paddings,
                       v1_shapes)
-from ._engine_model import HUB_KWARGS, EngineModel, PyTorchModelHubMixin, f32, infer_inputs
+from ._engine_model import HUB_KWARGS, EngineModel, PyTorchModelHubMixin, f32
 
 # ConvNeXt stages whose blocks run on e4m3 operands in precision "fp8" (engine_v1.cu kFp8Stage, the same fixed rule: a
 # stage runs e4m3 only where that is measured faster, which on an H100 is none of them, DESIGN.md section 8)
@@ -39,6 +38,7 @@ FP8_STAGES = (False, False, False, False)
 
 class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
     _ENGINE_FNS = ("udb_v1_create", "udb_v1_destroy", "udb_v1_set_weight", "udb_v1_set_scalar")
+    _INFER = (cabi.InferV1Args, "udb_infer_v1", "udb_v1_workspace_bytes")
 
     def __init__(self, config: dict, eps: float = 1e-6, **kwargs):
         super().__init__(config, eps, max_cached_workspaces=4)
@@ -58,9 +58,6 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         # same wgmma GEMM (include/udb.h udb_gemm_t.a_split_k), the encoder levels and the camera context stay f32, and
         # ViT-L's attention runs in the fp32 kernel.  The depth head runs as in "f16".  Slower; not a speed mode.
         self.precision = "f16"
-
-    def _fingerprint(self):
-        return (self.precision,) + super()._fingerprint()
 
     def _network_shape(self) -> Tuple[int, int]:
         """`image_shape` as (net_h, net_w), checked before anything is packed or launched for it."""
@@ -83,16 +80,9 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
                 "transpose; use a landscape or square shape (height <= width)")
         return h, w
 
-    # ------------------------------------------------------------------ weight packing
-    def _pack_tensors(self, dev):
-        """({engine tensor name: tensor on `dev`}, {scalar name: float}): plain torch layout work, the weights and the
-        two operands of the network shape `image_shape`.  The product packs the two parts separately (`_weights`,
-        `_shape_operands`); tests/test_engine_schedule_cpu.py runs this on the CPU to check, through the engine's dry run,
-        that the packer registers exactly the operands the C schedule asks for."""
-        T, S = self._pack_weights(dev)
-        T.update(self._shape_operands(self._network_shape(), dev))
-        return T, S
+    _default_shape = _network_shape
 
+    # ------------------------------------------------------------------ weight packing
     def _shape_operands(self, shape: Tuple[int, int], dev) -> Dict[str, torch.Tensor]:
         """The operands that depend on the network shape: "tokens_pos", the sine position embedding of the decoder's
         common grid plus the level embedding MLP of the four learned level vectors (decoder.py:410-433), and for DINOv2
@@ -111,15 +101,13 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         """The weight operands and scalars: everything but `_shape_operands`, so a change of network shape repacks
         nothing here."""
         s = self.spec
-        if self.precision not in ("split", "f16", "fp8"):
-            raise ValueError(f"precision must be 'split', 'f16' or 'fp8', not {self.precision!r}")
-        split, fp8 = self.precision == "split", self.precision == "fp8"
+        split, fp8, code = self._precision()
         sd = {k: v.detach() for k, v in self.state_dict().items()}
         # GEMM weight of the split-precision mode's operands: [N, 3K] = [hi | hi | lo], or f16 in the other modes
         s16 = split_weight if split else h16
         T: Dict[str, torch.Tensor] = {}
         # an engine without "precision" runs the f16 mode, so the f16 packing registers exactly the scalars it always has
-        S: Dict[str, float] = {"precision": 2.0} if fp8 else ({"precision": 1.0} if split else {})
+        S: Dict[str, float] = {"precision": float(code)} if code else {}
         pe, pd = "pixel_encoder.", "pixel_decoder."
         hid = s.hidden
 
@@ -200,8 +188,8 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         return T, S
 
     # ------------------------------------------------------------------ engine
-    def _engine_config(self) -> "cabi.V1Config":
-        """udb_v1_config_t of this model (include/udb.h)."""
+    def _engine_config(self, shape=None) -> "cabi.V1Config":
+        """udb_v1_config_t of this model at the network shape `shape` (default: `image_shape`) (include/udb.h)."""
         s = self.spec
         cfg = cabi.V1Config()
         for i in range(4):
@@ -209,40 +197,9 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         cfg.hidden, cfg.heads, cfg.expansion = s.hidden, s.heads, s.expansion
         for i in range(3):
             cfg.dec_depths[i] = s.dec_depths[i]
-        cfg.net_h, cfg.net_w = self._network_shape()
+        cfg.net_h, cfg.net_w = shape or self._network_shape()
         cfg.encoder = s.encoder
         return cfg
-
-    def _get_engine(self):
-        """The engine of the current network shape.  A new engine passes a dry run before it replaces the previous one,
-        which names any bound the shape breaks before anything is launched."""
-        shape = self._network_shape()
-
-        def check(handle):
-            lib = cabi.lib()
-            if lib.udb_v1_workspace_bytes(handle, 1, *shape) == 0:
-                raise NotImplementedError(f"UniDepthV1.image_shape {list(shape)}: {lib.udb_last_error().decode()}")
-
-        return self._shape_engine(shape, self._engine_config(), check)
-
-    def _forward_engine(self, rgb: torch.Tensor, K: Optional[torch.Tensor], skip_camera: bool, scale255: bool, normalize: bool):
-        eng = self._get_engine()
-        lib = cabi.lib()
-        dev = rgb.device
-        B, _, H, W = rgb.shape
-        ws = self._workspace((self._engine_key, B, H, W), lambda: lib.udb_v1_workspace_bytes(eng, B, H, W))
-        out = {"intrinsics": torch.empty((B, 3, 3), device=dev, dtype=f32),
-               "points": torch.empty((B, 3, H, W), device=dev, dtype=f32),
-               "depth": torch.empty((B, 1, H, W), device=dev, dtype=f32)}
-        a = cabi.InferV1Args()
-        a.rgb, a.rgb_is_u8, a.scale255, a.normalize = rgb.data_ptr(), int(rgb.dtype == torch.uint8), int(scale255), int(normalize)
-        a.B, a.H, a.W = B, H, W
-        a.intrinsics = K.data_ptr() if K is not None else None
-        a.skip_camera = int(bool(skip_camera and K is not None))
-        a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
-        a.out_intrinsics, a.out_points, a.out_depth = out["intrinsics"].data_ptr(), out["points"].data_ptr(), out["depth"].data_ptr()
-        cabi.check(lib.udb_infer_v1(eng, C.byref(a), C.c_void_p(torch.cuda.current_stream().cuda_stream)), "udb_infer_v1")
-        return out
 
     # ------------------------------------------------------------------ infer
     @torch.no_grad()
@@ -253,13 +210,13 @@ class UniDepthV1(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         if intrinsics is not None and intrinsics.ndim == 2:
             intrinsics = intrinsics.unsqueeze(0)
         shape = self._network_shape()
-        dev = self._cuda_device()
-        with torch.cuda.device(dev):
-            rgbs, K, scale255, normalize = infer_inputs(rgbs, intrinsics, dev)
-            self._get_engine()
-            run = lambda x, inputs: self._forward_engine(x, inputs.get("K"), skip_camera, scale255, normalize)
-            key = (shape, tuple(rgbs.shape), rgbs.dtype, scale255, normalize, K is not None, bool(skip_camera))
-            return self._run_graphed(run, rgbs, {} if K is None else {"K": K}, key)
+
+        def check(handle):      # a dry run names any bound the shape breaks before anything is launched
+            lib = cabi.lib()
+            if lib.udb_v1_workspace_bytes(handle, 1, *shape) == 0:
+                raise NotImplementedError(f"UniDepthV1.image_shape {list(shape)}: {lib.udb_last_error().decode()}")
+
+        return self._infer(rgbs, intrinsics, shape, check, skip_camera=int(bool(skip_camera and intrinsics is not None)))
 
     def forward(self, *args, **kwargs):
         raise NotImplementedError("training / validation forward of UniDepthV1 is out of scope; use .infer()")

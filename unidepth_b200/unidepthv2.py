@@ -69,21 +69,18 @@ class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         return bool(self.fuse_ln and self.precision == "f16")
 
     def _fingerprint(self):
-        return (self.precision, self._fuse()) + super()._fingerprint()
+        return super()._fingerprint() + (self._fuse(),)
 
-    def _pack_tensors(self, dev):
+    def _pack_weights(self, dev):
         """({engine tensor name: tensor on `dev`}, {scalar name: float}) (names: include/udb.h, DESIGN.md 'packed
-        tensors'): plain torch layout work, no kernel involved.  `_weights` is the only product caller (CUDA device);
-        tests/test_engine_schedule_cpu.py runs it on the CPU to check, through the engine's dry run, that every packing
-        mode registers exactly the operands the C schedule asks for."""
+        tensors'): plain torch layout work, no kernel involved.  UniDepthV2 has no shape operands: its engine keeps its
+        per-grid tables itself, so this is all of `_pack_tensors`."""
         s = self.spec
         if s.kernel_size != 3:
             raise NotImplementedError(f"pixel_decoder.kernel_size={s.kernel_size}: the residual conv units run as 3x3 "
                                       "convolutions (every shipped UniDepthV2 config sets 3)")
         sd = {k: v.detach() for k, v in self.state_dict().items()}
-        if self.precision not in ("f16", "split", "fp8"):
-            raise ValueError(f"precision must be 'f16', 'split' or 'fp8', not {self.precision!r}")
-        split, fp8 = self.precision == "split", self.precision == "fp8"
+        split, fp8, code = self._precision()
         fuse = self._fuse()
 
         d, hid = s.embed_dim, s.hidden
@@ -107,7 +104,7 @@ class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         pe = "pixel_encoder."
         T = pack_vit_encoder(sd, d, s.depth, dev, split, fuse, fp8=fp8)
         T["pos"] = c32(sd[pe + "pos_embed"].reshape(-1, d))      # the stored grid: the engine resizes it per shape
-        S: Dict[str, float] = {"precision": 1.0 if split else (2.0 if fp8 else 0.0), "fuse_ln": 1.0 if fuse else 0.0}
+        S: Dict[str, float] = {"precision": float(code), "fuse_ln": 1.0 if fuse else 0.0}
         T["norm_w"], T["norm_b"] = c32(sd[pe + "norm.weight"]), c32(sd[pe + "norm.bias"])
 
         pd = "pixel_decoder."
@@ -215,14 +212,14 @@ class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         super()._drop_engine()
         self._engine_shapes = set()
 
-    def _engine_config(self, T: dict) -> "cabi.Config":
-        """udb_config_t of this model (include/udb.h)."""
+    def _engine_config(self, shape=None) -> "cabi.Config":
+        """udb_config_t of this model (include/udb.h).  The engine takes every network shape: `shape` is not read."""
         s, sc = self.spec, self.shape_constraints
         cfg = cabi.Config()
         cfg.embed_dim, cfg.depth, cfg.enc_heads = s.embed_dim, s.depth, s.enc_heads
         for i, t in enumerate(s.taps):
             cfg.taps[i] = t
-        cfg.pos_grid = int(math.isqrt(T["pos"].shape[0] - 1))
+        cfg.pos_grid = int(math.isqrt(self.pixel_encoder.pos_embed.numel() // s.embed_dim - 1))
         cfg.hidden, cfg.dec_heads, cfg.expansion, cfg.out_dim = s.hidden, s.dec_heads, s.expansion, s.out_dim
         cfg.n_stages = len(s.dec_depths)
         for i, dd in enumerate(s.dec_depths):
@@ -232,20 +229,22 @@ class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         return cfg
 
     def _get_engine(self):
-        T, _ = self._weights()
+        """The engine of the current shape constraints, rebuilt when they change or once it holds the per-grid tables of
+        more than `max_engine_shapes` grids (the rebuild frees them)."""
+        self._weights()
         sc = self.shape_constraints
         key = (tuple(sc["ratio_bounds"]), sc["pixels_min"], sc["pixels_max"])
+        if len(self._engine_shapes) > self.max_engine_shapes:
+            self._drop_engine()
         if self._engine is not None and self._engine_key == key:
             return self._engine
-        self._drop_engine()
-        return self._create_engine(self._engine_config(T), key)
+        return self._create_engine(self._engine_config(), key)
 
-    def _forward_engine(self, rgb: torch.Tensor, geom: dict, normalize: bool, level, camera_k=None, rays_in=None,
+    def _forward_engine(self, eng, rgb: torch.Tensor, geom: dict, normalize: bool, level, camera_k=None, rays_in=None,
                         camera_model=0, camera_params=None, match_pads=None):
-        """The whole path as ONE C call (udb_infer_v2): torch only allocates outputs / workspace.  With `match_pads`
-        (device int32 [B, 4], network-only level, geom["match_hw"]) the engine matches the outputs to the ground truth
-        as `forward_test` returns them."""
-        eng = self._get_engine()
+        """The whole path as ONE C call (udb_infer_v2) of the engine `eng`: torch only allocates outputs / workspace.
+        With `match_pads` (device int32 [B, 4], network-only level, geom["match_hw"]) the engine matches the outputs to
+        the ground truth as `forward_test` returns them."""
         lib = cabi.lib()
         dev = rgb.device
         B, _, H, W = rgb.shape
@@ -382,10 +381,7 @@ class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         return out["points"], out["confidence"], out["intrinsics"]
 
     def _network_outputs(self, rgbs, rays=None):
-        assert rgbs.ndim == 4 and rgbs.shape[1] == 3, "rgbs must be [B,3,H,W]"
-        B, _, H, W = rgbs.shape
-        if H % PATCH or W % PATCH:
-            raise ValueError(f"network input {H}x{W} must be a multiple of {PATCH}")
+        B, H, W = self._network_input_shape(rgbs)
         rgbs = self._to_device_input(rgbs.float())
         geom = dict(paddings=(0, 0, 0, 0), padded_hw=(H, W), factor=1.0, net_hw=(H, W), out_hw=(H, W))
         rays_in = None
@@ -436,11 +432,7 @@ class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         the host.  CUDA graphs are cached per (B, h, w, H, W, camera source): the paddings are graph inputs, so a new
         batch with other paddings replays.  The caller's `inputs` is left unchanged."""
         image, gt = inputs["image"], inputs["depth"]
-        if image.ndim != 4 or image.shape[1] != 3:
-            raise ValueError(f"inputs['image'] must be [B, 3, h, w], not {tuple(image.shape)}")
-        B, _, h, w = image.shape
-        if h % PATCH or w % PATCH:
-            raise ValueError(f"network input {h}x{w} must be a multiple of {PATCH}")
+        B, h, w = self._network_input_shape(image)
         if gt.ndim != 4:
             raise ValueError(f"inputs['depth'] must be a [B, 1, H, W] ground truth, not {tuple(gt.shape)}")
         pads = self._match_paddings(inputs, image_metas, B, h, w)
@@ -458,8 +450,7 @@ class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
     def forward(self, inputs=None, image_metas=None, *args, **kwargs):
         """Evaluation-mode `forward` of the reference dispatches to `forward_test` (unidepthv2.py:162-166);
         training is out of scope."""
-        if self.training or not isinstance(inputs, dict):
-            raise NotImplementedError("training forward is out of scope; use .infer() / .forward_test() in eval mode")
+        self._check_eval_call(inputs)
         return self.forward_test(inputs, image_metas)
 
     def _to_device_input(self, rgb):
@@ -469,22 +460,16 @@ class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         return rgb.contiguous()
 
     def _run(self, rgb, geom, level, normalize, camera, key_extra, rays_in=None, match_pads=None):
-        """Common tail of infer / network_forward / forward_test: camera handling, the engine call, CUDA graph cache.
-        Everything runs with the model's device current (streams, cudaMalloc of the engine tables, the per-device
-        kernel attributes on the C side), so a model on cuda:1 works while cuda:0 is the process default."""
-        with torch.cuda.device(self.device):
-            return self._run_on_device(rgb, geom, level, normalize, camera, key_extra, rays_in, match_pads)
-
-    def _run_on_device(self, rgb, geom, level, normalize, camera, key_extra, rays_in=None, match_pads=None):
+        """Common tail of infer / network_forward / forward_test: camera handling, then the engine call on the CUDA graph
+        cache (`_run_graphed`)."""
         B, _, H, W = rgb.shape
         dev = rgb.device
         nh, nw = geom["net_hw"]
         gh, gw = nh // PATCH, nw // PATCH
         bands = self.spec.hidden // 2
-        # Weights first: a repack drops the engine, its workspaces and every captured graph, so the tensors created below
-        # for a graph to read must not be made before it.  (A frequency table once was, and a graph captured by the first
-        # infer then replayed the ray embedding from freed memory.)
-        self._weights()
+        # The frequency tables are never dropped and every graph entry owns the one it reads (`keep`), so the repack of
+        # `_get_engine` below, which drops the graphs, frees none.  (A table that a repack once freed was replayed from
+        # freed memory.)
         skey = (gh, gw, bands, dev.index)
         if skey not in self._scales_cache:
             # positional_embedding.py:231-233 -- computed with the same torch expression (host, once per grid)
@@ -494,11 +479,9 @@ class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
 
         source, cam = self._camera_source(camera, rays_in, B, geom, dev)
         model = source[1] if isinstance(source, tuple) else 0
-        if len(self._engine_shapes) > self.max_engine_shapes:
-            self._drop_engine()       # too many distinct grids seen: rebuild (frees the engine's per-shape tables)
 
-        def run(inp, cam):
-            return self._forward_engine(inp, geom, normalize, level, camera_k=cam.get("K"), rays_in=cam.get("rays"),
+        def run(eng, inp, cam):
+            return self._forward_engine(eng, inp, geom, normalize, level, camera_k=cam.get("K"), rays_in=cam.get("rays"),
                                         camera_model=model, camera_params=cam.get("params"), match_pads=cam.get("pads"))
 
         if match_pads is not None:
@@ -507,4 +490,4 @@ class UniDepthV2(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         # the entry owns static copies of the camera tensors (and of forward_test's paddings), refreshed before every
         # replay like the image.
         key = (B, H, W, rgb.dtype, bool(normalize)) + tuple(key_extra) + (source,)
-        return self._run_graphed(run, rgb, cam, key, keep=scales)
+        return self._run_graphed(self._get_engine, run, rgb, cam, key, keep=scales)

@@ -26,12 +26,12 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-from typing import Dict, Optional, Tuple
+from typing import Dict, Tuple
 
 import torch
 
 from . import _cabi as cabi
-from ._engine_model import HUB_KWARGS, EngineModel, PyTorchModelHubMixin, f32, infer_inputs
+from ._engine_model import HUB_KWARGS, EngineModel, PyTorchModelHubMixin, f32
 from ._pack import (adapter, attn_block, c32, convnext_block, cross_block, h16, latents, mlp, pack_vit_encoder,
                     pos_table_by_size, split_weight, tokens_pos)
 from .spec import PATCH
@@ -49,6 +49,7 @@ def v2old_geometry(H: int, W: int, level: int, pixels_bounds) -> Tuple[Tuple[int
 
 class UniDepthV2old(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
     _ENGINE_FNS = ("udb_v2old_create", "udb_v2old_destroy", "udb_v2old_set_weight", "udb_v2old_set_scalar")
+    _INFER = (cabi.InferV2oldArgs, "udb_infer_v2old", "udb_v2old_workspace_bytes")
 
     def __init__(self, config: dict, eps: float = 1e-6, **kwargs):
         super().__init__(config, eps, max_cached_workspaces=4)
@@ -70,21 +71,11 @@ class UniDepthV2old(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         # speed mode.  Changing it repacks the weights.
         self.precision = "f16"
 
-    def _fingerprint(self):
-        return (self.precision,) + super()._fingerprint()
+    def _default_shape(self) -> Tuple[int, int]:
+        """The network shape of a 480 x 640 input at the maximum level."""
+        return v2old_geometry(480, 640, 10, self.shape_constraints["pixels_bounds_ori"])[0]
 
     # ------------------------------------------------------------------ weight packing
-    def _pack_tensors(self, dev, shape: Optional[Tuple[int, int]] = None):
-        """({engine tensor name: tensor on `dev`}, {scalar name: float}) of the weights and of the operands of the
-        network shape `shape` (default: the shape of a 480 x 640 input at the maximum level).  The product packs the
-        two parts separately (`_weights`, `_shape_operands`); tests/test_v2old_cpu.py runs this on the CPU to check,
-        through the engine's dry run, that the packer registers exactly the operands the C schedule asks for."""
-        T, S = self._pack_weights(dev)
-        if shape is None:
-            shape, _ = v2old_geometry(480, 640, 10, self.shape_constraints["pixels_bounds_ori"])
-        T.update(self._shape_operands(shape, dev))
-        return T, S
-
     def _shape_operands(self, shape: Tuple[int, int], dev) -> Dict[str, torch.Tensor]:
         """The operands that depend on the network shape: "pos", the DINOv2 position table resized (bicubic, to the
         patch grid's size: interpolate_offset 0, dinov2.py:267-304); "tokens_pos", the sine position embedding of the
@@ -106,15 +97,13 @@ class UniDepthV2old(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
 
     def _pack_weights(self, dev):
         s = self.spec
-        if self.precision not in ("split", "f16", "fp8"):
-            raise ValueError(f"precision must be 'split', 'f16' or 'fp8', not {self.precision!r}")
-        split, fp8 = self.precision == "split", self.precision == "fp8"
+        split, fp8, code = self._precision()
         # GEMM weight of the split mode's operands: [N, 3K] = [hi | hi | lo], or f16 in the other modes
         s16 = split_weight if split else h16
         sd = {k: v.detach() for k, v in self.state_dict().items()}
         T: Dict[str, torch.Tensor] = {}
         # an engine without "precision" runs the f16 mode, so the f16 packing registers exactly the scalars it always has
-        S: Dict[str, float] = {"precision": 2.0} if fp8 else ({"precision": 1.0} if split else {})
+        S: Dict[str, float] = {"precision": float(code)} if code else {}
         pd, dl = "pixel_decoder.", "pixel_decoder.depth_layer."
         hid, D = s.hidden, s.embed_dim
 
@@ -191,8 +180,8 @@ class UniDepthV2old(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         return T, S
 
     # ------------------------------------------------------------------ engine
-    def _engine_config(self, shape: Tuple[int, int]) -> "cabi.V2oldConfig":
-        """udb_v2old_config_t of this model at the network shape `shape` (include/udb.h)."""
+    def _engine_config(self, shape=None) -> "cabi.V2oldConfig":
+        """udb_v2old_config_t of this model at the network shape `shape` (default: `_default_shape()`) (include/udb.h)."""
         s = self.spec
         cfg = cabi.V2oldConfig()
         cfg.embed_dim, cfg.enc_depth, cfg.enc_heads = s.embed_dim, s.enc_depth, s.enc_heads
@@ -200,29 +189,8 @@ class UniDepthV2old(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
             cfg.output_idx[i] = s.output_idx[i]
         cfg.hidden, cfg.heads, cfg.expansion = s.hidden, s.heads, s.expansion
         cfg.nystrom_depth = s.dec_depths[0]
-        cfg.net_h, cfg.net_w = shape
+        cfg.net_h, cfg.net_w = shape or self._default_shape()
         return cfg
-
-    def _forward_engine(self, rgb: torch.Tensor, K: Optional[torch.Tensor], scale255: bool, normalize: bool, mode: int):
-        eng = self._engine
-        lib = cabi.lib()
-        dev = rgb.device
-        B, _, H, W = rgb.shape
-        ws = self._workspace((self._engine_key, B, H, W), lambda: lib.udb_v2old_workspace_bytes(eng, B, H, W))
-        out = {"intrinsics": torch.empty((B, 3, 3), device=dev, dtype=f32),
-               "points": torch.empty((B, 3, H, W), device=dev, dtype=f32),
-               "depth": torch.empty((B, 1, H, W), device=dev, dtype=f32),
-               "confidence": torch.empty((B, 1, H, W), device=dev, dtype=f32)}
-        a = cabi.InferV2oldArgs()
-        a.rgb, a.rgb_is_u8, a.scale255, a.normalize = rgb.data_ptr(), int(rgb.dtype == torch.uint8), int(scale255), int(normalize)
-        a.B, a.H, a.W = B, H, W
-        a.intrinsics = K.data_ptr() if K is not None else None
-        a.interpolation = mode
-        a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
-        a.out_intrinsics, a.out_points = out["intrinsics"].data_ptr(), out["points"].data_ptr()
-        a.out_depth, a.out_confidence = out["depth"].data_ptr(), out["confidence"].data_ptr()
-        cabi.check(lib.udb_infer_v2old(eng, C.byref(a), C.c_void_p(torch.cuda.current_stream().cuda_stream)), "udb_infer_v2old")
-        return out
 
     # ------------------------------------------------------------------ infer
     @torch.no_grad()
@@ -231,48 +199,17 @@ class UniDepthV2old(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         if self.interpolation_mode not in cabi.V2OLD_INTERP_MODES:
             raise NotImplementedError(f"interpolation_mode {self.interpolation_mode!r}: only 'bilinear' and 'nearest-exact' "
                                       "are implemented")
-        mode = cabi.V2OLD_INTERP_MODES[self.interpolation_mode]
         if rgbs.ndim == 3:
             rgbs = rgbs.unsqueeze(0)
         if intrinsics is not None and intrinsics.ndim == 2:
             intrinsics = intrinsics.unsqueeze(0)
-        dev = self._cuda_device()
         B, _, H, W = rgbs.shape
         level = check_resolution(self.resolution_level)
         check_ratio((H, W), self.shape_constraints["ratio_bounds"])
         shape, _ = v2old_geometry(H, W, level, self.shape_constraints["pixels_bounds_ori"])
-        with torch.cuda.device(dev):
-            rgbs, K, scale255, normalize = infer_inputs(rgbs, intrinsics, dev)
-            self._shape_engine(shape, self._engine_config(shape))
-            run = lambda x, inputs: self._forward_engine(x, inputs.get("K"), scale255, normalize, mode)
-            key = (shape, tuple(rgbs.shape), rgbs.dtype, scale255, normalize, K is not None, mode)
-            return self._run_graphed(run, rgbs, {} if K is None else {"K": K}, key)
+        return self._infer(rgbs, intrinsics, shape, interpolation=cabi.V2OLD_INTERP_MODES[self.interpolation_mode])
 
     # ------------------------------------------------------------------ forward
-    def _forward_network(self, image: torch.Tensor, K: Optional[torch.Tensor], out_hw: Tuple[int, int]):
-        """One network-only call of the engine (udb_infer_v2old with network_only = 1) on the normalised f32 network
-        input `image` [B, 3, h, w] -> the outputs of `forward`, maps at `out_hw`."""
-        eng = self._engine
-        lib = cabi.lib()
-        dev = image.device
-        B, _, h, w = image.shape
-        H, W = out_hw
-        ws = self._workspace((self._engine_key, B, h, w), lambda: lib.udb_v2old_workspace_bytes(eng, B, h, w))
-        out = {"K": torch.empty((B, 3, 3), device=dev, dtype=f32),
-               "depth": torch.empty((B, 1, H, W), device=dev, dtype=f32),
-               "confidence": torch.empty((B, 1, H, W), device=dev, dtype=f32),
-               "points": torch.empty((B, 3, H, W), device=dev, dtype=f32),
-               "depth_features": torch.empty((B, (h // PATCH) * (w // PATCH), self.spec.hidden), device=dev, dtype=f32)}
-        a = cabi.InferV2oldArgs()
-        a.rgb, a.B, a.H, a.W = image.data_ptr(), B, h, w
-        a.intrinsics = K.data_ptr() if K is not None else None
-        a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
-        a.out_intrinsics, a.out_points = out["K"].data_ptr(), out["points"].data_ptr()
-        a.out_depth, a.out_confidence = out["depth"].data_ptr(), out["confidence"].data_ptr()
-        a.network_only, a.out_h, a.out_w, a.out_depth_features = 1, H, W, out["depth_features"].data_ptr()
-        cabi.check(lib.udb_infer_v2old(eng, C.byref(a), C.c_void_p(torch.cuda.current_stream().cuda_stream)), "udb_infer_v2old")
-        return out
-
     @torch.no_grad()
     def forward(self, inputs, image_metas=None):
         """The reference's evaluation call `model(inputs, image_metas)` (unidepthv2_old.py:134-196), in eval mode only:
@@ -290,18 +227,14 @@ class UniDepthV2old(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
         "features", "tokens", "global_tokens" and "camera_tokens" to it.  `precision` applies as in `infer`; the outputs
         are new tensors (`output_buffers` holds `infer`'s only).  Training mode raises NotImplementedError: the training
         forward is out of scope."""
-        if self.training or not isinstance(inputs, dict):
-            raise NotImplementedError("UniDepthV2old.forward runs the evaluation call model(inputs_dict, image_metas) in "
-                                      "eval mode only (model.eval()); the training forward is out of scope")
+        self._check_eval_call(inputs)
         for k in ("image", "depth"):
             if k not in inputs:
                 raise ValueError(f"inputs needs {k!r}: the network input and the ground truth whose size the outputs take")
         image = inputs["image"]
-        if image.ndim != 4 or image.shape[1] != 3 or not image.dtype.is_floating_point:
-            raise ValueError(f"inputs['image'] must be a float [B, 3, h, w] tensor, not {image.dtype} {tuple(image.shape)}")
-        B, _, h, w = image.shape
-        if h % PATCH or w % PATCH:
-            raise ValueError(f"inputs['image'] is {h}x{w}: both sides must be multiples of the patch size {PATCH}")
+        B, h, w = self._network_input_shape(image)
+        if not image.dtype.is_floating_point:
+            raise ValueError(f"inputs['image'] must be a float tensor, not {image.dtype}")
         H, W = (int(v) for v in inputs["depth"].shape[-2:])
         K = inputs.get("K")
         if K is not None:
@@ -311,11 +244,15 @@ class UniDepthV2old(EngineModel, PyTorchModelHubMixin, **HUB_KWARGS):
                 raise ValueError(f"inputs['K'] with a ground truth of {H}x{W} and an image of {h}x{w}: the rays of K are "
                                  "reshaped to the image grid, so the two sizes must be equal")
         dev = self._cuda_device()
-        shape = (h, w)
-        with torch.cuda.device(dev):
-            x = image.to(dev, f32).contiguous()
-            Kd = K.to(dev, f32).contiguous() if K is not None else None
-            self._shape_engine(shape, self._engine_config(shape))
-            run = lambda x, ins: self._forward_network(x, ins.get("K"), (H, W))
-            key = ("forward", B, h, w, H, W, K is not None)
-            return self._run_graphed(run, x, {} if Kd is None else {"K": Kd}, key, output_buffers=False)
+        x = image.to(dev, f32).contiguous()
+        ins = {} if K is None else {"K": K.to(dev, f32).contiguous()}
+
+        def run(eng, x, ins):
+            # the network-only call of udb_infer_v2old on the normalised network input; maps at the ground truth's size
+            feats = torch.empty((B, (h // PATCH) * (w // PATCH), self.spec.hidden), device=dev, dtype=f32)
+            out = self._infer_call(eng, x, ins.get("K"), network_only=1, out_h=H, out_w=W,
+                                   out_depth_features=feats.data_ptr())
+            return {"K": out.pop("intrinsics"), **out, "depth_features": feats}
+
+        key = ("forward", B, h, w, H, W, K is not None)
+        return self._run_graphed(lambda: self._shape_engine((h, w)), run, x, ins, key, output_buffers=False)
