@@ -9,7 +9,7 @@ namespace udb {
 constexpr int AT_BQ = 128;       // queries per CTA (two warpgroups of 64)
 constexpr int AT_BK = 128;       // keys per tile
 constexpr int AT_STAGES = 3;     // K / V rings
-constexpr int AT_THREADS = 288;  // two consumer warpgroups + the TMA warp
+constexpr int AT_THREADS = 256;  // two warpgroups, two CTAs per SM
 
 struct AttnArgs {
   __half* out;
@@ -25,23 +25,61 @@ __device__ __forceinline__ float ex2(float x) {
   return y;
 }
 
+// Online-softmax step of one key tile, in place on the S accumulator fragment: keys >= kv_left are masked, S becomes the
+// unnormalised P = 2^(S * sc - m_new), the running max and row sums advance, and alpha[h] = 2^(m_old - m_new) is the
+// factor the caller applies to O (rows lane/4 and lane/4 + 8 of the warp's 16; cq as in the kernel).
+__device__ __forceinline__ void attn_softmax_tile(float (&s)[AT_BK / 2], int kv_left, int cq, float sc, float (&m_run)[2],
+                                                  float (&l_run)[2], float (&alpha)[2]) {
+  if (kv_left < AT_BK) {
+#pragma unroll
+    for (int i = 0; i < AT_BK / 2; ++i)
+      if (8 * (i >> 2) + cq + (i & 1) >= kv_left) s[i] = -INFINITY;
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float mx = -INFINITY;
+#pragma unroll
+    for (int jj = 0; jj < AT_BK / 8; ++jj) mx = fmaxf(mx, fmaxf(s[4 * jj + 2 * h], s[4 * jj + 2 * h + 1]));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+    const float m_new = fmaxf(m_run[h], mx * sc);
+    alpha[h] = ex2(m_run[h] - m_new);                   // 0 on the first tile
+    m_run[h] = m_new;
+    float ls = 0.f;
+#pragma unroll
+    for (int jj = 0; jj < AT_BK / 8; ++jj) {
+      const float e0 = ex2(fmaf(s[4 * jj + 2 * h], sc, -m_new));
+      const float e1 = ex2(fmaf(s[4 * jj + 2 * h + 1], sc, -m_new));
+      s[4 * jj + 2 * h] = e0;
+      s[4 * jj + 2 * h + 1] = e1;
+      ls += e0 + e1;
+    }
+    l_run[h] = fmaf(l_run[h], alpha[h], ls);
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
-// One CTA = one (batch, head, 128-query tile).  Warps 0..7 are two consumer warpgroups, warpgroup g owns queries
-// [64g, 64g+64); warp 8 is the TMA producer (Q once, K / V tiles of 128 keys through AT_STAGES-deep rings).  Per key tile
-// a warpgroup computes S = Q K^T with one m64n128 wgmma chain (both operands in shared memory), runs the online softmax
-// on the accumulator registers (a row lives in the four lanes of a quad: max / sum by two shuffles), converts P to f16
-// in place -- the m64n128 accumulator fragment of keys [16k, 16k+16) is exactly the register A fragment of the k-th
-// m64k16 step -- and accumulates O += P V with register-A wgmmas (V read MN-major from shared memory).  P never touches
-// shared memory; the two warpgroups run independently and overlap each other's softmax with their MMAs.
+// One CTA = one (batch, head, 128-query tile), 256 threads: two warpgroups, warpgroup g owns queries [64g, 64g+64).  Per
+// key tile a warpgroup computes S = Q K^T with one m64n128 wgmma chain (both operands in shared memory), runs the online
+// softmax on the accumulator registers (a row lives in the four lanes of a quad: max / sum by two shuffles), converts P
+// to f16 in place -- the m64n128 accumulator fragment of keys [16k, 16k+16) is exactly the register A fragment of the
+// k-th m64k16 step -- and accumulates O += P V with register-A wgmmas (V read MN-major from shared memory).  P never
+// touches shared memory.
+//
+// Two CTAs share an SM (128 registers per thread, 112.25 KB of shared memory each), so one CTA's MMAs run under the
+// other's softmax and each scheduler has four math warps to pick from.  There is no producer warp: thread 0 issues the
+// TMA loads of Q and of the first AT_STAGES K / V tiles, and afterwards the last of the eight warps to release a K or V
+// stage (a shared-memory counter per stage) loads tile j + AT_STAGES into it, so no warp waits for the others.
 // ---------------------------------------------------------------------------------------------
 template <int HD>
-__global__ void __launch_bounds__(AT_THREADS, 1)
+__global__ void __launch_bounds__(AT_THREADS, 2)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const AttnArgs p) {
   static_assert(HD == 64, "head_dim 64 only");
   constexpr int kQBytes = AT_BQ * HD * 2;      // 16 KB
   constexpr int kKBytes = AT_BK * HD * 2;      // 16 KB
   constexpr int NS = AT_STAGES;
+  constexpr uint32_t kWarps = AT_THREADS / 32;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sQ = smem;
   uint8_t* sK = sQ + kQBytes;                  // NS stages
@@ -50,8 +88,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   uint64_t* q_full = bars;
   uint64_t* k_full = bars + 1;             // [NS]
   uint64_t* v_full = k_full + NS;          // [NS]
-  uint64_t* k_empty = v_full + NS;         // [NS]  every consumer warp's QK^T of the tile has completed
-  uint64_t* v_empty = k_empty + NS;        // [NS]  every consumer warp's PV of the tile has completed
+  uint32_t* k_done = reinterpret_cast<uint32_t*>(v_full + NS);   // [NS]  warps that finished with the stage's K tile
+  uint32_t* v_done = k_done + NS;                                // [NS]  ... and with its V tile (running counts)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -59,6 +97,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const int head = blockIdx.y;
   const int b = blockIdx.z;
   const int n_tiles = p.n_kv_tiles;
+  const int kc = p.k_col0 + head * HD, vc = p.v_col0 + head * HD;
   pdl_launch_dependents();
 
   if (threadIdx.x == 0) {
@@ -70,42 +109,37 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     for (int i = 0; i < NS; ++i) {
       mbar_init(&k_full[i], 1);
       mbar_init(&v_full[i], 1);
-      mbar_init(&k_empty[i], 8);
-      mbar_init(&v_empty[i], 8);
+      k_done[i] = 0;
+      v_done[i] = 0;
     }
     fence_barrier_init();
   }
   __syncthreads();
   pdl_wait();
-
-  if (warp == 8) {
-    const bool leader = elect_one();
-    if (leader) {
-      mbar_arrive_expect_tx(q_full, kQBytes);
-      tma_load_3d(sQ, &tmQ, q_full, p.q_col0 + head * HD, q0, b);
+  if (threadIdx.x == 0) {
+    mbar_arrive_expect_tx(q_full, kQBytes);
+    tma_load_3d(sQ, &tmQ, q_full, p.q_col0 + head * HD, q0, b);
+    for (int j = 0; j < NS && j < n_tiles; ++j) {
+      mbar_arrive_expect_tx(&k_full[j], kKBytes);
+      tma_load_3d(sK + j * kKBytes, &tmK, &k_full[j], kc, j * AT_BK, b);
+      mbar_arrive_expect_tx(&v_full[j], kKBytes);
+      tma_load_3d(sV + j * kKBytes, &tmV, &v_full[j], vc, j * AT_BK, b);
     }
-    __syncwarp();
-    int st = 0;
-    uint32_t ph = 1;
-    for (int j = 0; j < n_tiles; ++j) {
-      mbar_wait(&k_empty[st], ph);
-      if (leader) {
-        mbar_arrive_expect_tx(&k_full[st], kKBytes);
-        tma_load_3d(sK + st * kKBytes, &tmK, &k_full[st], p.k_col0 + head * HD, j * AT_BK, b);
-      }
-      __syncwarp();
-      mbar_wait(&v_empty[st], ph);
-      if (leader) {
-        mbar_arrive_expect_tx(&v_full[st], kKBytes);
-        tma_load_3d(sV + st * kKBytes, &tmV, &v_full[st], p.v_col0 + head * HD, j * AT_BK, b);
-      }
-      __syncwarp();
-      if (++st == NS) { st = 0; ph ^= 1; }
-    }
-    return;
   }
+  // A warp is done with tile j's K (or V) in stage st once its wgmmas that read it have completed; the eighth warp to
+  // say so refills the stage with tile j + NS.  The fences order the wgmma reads before the count, and the count before
+  // the refill.
+  const auto release = [&](uint32_t* done, uint64_t* full, uint8_t* buf, const CUtensorMap* tm, int col, int st, int j) {
+    if (lane == 0) {
+      __threadfence_block();
+      if (atomicAdd(&done[st], 1u) % kWarps == kWarps - 1 && j + NS < n_tiles) {
+        __threadfence_block();
+        mbar_arrive_expect_tx(&full[st], kKBytes);
+        tma_load_3d(buf + st * kKBytes, tm, &full[st], col, (j + NS) * AT_BK, b);
+      }
+    }
+  };
 
-  // ------------------------------------------------------------------ consumer warpgroups
   const int wg = warp >> 2, wq = warp & 3;
   const int cq = 2 * (lane & 3);                       // first of this thread's two columns in every 8-column group
   const float sc = p.scale_log2;
@@ -118,7 +152,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   int st = 0;
   uint32_t ph = 0;
   for (int j = 0; j < n_tiles; ++j) {
-    float s[AT_BK / 2];
+    float s[AT_BK / 2], alpha[2];
     mbar_wait(&k_full[st], ph);
     {
       const uint64_t dk = gmma_desc_sw128(smem_u32(sK + st * kKBytes), 16, 1024);
@@ -129,39 +163,15 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       wgmma_wait<0>();
       wgmma_fence_regs(s);
     }
-    if (lane == 0) mbar_arrive(&k_empty[st]);
-    const int kv_left = p.seq_k - j * AT_BK;           // valid keys in this tile (>= 1)
-    if (kv_left < AT_BK) {
+    release(k_done, k_full, sK, &tmK, kc, st, j);
+    attn_softmax_tile(s, p.seq_k - j * AT_BK, cq, sc, m_run, l_run, alpha);
 #pragma unroll
-      for (int i = 0; i < AT_BK / 2; ++i)
-        if (8 * (i >> 2) + cq + (i & 1) >= kv_left) s[i] = -INFINITY;
-    }
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      float mx = -INFINITY;
-#pragma unroll
-      for (int jj = 0; jj < AT_BK / 8; ++jj) mx = fmaxf(mx, fmaxf(s[4 * jj + 2 * h], s[4 * jj + 2 * h + 1]));
-      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-      const float m_new = fmaxf(m_run[h], mx * sc);
-      const float alpha = ex2(m_run[h] - m_new);        // 0 on the first tile
-      m_run[h] = m_new;
-      float ls = 0.f;
-#pragma unroll
-      for (int jj = 0; jj < AT_BK / 8; ++jj) {
-        const float e0 = ex2(fmaf(s[4 * jj + 2 * h], sc, -m_new));
-        const float e1 = ex2(fmaf(s[4 * jj + 2 * h + 1], sc, -m_new));
-        s[4 * jj + 2 * h] = e0;
-        s[4 * jj + 2 * h + 1] = e1;
-        ls += e0 + e1;
-      }
-      l_run[h] = fmaf(l_run[h], alpha, ls);
+    for (int h = 0; h < 2; ++h)
 #pragma unroll
       for (int jj = 0; jj < HD / 8; ++jj) {
-        o[4 * jj + 2 * h] *= alpha;
-        o[4 * jj + 2 * h + 1] *= alpha;
+        o[4 * jj + 2 * h] *= alpha[h];
+        o[4 * jj + 2 * h + 1] *= alpha[h];
       }
-    }
     uint32_t pa[AT_BK / 16][4];
 #pragma unroll
     for (int kk = 0; kk < AT_BK / 16; ++kk)
@@ -178,7 +188,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       wgmma_wait<0>();
       wgmma_fence_regs(o);
     }
-    if (lane == 0) mbar_arrive(&v_empty[st]);
+    release(v_done, v_full, sV, &tmV, vc, st, j);
     if (++st == NS) { st = 0; ph ^= 1; }
   }
 #pragma unroll
@@ -409,6 +419,9 @@ extern "C" int udb_attention_f16(const udb_attn_t* a, void* stream) {
   static std::atomic<uint64_t> attr_mask{0};
   if (first_on_device(attr_mask)) {
     cudaError_t ea = cudaFuncSetAttribute(attn_fwd_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
+    // two CTAs per SM need the whole shared-memory carveout (2 x (112.25 + 1) KB of the SM's 228 KB)
+    if (ea == cudaSuccess)
+      ea = cudaFuncSetAttribute(attn_fwd_kernel<HD>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     if (ea != cudaSuccess) { set_error("attention: cudaFuncSetAttribute: %s", cudaGetErrorString(ea)); return 1; }
   }
   cudaError_t e = launch_ex(attn_fwd_kernel<HD>, grid, dim3(AT_THREADS), smem_bytes, reinterpret_cast<cudaStream_t>(stream), 1,
