@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libudb.so")
 SOURCES = ["common.cu", "gemm.cu", "conv_halo.cu", "attention.cu", "elementwise.cu", "camera.cu", "metrics.cu", "v1_kernels.cu", "engine.cu", "engine_v1.cu", "engine_v2old.cu", "p2p.cu"]
-HEADERS = ["common.h", "ptx.cuh", "engine_common.h", os.path.join("..", "..", "include", "udb.h")]
+HEADERS = ["common.h", "cuda_core.cuh", "ptx.cuh", "engine_common.h", os.path.join("..", "..", "include", "udb.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "-Xptxas", "-v", "--expt-relaxed-constexpr"]

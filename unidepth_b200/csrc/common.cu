@@ -63,6 +63,23 @@ int num_sms() {
   return n;
 }
 
+int check_dims(const char* fn, std::initializer_list<NamedDim> dims) {
+  for (const auto& d : dims)
+    if (d.v < 1) { set_error("%s: %s=%d must be >= 1", fn, d.name, d.v); return 1; }
+  return 0;
+}
+
+int check_ptrs(const char* fn, std::initializer_list<NamedPtr> ptrs, int align, const char* noun) {
+  for (const auto& a : ptrs) {
+    if (align > 0 && (!a.p || reinterpret_cast<uintptr_t>(a.p) % align)) {
+      set_error("%s: `%s` must be a non-null, %d-byte aligned %s", fn, a.name, align, noun);
+      return 1;
+    }
+    if (!a.p) { set_error("%s: `%s` must be non-null", fn, a.name); return 1; }
+  }
+  return 0;
+}
+
 bool pdl_enabled() {
   static const bool on = [] {
     const char* e = getenv("UDB_PDL");

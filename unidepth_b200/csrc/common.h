@@ -6,6 +6,7 @@
 #include <stdio.h>
 
 #include <atomic>
+#include <initializer_list>
 
 #include "../../include/udb.h"
 
@@ -21,6 +22,21 @@ int check_launch(const char* what);
 void note_work(double flops, double bytes);
 
 int num_sms();   // of the CURRENT device (cached per device)
+
+#define ST(s) reinterpret_cast<cudaStream_t>(s)
+
+// Blocks of 256 threads for a grid-stride loop over `total` items: at least 1, at most per_sm per SM.
+inline int grid_1d(long long total, int per_sm) {
+  const long long g = (total + 255) / 256, cap = (long long)num_sms() * per_sm;
+  return (int)(g > cap ? cap : (g < 1 ? 1 : g));
+}
+
+// Argument checks of the launchers: 0 when they hold, else 1 with the error "<fn>: <name>=<v> must be >= 1",
+// "<fn>: `<name>` must be non-null" or, with align > 0, "<fn>: `<name>` must be a non-null, <align>-byte aligned <noun>".
+struct NamedDim { int v; const char* name; };
+struct NamedPtr { const void* p; const char* name; };
+int check_dims(const char* fn, std::initializer_list<NamedDim> dims);
+int check_ptrs(const char* fn, std::initializer_list<NamedPtr> ptrs, int align = 0, const char* noun = "pointer");
 
 // Shape bounds of udb_cross_attn_small(_f32): 0, or 1 with the error set under the name `fn`.  The V1 engine checks its
 // camera head's context length with it before anything is enqueued, so that its dry run names the bound.

@@ -2,20 +2,10 @@
 // patch extraction, position-embedding resize, the fp32 camera head, ray embedding, bilinear
 // resamplers and the output assembly.  Reference call sites are cited in include/udb.h.
 #include "common.h"
+#include "cuda_core.cuh"
 #include "ptx.cuh"
 
 namespace udb {
-
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ float warp_max(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
 
 // ------------------------------------------------------------------------------------ LayerNorm
 // One warp per R rows (R = 1 by default; the R = 2 variant -- both rows' loads in flight before the first
@@ -185,17 +175,6 @@ __global__ void __launch_bounds__(256) layernorm_f16_small_kernel(const udb_laye
 }
 
 // ------------------------------------------------------------------------------------ preprocess
-__device__ __forceinline__ void bilinear_src(float scale, int dst, int in_size, int& i0, int& i1, float& l0, float& l1) {
-  // ATen area_pixel_compute_source_index (align_corners=False): fp32 index arithmetic
-  float src = scale * ((float)dst + 0.5f) - 0.5f;
-  if (src < 0.f) src = 0.f;
-  i0 = (int)src;
-  if (i0 > in_size - 1) i0 = in_size - 1;
-  i1 = i0 + ((i0 < in_size - 1) ? 1 : 0);
-  l1 = src - (float)i0;
-  l0 = 1.f - l1;
-}
-
 // One thread per 8 consecutive patch-matrix columns (one 16-byte store).  `split`: the row holds [hi | lo] halves of
 // ldp/2 columns each, lo = f16(val - f32(hi)) (split-f16 precise mode, see udb_gemm_t.a_split_k).
 __global__ void __launch_bounds__(256) preprocess_patchify_kernel(const udb_preprocess_t p, int gh, int gw, float sh, float sw) {
@@ -395,17 +374,10 @@ __global__ void camera_intrinsics_kernel(const float* x, int B, int net_h, int n
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
   const float diag = sqrtf((float)(net_h * net_h + net_w * net_w));
-  const float fx = expf(x[b * 4 + 0]) * (0.7f * diag);
-  const float fy = expf(x[b * 4 + 1]) * (0.7f * diag);
-  const float cx = (1.f / (1.f + expf(-x[b * 4 + 2]))) * (float)net_w;
-  const float cy = (1.f / (1.f + expf(-x[b * 4 + 3]))) * (float)net_h;
-  intr4[b * 4 + 0] = fx; intr4[b * 4 + 1] = fy; intr4[b * 4 + 2] = cx; intr4[b * 4 + 3] = cy;
-  float* k = k_net + b * 9;
-  k[0] = fx; k[1] = 0.f; k[2] = cx; k[3] = 0.f; k[4] = fy; k[5] = cy; k[6] = 0.f; k[7] = 0.f; k[8] = 1.f;
-  float* o = k_out + b * 9;
-  o[0] = fx / factor; o[1] = 0.f; o[2] = cx / factor - (float)pad_l;
-  o[3] = 0.f; o[4] = fy / factor; o[5] = cy / factor - (float)pad_t;
-  o[6] = 0.f; o[7] = 0.f; o[8] = 1.f;
+  const float4 k = decode_camera(x + b * 4, 0.7f * diag, net_h, net_w);
+  intr4[b * 4 + 0] = k.x; intr4[b * 4 + 1] = k.y; intr4[b * 4 + 2] = k.z; intr4[b * 4 + 3] = k.w;
+  store_k3(k_net + b * 9, k.x, k.y, k.z, k.w);
+  store_k3(k_out + b * 9, k.x / factor, k.y / factor, k.z / factor - (float)pad_l, k.w / factor - (float)pad_t);
 }
 
 // ------------------------------------------------------------------------------------ rays
@@ -415,18 +387,6 @@ __device__ __forceinline__ float3 unit_ray(const float4 k /*fx,fy,cx,cy*/, int y
   const float ry = (1.0f / k.y) * ((float)y + 0.5f) + (-k.w / k.y);
   const float n = fmaxf(sqrtf(rx * rx + ry * ry + 1.0f), 1e-5f);
   return make_float3(rx / n, ry / n, 1.0f / n);
-}
-
-// antialiased-bilinear tap range along one axis (ATen _upsample_bilinear2d_aa weights)
-__device__ __forceinline__ void aa_range(float scale, int o, int in_size, int& lo, int& cnt, float& center) {
-  const float support = (scale >= 1.f) ? scale : 1.f;
-  center = scale * ((float)o + 0.5f);
-  lo = max((int)(center - support + 0.5f), 0);
-  cnt = min((int)(center + support + 0.5f), in_size) - lo;
-}
-__device__ __forceinline__ float aa_w(float scale, int k, float center) {
-  const float inv = (scale >= 1.f) ? 1.f / scale : 1.f;
-  return fmaxf(0.f, 1.f - fabsf(((float)k - center + 0.5f) * inv));
 }
 
 // one warp per output token
@@ -439,19 +399,15 @@ __global__ void __launch_bounds__(256) ray_embed_kernel(const udb_ray_embed_t p,
   if (tok >= p.B * n) return;
   const int b = tok / n, i = (tok % n) / p.gw, j = tok % p.gw;
   const float sy = (float)p.net_h / (float)p.gh, sx = (float)p.net_w / (float)p.gw;
-  int ylo, ycnt, xlo, xcnt;
-  float yc, xc;
-  aa_range(sy, i, p.net_h, ylo, ycnt, yc);
-  aa_range(sx, j, p.net_w, xlo, xcnt, xc);
+  const AAxis wy = aa_axis(i, p.net_h, sy), wx = aa_axis(j, p.net_w, sx);
   float4 k = make_float4(1.f, 1.f, 0.f, 0.f);
   if (!p.rays_in) k = *reinterpret_cast<const float4*>(p.intr4 + b * 4);
-  float ax = 0.f, ay = 0.f, az = 0.f, wsum_y = 0.f, wsum_x = 0.f;
-  for (int a = 0; a < ycnt; ++a) wsum_y += aa_w(sy, ylo + a, yc);
-  for (int a = 0; a < xcnt; ++a) wsum_x += aa_w(sx, xlo + a, xc);
-  const int taps = ycnt * xcnt;
+  float ax = 0.f, ay = 0.f, az = 0.f;
+  const int taps = wy.xsize * wx.xsize;
   for (int t = lane; t < taps; t += 32) {
-    const int yy = ylo + t / xcnt, xx = xlo + t % xcnt;
-    const float w = (aa_w(sy, yy, yc) / wsum_y) * (aa_w(sx, xx, xc) / wsum_x);
+    const int ty = t / wx.xsize, tx = t % wx.xsize, yy = wy.xmin + ty, xx = wx.xmin + tx;
+    // raw weight / window sum, not times `norm` (1 / sum), which rounds differently
+    const float w = (wy.tri(ty, 1.f) / wy.sum) * (wx.tri(tx, 1.f) / wx.sum);
     float3 r;
     if (p.rays_in) {
       const float* rp = p.rays_in + ((long long)b * p.net_h * p.net_w + (long long)yy * p.net_w + xx) * 3;
@@ -536,8 +492,6 @@ __global__ void __launch_bounds__(256) upsample2x_kernel(const __half* __restric
   lerp8(v10, v11, lx0, lx1, acc, ly1);
   reinterpret_cast<uint4*>(out)[((size_t)(b * 2 * H + Y) * 2 * W + X) * cv + c8] = pack8(acc);
 }
-
-__device__ __forceinline__ int reflect_idx(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * (n - 1) - i : i); }
 
 __global__ void __launch_bounds__(256) resize_ac_pad_kernel(const __half* __restrict__ in, __half* __restrict__ out, int H, int W,
                                                             int C, int oh, int ow, int pad, float sh, float sw) {
@@ -818,16 +772,9 @@ __global__ void __launch_bounds__(256) quantize_rows_e4m3_kernel(const __half* _
   }
 }
 
-static inline int grid_for(long long total, int block = 256) {
-  long long g = (total + block - 1) / block;
-  const long long cap = (long long)num_sms() * 16;
-  return (int)(g < cap ? (g > 0 ? g : 1) : cap);
-}
-
 }  // namespace udb
 
 using namespace udb;
-#define ST(s) reinterpret_cast<cudaStream_t>(s)
 
 extern "C" int udb_layernorm_e4m3(const udb_layernorm_t* p, float* out_scale, void* stream) {
   if (!p || !p->in_f32 || p->out_split || (p->dim_valid && p->dim_valid != p->dim) || !out_scale || (reinterpret_cast<uintptr_t>(out_scale) & 3)) {
@@ -929,12 +876,12 @@ extern "C" int udb_preprocess_patchify(const udb_preprocess_t* p, void* stream) 
   const float sh = (float)padded_h / (float)p->net_h, sw = (float)padded_w / (float)p->net_w;
   const long long total = (long long)p->B * gh * gw * (p->ldp / 8);
   note_work(0.0, (double)p->B * 3 * p->H * p->W * (p->rgb_is_u8 ? 1 : 4) + (double)p->B * gh * gw * p->ldp * 2);
-  preprocess_patchify_kernel<<<grid_for(total), 256, 0, ST(stream)>>>(*p, gh, gw, sh, sw);
+  preprocess_patchify_kernel<<<grid_1d(total, 16), 256, 0, ST(stream)>>>(*p, gh, gw, sh, sw);
   return check_launch("preprocess_patchify_kernel");
 }
 
 extern "C" int udb_posembed_bicubic(const float* grid, int32_t m, int32_t dim, float* out, int32_t gh, int32_t gw, void* stream) {
-  posembed_bicubic_kernel<<<grid_for((long long)gh * gw * dim), 256, 0, ST(stream)>>>(grid, m, dim, out, gh, gw);
+  posembed_bicubic_kernel<<<grid_1d((long long)gh * gw * dim, 16), 256, 0, ST(stream)>>>(grid, m, dim, out, gh, gw);
   return check_launch("posembed_bicubic_kernel");
 }
 
@@ -1060,7 +1007,7 @@ extern "C" int udb_postprocess(const udb_postprocess_t* p, void* stream) {
     return 1;
   }
   note_work(0.0, 4.0 * p->B * (2.0 * p->net_h * p->net_w + 9.0 * p->H * p->W));
-  const int grid = grid_for((long long)p->B * p->H * p->W);
+  const int grid = grid_1d((long long)p->B * p->H * p->W, 16);
   if (p->mode == UDB_INTERP_BICUBIC) {
     postprocess_bicubic_kernel<<<grid, 256, 0, ST(stream)>>>(*p);
     return check_launch("postprocess_bicubic_kernel");
@@ -1070,19 +1017,16 @@ extern "C" int udb_postprocess(const udb_postprocess_t* p, void* stream) {
 }
 
 extern "C" int udb_match_gt(const udb_match_gt_t* p, void* stream) {
-  const struct { int v; const char* name; } dims[] = {{p->B, "B"}, {p->H, "H"}, {p->W, "W"}, {p->net_h, "net_h"}, {p->net_w, "net_w"}};
-  for (const auto& d : dims)
-    if (d.v < 1) { set_error("udb_match_gt: %s=%d must be >= 1", d.name, d.v); return 1; }
-  const struct { const void* q; const char* name; } ptrs[] = {
-      {p->radius, "radius"}, {p->confidence, "confidence"}, {p->pads, "pads"}, {p->intrinsics, "intrinsics"},
-      {p->out_confidence, "out_confidence"}, {p->out_depth, "out_depth"}, {p->out_points, "out_points"}, {p->out_rays, "out_rays"}};
-  for (const auto& a : ptrs)
-    if (!a.q) { set_error("udb_match_gt: `%s` must be non-null", a.name); return 1; }
+  if (check_dims("udb_match_gt", {{p->B, "B"}, {p->H, "H"}, {p->W, "W"}, {p->net_h, "net_h"}, {p->net_w, "net_w"}})) return 1;
+  if (check_ptrs("udb_match_gt", {{p->radius, "radius"}, {p->confidence, "confidence"}, {p->pads, "pads"}, {p->intrinsics, "intrinsics"},
+                                  {p->out_confidence, "out_confidence"}, {p->out_depth, "out_depth"}, {p->out_points, "out_points"},
+                                  {p->out_rays, "out_rays"}}))
+    return 1;
   if (!p->rays_in && !p->intr4) { set_error("udb_match_gt: `intr4` must be non-null when `rays_in` is null"); return 1; }
   if (!p->rays_in && (reinterpret_cast<uintptr_t>(p->intr4) & 15)) { set_error("udb_match_gt: `intr4` must be 16-byte aligned"); return 1; }
   const long long n_out = (long long)p->B * p->H * p->W, n_net = (long long)p->B * p->net_h * p->net_w;
   const long long total = n_out > n_net ? n_out : n_net;
   note_work(0.0, 4.0 * (2.0 * n_net + 5.0 * n_out + 3.0 * n_net));
-  match_gt_kernel<<<grid_for(total), 256, 0, ST(stream)>>>(*p, total);
+  match_gt_kernel<<<grid_1d(total, 16), 256, 0, ST(stream)>>>(*p, total);
   return check_launch("match_gt_kernel");
 }

@@ -8,58 +8,10 @@
 #include <math.h>
 
 #include "common.h"
+#include "cuda_core.cuh"
 #include "ptx.cuh"
 
 namespace udb {
-
-#define ST(s) reinterpret_cast<cudaStream_t>(s)
-
-static inline int grid_1d(long long total, int block = 256) {
-  long long g = (total + block - 1) / block;
-  const long long cap = (long long)num_sms() * 32;
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return (int)g;
-}
-
-__device__ __forceinline__ float wsum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ float wmax(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// Antialiased bilinear weights of ONE axis, exactly ATen's _compute_indices_min_size_weights_aa (UpSampleKernel.cpp;
-// F.interpolate(mode="bilinear", align_corners=False, antialias=True)): triangle filter of half-width
-// max(scale, 1) around scale*(i+0.5), window clipped to the input, weights renormalised.
-// Returns xmin / xsize and the inverse weight sum; weight(j) = tri((j + xmin - center + 0.5) * invscale) * norm.
-// ------------------------------------------------------------------------------------------------------------------
-struct AAxis {
-  int xmin, xsize;
-  float center, invscale, norm;
-  __device__ __forceinline__ float w(int j) const {
-    const float x = fabsf(((float)(j + xmin) - center + 0.5f) * invscale);
-    return x < 1.f ? (1.f - x) * norm : 0.f;
-  }
-};
-__device__ __forceinline__ AAxis aa_axis(int i, int in_size, float scale) {
-  AAxis a;
-  const float support = scale >= 1.f ? scale : 1.f;
-  a.center = scale * ((float)i + 0.5f);
-  a.invscale = scale >= 1.f ? 1.f / scale : 1.f;
-  a.xmin = max((int)(a.center - support + 0.5f), 0);
-  a.xsize = min((int)(a.center + support + 0.5f), in_size) - a.xmin;
-  float tot = 0.f;
-  a.norm = 1.f;
-  for (int j = 0; j < a.xsize; ++j) tot += a.w(j);
-  a.norm = tot != 0.f ? 1.f / tot : 1.f;
-  return a;
-}
 
 // ------------------------------------------------------------------------------------------------------------------
 // V1 pre-processing (unidepthv1.py:49-63,298-317): u8 / f32 NCHW -> /255 -> ImageNet normalise -> antialiased bilinear
@@ -173,12 +125,12 @@ __global__ void __launch_bounds__(256) layernorm_any_kernel(const udb_layernorm_
 #pragma unroll
   for (int r = 0; r < R; ++r) {
     const long long row = row0 + r;
-    const float mean = wsum(s[r]) / (float)p.dim;
+    const float mean = warp_sum(s[r]) / (float)p.dim;
     float v = 0.f;
 #pragma unroll
     for (int i = 0; i < NV; ++i)
       if (i < nv) v += (x[r][i].x - mean) * (x[r][i].x - mean) + (x[r][i].y - mean) * (x[r][i].y - mean);
-    const float rstd = rsqrtf(wsum(v) / (float)p.dim + p.eps);
+    const float rstd = rsqrtf(warp_sum(v) / (float)p.dim + p.eps);
     if (row >= p.rows) continue;
     long long obase = row * p.ld_out;
     if (p.s2d_w > 0) {
@@ -459,7 +411,7 @@ __global__ void __launch_bounds__(256) dwconv7_ln_e4m3_kernel(const __half* __re
     float s = 0.f;
 #pragma unroll
     for (int k = 0; k < 8; ++k) s += f[k];
-    s = wsum(mine ? s : 0.f);
+    s = warp_sum(mine ? s : 0.f);
     if (lane == 0) part[0][p] = s;
   }
   cluster.sync();
@@ -473,7 +425,7 @@ __global__ void __launch_bounds__(256) dwconv7_ln_e4m3_kernel(const __half* __re
     float q = 0.f;
 #pragma unroll
     for (int k = 0; k < 8; ++k) q += (f[k] - mean[i]) * (f[k] - mean[i]);
-    q = wsum(mine ? q : 0.f);
+    q = warp_sum(mine ? q : 0.f);
     if (lane == 0) part[1][p] = q;
   }
   cluster.sync();
@@ -496,7 +448,7 @@ __global__ void __launch_bounds__(256) dwconv7_ln_e4m3_kernel(const __half* __re
 #pragma unroll
       for (int k = 0; k < 8; ++k) am = fmaxf(am, fabsf((f[k] - mean[i]) * rstd[i] * wk[k] + bk[k]));
     }
-    am = wmax(am);
+    am = warp_max(am);
     if (lane == 0) part[2][p] = am;
   }
   cluster.sync();
@@ -697,7 +649,7 @@ __global__ void __launch_bounds__(256) rays_sh81_kernel(const udb_v1_rays_t p) {
     ry += wgt * dy * inv;
     rz += wgt * inv;
   }
-  rx = wsum(rx); ry = wsum(ry); rz = wsum(rz);
+  rx = warp_sum(rx); ry = warp_sum(ry); rz = warp_sum(rz);
   {
     const float inv = 1.0f / fmaxf(sqrtf(rx * rx + ry * ry + rz * rz), 1e-12f);
     rx *= inv; ry *= inv; rz *= inv;
@@ -740,7 +692,7 @@ __global__ void __launch_bounds__(256) rays_sh81_kernel(const udb_v1_rays_t p) {
     if (id < 81) v += (mine[j] - mean) * (mine[j] - mean);
   }
   (void)sq;
-  const float rstd = rsqrtf(wsum(v) / 81.f + 1e-5f);
+  const float rstd = rsqrtf(warp_sum(v) / 81.f + 1e-5f);
   __half* o = reinterpret_cast<__half*>(p.out) + tok * 128;
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
@@ -760,11 +712,8 @@ __global__ void v1_camera_intrinsics_kernel(const float* x4, const float* gt_k, 
   if (b >= B) return;
   float fx = 0.f, fy = 0.f, cx = 0.f, cy = 0.f;
   if (x4) {
-    const float half_max = (float)max(net_h, net_w) / 2.0f;
-    fx = half_max * expf(x4[b * 4]);
-    fy = half_max * expf(x4[b * 4 + 1]);
-    cx = (1.0f / (1.0f + expf(-x4[b * 4 + 2]))) * (float)net_w;
-    cy = (1.0f / (1.0f + expf(-x4[b * 4 + 3]))) * (float)net_h;
+    const float4 k = decode_camera(x4 + b * 4, (float)max(net_h, net_w) / 2.0f, net_h, net_w);
+    fx = k.x; fy = k.y; cx = k.z; cy = k.w;
   }
   float rfx = fx, rfy = fy, rcx = cx, rcy = cy;     // K the rays are generated from
   if (gt_k) {
@@ -776,9 +725,7 @@ __global__ void v1_camera_intrinsics_kernel(const float* x4, const float* gt_k, 
   }
   intr4_rays[b * 4] = rfx; intr4_rays[b * 4 + 1] = rfy; intr4_rays[b * 4 + 2] = rcx; intr4_rays[b * 4 + 3] = rcy;
   float* k = k_out + b * 9;
-  k[0] = fx / ratio; k[1] = 0.f; k[2] = (cx - (float)pad_l) / ratio;
-  k[3] = 0.f; k[4] = fy / ratio; k[5] = (cy - (float)pad_t) / ratio;
-  k[6] = 0.f; k[7] = 0.f; k[8] = 1.f;
+  store_k3(k, fx / ratio, fy / ratio, (cx - (float)pad_l) / ratio, (cy - (float)pad_t) / ratio);
   // K the final back-projection uses on the ORIGINAL pixel grid (unidepthv1.py:354-356): the pre-processed GT K when one
   // was given (the reference does not undo its resize there), else the returned prediction
   float* kp = k4_points + b * 4;
@@ -837,7 +784,7 @@ __global__ void __launch_bounds__(256) cross_attn_partial_kernel(const float* __
 #pragma unroll
     for (int qi = 0; qi < CA_MAXQ; ++qi)
       if (qi < nq) {
-        const float v = wsum(a[qi]);
+        const float v = warp_sum(a[qi]);
         if (lane == 0) sc[qi * chunk + j] = v;
       }
   }
@@ -846,14 +793,14 @@ __global__ void __launch_bounds__(256) cross_attn_partial_kernel(const float* __
   if (warp < nq) {
     float m = -INFINITY;
     for (int j = lane; j < n; j += 32) m = fmaxf(m, sc[warp * chunk + j]);
-    m = wmax(m);
+    m = warp_max(m);
     float l = 0.f;
     for (int j = lane; j < n; j += 32) {
       const float e = expf(sc[warp * chunk + j] - m);
       sc[warp * chunk + j] = e;
       l += e;
     }
-    l = wsum(l);
+    l = warp_sum(l);
     if (lane == 0) { red[warp * 2] = m; red[warp * 2 + 1] = l; }
   }
   __syncthreads();
@@ -911,10 +858,10 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restri
   const float* sr = s + row * ld_in;
   float m = -INFINITY;
   for (int j = lane; j < n_valid; j += 32) m = fmaxf(m, sr[j]);
-  m = wmax(m);
+  m = warp_max(m);
   float tot = 0.f;
   for (int j = lane; j < n_valid; j += 32) tot += expf((sr[j] - m) * scale);
-  tot = wsum(tot);
+  tot = warp_sum(tot);
   const float inv = 1.0f / tot;
   __half* pr = p + row * ld_out;
   for (int j = lane; j < ld_out; j += 32) pr[j] = __float2half_rn(j < n_valid ? expf((sr[j] - m) * scale) * inv : 0.f);
@@ -1019,10 +966,10 @@ __global__ void __launch_bounds__(128) nystrom_k2_kernel(const __half* __restric
     s[j] = a * 0.125f;
     mx = fmaxf(mx, s[j]);
   }
-  mx = wmax(mx);
+  mx = warp_max(mx);
   float tot = 0.f;
   for (int j = 0; j < 4; ++j) { s[j] = expf(s[j] - mx); tot += s[j]; }
-  tot = wsum(tot);
+  tot = warp_sum(tot);
   for (int j = 0; j < 4; ++j) k2[((long long)bh * m + row) * m + lane + 32 * j] = s[j] / tot;
 }
 
@@ -1034,7 +981,7 @@ __global__ void __launch_bounds__(128) nystrom_pinv_init_kernel(const float* __r
   const int j = threadIdx.x;      // m == 128 threads: column sums
   float cs = 0.f;
   for (int i = 0; i < m; ++i) cs += K[i * m + j];
-  float mx = wmax(cs);
+  float mx = warp_max(cs);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
   __syncthreads();
   mx = fmaxf(fmaxf(red[0], red[1]), fmaxf(red[2], red[3]));
@@ -1131,14 +1078,7 @@ __global__ void __launch_bounds__(256) v1_mean_maps_kernel(const float* __restri
     for (int lvl = 0; lvl < 3; ++lvl) {
       const int h = gh << (lvl + 1), w = gw << (lvl + 1);
       const float* src = (lvl == 0 ? o8 : (lvl == 1 ? o4 : o2)) + (long long)b * h * w;
-      const AAxis ay = aa_axis(Y, h, (float)h / (float)net_h), ax = aa_axis(X, w, (float)w / (float)net_w);
-      float acc = 0.f;
-      for (int jy = 0; jy < ay.xsize; ++jy) {
-        float r = 0.f;
-        for (int jx = 0; jx < ax.xsize; ++jx) r += ax.w(jx) * src[(long long)(ay.xmin + jy) * w + ax.xmin + jx];
-        acc += ay.w(jy) * r;
-      }
-      tot += acc;
+      tot += aa_sample(src, aa_axis(Y, h, (float)h / (float)net_h), aa_axis(X, w, (float)w / (float)net_w), w);
     }
     mean[idx] = tot / 3.0f;
   }
@@ -1150,25 +1090,29 @@ __global__ void __launch_bounds__(256) v1_postprocess_kernel(const udb_v1_postpr
   const float sh = (float)ch / (float)p.H, sw = (float)cw / (float)p.W;
   for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
     const int X = (int)(idx % p.W), Y = (int)((idx / p.W) % p.H), b = (int)(idx / ((long long)p.W * p.H));
-    const AAxis ay = aa_axis(Y, ch, sh), ax = aa_axis(X, cw, sw);
-    const float* src = p.mean + (long long)b * p.net_h * p.net_w;
-    float z = 0.f;
-    for (int jy = 0; jy < ay.xsize; ++jy) {
-      float r = 0.f;
-      for (int jx = 0; jx < ax.xsize; ++jx) r += ax.w(jx) * src[(long long)(p.pad_t + ay.xmin + jy) * p.net_w + p.pad_l + ax.xmin + jx];
-      z += ay.w(jy) * r;
-    }
-    const float* k = p.k4 + b * 4;       // fx, fy, cx, cy of the K the points are generated with
-    const float dx = ((float)X + 0.5f - k[2]) / k[0], dy = ((float)Y + 0.5f - k[3]) / k[1];
-    const float inv = 1.0f / fmaxf(sqrtf(dx * dx + dy * dy + 1.0f), 1e-12f);
-    const float rx = dx * inv, ry = dy * inv, rz = inv;
-    const float theta = atan2f(rx, rz), phi = acosf(ry);
+    const float* src = p.mean + (long long)b * p.net_h * p.net_w + (long long)p.pad_t * p.net_w + p.pad_l;   // the crop
+    const float z = aa_sample(src, aa_axis(Y, ch, sh), aa_axis(X, cw, sw), p.net_w);
     const long long hw = (long long)p.H * p.W, pix = (long long)Y * p.W + X;
     p.out_depth[b * hw + pix] = z;
-    p.out_points[(b * 3 + 0) * hw + pix] = z * tanf(theta);
-    p.out_points[(b * 3 + 1) * hw + pix] = z / tanf(phi) / cosf(theta);
-    p.out_points[(b * 3 + 2) * hw + pix] = z;
+    backproject(p.k4 + b * 4, X, Y, z, p.out_points + b * 3 * hw + pix, hw);   // k4: the K the points are generated with
   }
+}
+
+// udb_v1_preprocess (f16 patch rows) and udb_v1_preprocess_split ([hi | lo] rows), errors under the name `fn`
+template <bool SPLIT>
+static int v1_preprocess(const char* fn, const udb_v1_preprocess_t* p, void* stream) {
+  const float sh = (float)p->H / (float)p->rh, sw = (float)p->W / (float)p->rw;
+  if (p->patch == 14) {
+    if (p->net_h % 14 || p->net_w % 14) { set_error("%s: network shape %dx%d is not a multiple of 14", fn, p->net_h, p->net_w); return 1; }
+    const int gh = p->net_h / 14, gw = p->net_w / 14;
+    v1_preprocess_kernel<14, SPLIT><<<grid_1d((long long)p->B * gh * gw * 80, 32), 256, 0, ST(stream)>>>(*p, gh, gw, sh, sw);
+    return check_launch(SPLIT ? "v1_preprocess_split_kernel<14>" : "v1_preprocess_kernel<14>");
+  }
+  if (p->patch != 0 && p->patch != 4) { set_error("%s: patch %d unsupported (0 / 4 or 14)", fn, p->patch); return 1; }
+  if (p->net_h < 4 || p->net_w < 4) { set_error("%s: bad network shape", fn); return 1; }
+  const int gh = (p->net_h - 4) / 4 + 1, gw = (p->net_w - 4) / 4 + 1;
+  v1_preprocess_kernel<4, SPLIT><<<grid_1d((long long)p->B * gh * gw * 8, 32), 256, 0, ST(stream)>>>(*p, gh, gw, sh, sw);
+  return check_launch(SPLIT ? "v1_preprocess_split_kernel" : "v1_preprocess_kernel");
 }
 
 }  // namespace udb
@@ -1177,34 +1121,10 @@ using namespace udb;
 
 extern "C" {
 
-int udb_v1_preprocess(const udb_v1_preprocess_t* p, void* stream) {
-  const float sh = (float)p->H / (float)p->rh, sw = (float)p->W / (float)p->rw;
-  if (p->patch == 14) {
-    if (p->net_h % 14 || p->net_w % 14) { set_error("udb_v1_preprocess: network shape %dx%d is not a multiple of 14", p->net_h, p->net_w); return 1; }
-    const int gh = p->net_h / 14, gw = p->net_w / 14;
-    v1_preprocess_kernel<14, false><<<grid_1d((long long)p->B * gh * gw * 80), 256, 0, ST(stream)>>>(*p, gh, gw, sh, sw);
-    return check_launch("v1_preprocess_kernel<14>");
-  }
-  if (p->patch != 0 && p->patch != 4) { set_error("udb_v1_preprocess: patch %d unsupported (0 / 4 or 14)", p->patch); return 1; }
-  if (p->net_h < 4 || p->net_w < 4) { set_error("udb_v1_preprocess: bad network shape"); return 1; }
-  const int gh = (p->net_h - 4) / 4 + 1, gw = (p->net_w - 4) / 4 + 1;
-  v1_preprocess_kernel<4, false><<<grid_1d((long long)p->B * gh * gw * 8), 256, 0, ST(stream)>>>(*p, gh, gw, sh, sw);
-  return check_launch("v1_preprocess_kernel");
-}
+int udb_v1_preprocess(const udb_v1_preprocess_t* p, void* stream) { return v1_preprocess<false>("udb_v1_preprocess", p, stream); }
 
 int udb_v1_preprocess_split(const udb_v1_preprocess_t* p, void* stream) {
-  const float sh = (float)p->H / (float)p->rh, sw = (float)p->W / (float)p->rw;
-  if (p->patch == 14) {
-    if (p->net_h % 14 || p->net_w % 14) { set_error("udb_v1_preprocess_split: network shape %dx%d is not a multiple of 14", p->net_h, p->net_w); return 1; }
-    const int gh = p->net_h / 14, gw = p->net_w / 14;
-    v1_preprocess_kernel<14, true><<<grid_1d((long long)p->B * gh * gw * 80), 256, 0, ST(stream)>>>(*p, gh, gw, sh, sw);
-    return check_launch("v1_preprocess_split_kernel<14>");
-  }
-  if (p->patch != 0 && p->patch != 4) { set_error("udb_v1_preprocess_split: patch %d unsupported (0 / 4 or 14)", p->patch); return 1; }
-  if (p->net_h < 4 || p->net_w < 4) { set_error("udb_v1_preprocess_split: bad network shape"); return 1; }
-  const int gh = (p->net_h - 4) / 4 + 1, gw = (p->net_w - 4) / 4 + 1;
-  v1_preprocess_kernel<4, true><<<grid_1d((long long)p->B * gh * gw * 8), 256, 0, ST(stream)>>>(*p, gh, gw, sh, sw);
-  return check_launch("v1_preprocess_split_kernel");
+  return v1_preprocess<true>("udb_v1_preprocess_split", p, stream);
 }
 
 int udb_layernorm_any(const udb_layernorm_any_t* p, void* stream) {
@@ -1255,16 +1175,10 @@ int udb_dwconv7_nhwc_f16(const void* x, const float* w, const float* bias, void*
 int udb_dwconv7_ln_e4m3(const void* x, const float* w, const float* bias, const float* ln_w, const float* ln_b, void* out,
                         float* out_scale, int32_t B, int32_t H, int32_t W, int32_t C, void* stream) {
   if (C <= 0 || C % DW_CB || C > DWL_MAXC) { set_error("udb_dwconv7_ln_e4m3: C=%d must be a multiple of 64 up to 1536", C); return 1; }
-  const struct { int v; const char* name; } dims[] = {{B, "B"}, {H, "H"}, {W, "W"}};
-  for (const auto& d : dims)
-    if (d.v < 1) { set_error("udb_dwconv7_ln_e4m3: %s=%d must be >= 1", d.name, d.v); return 1; }
-  const struct { const void* p; const char* name; } ptrs[] = {{x, "x"}, {w, "w"}, {bias, "bias"}, {ln_w, "ln_w"}, {ln_b, "ln_b"},
-                                                              {out, "out"}, {out_scale, "out_scale"}};
-  for (const auto& a : ptrs)
-    if (!a.p || (reinterpret_cast<uintptr_t>(a.p) & 15)) {
-      set_error("udb_dwconv7_ln_e4m3: `%s` must be a non-null, 16-byte aligned device pointer", a.name);
-      return 1;
-    }
+  if (check_dims("udb_dwconv7_ln_e4m3", {{B, "B"}, {H, "H"}, {W, "W"}})) return 1;
+  if (check_ptrs("udb_dwconv7_ln_e4m3", {{x, "x"}, {w, "w"}, {bias, "bias"}, {ln_w, "ln_w"}, {ln_b, "ln_b"}, {out, "out"}, {out_scale, "out_scale"}},
+                 16, "device pointer"))
+    return 1;
   const int chunks = C / DW_CB, K = (chunks + DWL_CPB - 1) / DWL_CPB;     // cluster size: 1..8
   static std::atomic<uint64_t> attr_mask{0};
   if (first_on_device(attr_mask)) {
@@ -1299,14 +1213,14 @@ int udb_dwconv7_nhwc_f32(const float* x, const float* w, const float* bias, floa
 int udb_max_accum_f32(const float* src, float* dst, int64_t n, int32_t first, void* stream) {
   if (n % 4) { set_error("udb_max_accum_f32: n must be a multiple of 4"); return 1; }
   note_work(0.0, (first ? 8.0 : 12.0) * n);
-  max_accum_f32_kernel<<<grid_1d(n / 4), 256, 0, ST(stream)>>>(reinterpret_cast<const float4*>(src), reinterpret_cast<float4*>(dst), n / 4, first);
+  max_accum_f32_kernel<<<grid_1d(n / 4, 32), 256, 0, ST(stream)>>>(reinterpret_cast<const float4*>(src), reinterpret_cast<float4*>(dst), n / 4, first);
   return check_launch("max_accum_f32_kernel");
 }
 
 int udb_max_accum_f16(const void* src, void* dst, int64_t n, int32_t first, void* stream) {
   if (n % 8) { set_error("udb_max_accum_f16: n must be a multiple of 8"); return 1; }
   note_work(0.0, (first ? 4.0 : 6.0) * n);
-  max_accum_kernel<<<grid_1d(n / 8), 256, 0, ST(stream)>>>(reinterpret_cast<const uint4*>(src), reinterpret_cast<uint4*>(dst), n / 8, first);
+  max_accum_kernel<<<grid_1d(n / 8, 32), 256, 0, ST(stream)>>>(reinterpret_cast<const uint4*>(src), reinterpret_cast<uint4*>(dst), n / 8, first);
   return check_launch("max_accum_kernel");
 }
 
@@ -1314,7 +1228,7 @@ int udb_vit_tap(const float* x, void* acc, float* cls_out, int32_t B, int32_t N,
   if (D % 8 || D <= 0 || N <= 0 || B <= 0) { set_error("udb_vit_tap: bad shape B=%d N=%d D=%d (D %% 8 == 0)", B, N, D); return 1; }
   const long long items = (long long)B * N * (D / 8) + (cls_out ? (long long)B * (D / 8) : 0);
   note_work((double)B * N * D, (double)B * N * D * (4.0 + (first ? 2.0 : 4.0)) + (cls_out ? 8.0 * B * D : 0.0));
-  vit_tap_kernel<false><<<grid_1d(items), 256, 0, ST(stream)>>>(x, reinterpret_cast<uint4*>(acc), cls_out, B, N, D, first);
+  vit_tap_kernel<false><<<grid_1d(items, 32), 256, 0, ST(stream)>>>(x, reinterpret_cast<uint4*>(acc), cls_out, B, N, D, first);
   return check_launch("vit_tap_kernel");
 }
 
@@ -1322,7 +1236,7 @@ int udb_vit_tap_f32(const float* x, float* acc, float* cls_out, int32_t B, int32
   if (D % 8 || D <= 0 || N <= 0 || B <= 0) { set_error("udb_vit_tap_f32: bad shape B=%d N=%d D=%d (D %% 8 == 0)", B, N, D); return 1; }
   const long long items = (long long)B * N * (D / 8) + (cls_out ? (long long)B * (D / 8) : 0);
   note_work((double)B * N * D, (double)B * N * D * (4.0 + (first ? 4.0 : 8.0)) + (cls_out ? 8.0 * B * D : 0.0));
-  vit_tap_kernel<true><<<grid_1d(items), 256, 0, ST(stream)>>>(x, reinterpret_cast<uint4*>(acc), cls_out, B, N, D, first);
+  vit_tap_kernel<true><<<grid_1d(items, 32), 256, 0, ST(stream)>>>(x, reinterpret_cast<uint4*>(acc), cls_out, B, N, D, first);
   return check_launch("vit_tap_f32_kernel");
 }
 
@@ -1336,7 +1250,7 @@ int udb_spatial_mean_f32(const float* x, float* out, int32_t B, int32_t HW, int3
 int udb_aa_resize_nhwc_f16(const void* in, void* out, int32_t B, int32_t H, int32_t W, int32_t C, int32_t oh, int32_t ow, void* stream) {
   if (C % 8) { set_error("udb_aa_resize_nhwc_f16: C must be a multiple of 8"); return 1; }
   note_work(0.0, 2.0 * B * C * ((double)H * W + (double)oh * ow));
-  aa_resize_nhwc_kernel<__half><<<grid_1d((long long)B * oh * ow * (C / 8)), 256, 0, ST(stream)>>>(
+  aa_resize_nhwc_kernel<__half><<<grid_1d((long long)B * oh * ow * (C / 8), 32), 256, 0, ST(stream)>>>(
       reinterpret_cast<const __half*>(in), reinterpret_cast<__half*>(out), B, H, W, C, oh, ow, (float)H / (float)oh, (float)W / (float)ow);
   return check_launch("aa_resize_nhwc_kernel");
 }
@@ -1344,7 +1258,7 @@ int udb_aa_resize_nhwc_f16(const void* in, void* out, int32_t B, int32_t H, int3
 int udb_aa_resize_nhwc_f32(const float* in, float* out, int32_t B, int32_t H, int32_t W, int32_t C, int32_t oh, int32_t ow, void* stream) {
   if (C % 8) { set_error("udb_aa_resize_nhwc_f32: C must be a multiple of 8"); return 1; }
   note_work(0.0, 4.0 * B * C * ((double)H * W + (double)oh * ow));
-  aa_resize_nhwc_kernel<float><<<grid_1d((long long)B * oh * ow * (C / 8)), 256, 0, ST(stream)>>>(
+  aa_resize_nhwc_kernel<float><<<grid_1d((long long)B * oh * ow * (C / 8), 32), 256, 0, ST(stream)>>>(
       in, out, B, H, W, C, oh, ow, (float)H / (float)oh, (float)W / (float)ow);
   return check_launch("aa_resize_nhwc_f32_kernel");
 }
@@ -1424,7 +1338,7 @@ int udb_softmax_rows(const float* s, void* p, int64_t rows, int32_t n_valid, int
 int udb_add_f32(const float* a, const float* b, float* out, void* out_f16, int64_t n, void* stream) {
   if (n % 4) { set_error("udb_add_f32: n must be a multiple of 4"); return 1; }
   note_work(0.0, (8.0 + (out ? 4.0 : 0.0) + (out_f16 ? 2.0 : 0.0)) * n);
-  add_f32_kernel<<<grid_1d(n / 4), 256, 0, ST(stream)>>>(reinterpret_cast<const float4*>(a), reinterpret_cast<const float4*>(b),
+  add_f32_kernel<<<grid_1d(n / 4, 32), 256, 0, ST(stream)>>>(reinterpret_cast<const float4*>(a), reinterpret_cast<const float4*>(b),
                                                          reinterpret_cast<float4*>(out), reinterpret_cast<uint2*>(out_f16), n / 4);
   return check_launch("add_f32_kernel");
 }
@@ -1435,7 +1349,7 @@ int udb_copy_rows_f32_to_f16(const float* src, void* dst, int32_t groups, int32_
     set_error("udb_copy_rows_f32_to_f16: groups=%d rows_per_group=%d D=%d must all be >= 1", groups, rows_per_group, D);
     return 1;
   }
-  copy_rows_f16_kernel<<<grid_1d((long long)groups * rows_per_group * D), 256, 0, ST(stream)>>>(src, reinterpret_cast<__half*>(dst), groups,
+  copy_rows_f16_kernel<<<grid_1d((long long)groups * rows_per_group * D, 32), 256, 0, ST(stream)>>>(src, reinterpret_cast<__half*>(dst), groups,
                                                                                                 rows_per_group, D, dst_group_stride, dst_row0);
   return check_launch("copy_rows_f16_kernel");
 }
@@ -1486,7 +1400,7 @@ int udb_nystrom_k2_pinv(const void* landmarks, float* k2, float* z, float* tmp, 
   for (int it = 0; it < iters; ++it) {
     float* T2 = spare;
     if (mmul(k2, Z, KV, 1.f, 0.f)) return 1;                       // KV = K Z
-    eye_minus_kernel<<<grid_1d(nb * mm), 256, 0, ST(stream)>>>(KV, Ta, 7.f, m, nb * mm);     // T1 = 7I - KV
+    eye_minus_kernel<<<grid_1d(nb * mm, 32), 256, 0, ST(stream)>>>(KV, Ta, 7.f, m, nb * mm);     // T1 = 7I - KV
     if (check_launch("eye_minus_kernel")) return 1;
     if (mmul(KV, Ta, T2, -1.f, 15.f)) return 1;                    // T2 = 15I - KV T1
     if (mmul(KV, T2, Ta, -1.f, 13.f)) return 1;                    // T3 = 13I - KV T2   (over T1)
@@ -1515,23 +1429,19 @@ int udb_nystrom_zk3(const float* z, const void* k3, int32_t ldk3, void* out, int
 
 int udb_v1_mean_maps(const float* o8, const float* o4, const float* o2, float* mean, int32_t B, int32_t gh, int32_t gw, int32_t net_h,
                      int32_t net_w, void* stream) {
-  const struct { int v; const char* name; } dims[] = {{B, "B"}, {gh, "gh"}, {gw, "gw"}, {net_h, "net_h"}, {net_w, "net_w"}};
-  for (const auto& d : dims)
-    if (d.v < 1) { set_error("udb_v1_mean_maps: %s=%d must be >= 1", d.name, d.v); return 1; }
-  v1_mean_maps_kernel<<<grid_1d((long long)B * net_h * net_w), 256, 0, ST(stream)>>>(o8, o4, o2, mean, B, gh, gw, net_h, net_w);
+  if (check_dims("udb_v1_mean_maps", {{B, "B"}, {gh, "gh"}, {gw, "gw"}, {net_h, "net_h"}, {net_w, "net_w"}})) return 1;
+  v1_mean_maps_kernel<<<grid_1d((long long)B * net_h * net_w, 32), 256, 0, ST(stream)>>>(o8, o4, o2, mean, B, gh, gw, net_h, net_w);
   return check_launch("v1_mean_maps_kernel");
 }
 
 int udb_v1_postprocess(const udb_v1_postprocess_t* p, void* stream) {
-  const struct { int v; const char* name; } dims[] = {{p->B, "B"}, {p->H, "H"}, {p->W, "W"},
-                                                       {p->net_h - p->pad_t - p->pad_b, "net_h - pad_t - pad_b"},
-                                                       {p->net_w - p->pad_l - p->pad_r, "net_w - pad_l - pad_r"}};
-  for (const auto& d : dims)
-    if (d.v < 1) { set_error("udb_v1_postprocess: %s=%d must be >= 1", d.name, d.v); return 1; }
+  if (check_dims("udb_v1_postprocess", {{p->B, "B"}, {p->H, "H"}, {p->W, "W"}, {p->net_h - p->pad_t - p->pad_b, "net_h - pad_t - pad_b"},
+                                        {p->net_w - p->pad_l - p->pad_r, "net_w - pad_l - pad_r"}}))
+    return 1;
   const int pads[] = {p->pad_l, p->pad_r, p->pad_t, p->pad_b};
   for (int i = 0; i < 4; ++i)
     if (pads[i] < 0) { set_error("udb_v1_postprocess: paddings (pad_l, pad_r, pad_t, pad_b) must be >= 0"); return 1; }
-  v1_postprocess_kernel<<<grid_1d((long long)p->B * p->H * p->W), 256, 0, ST(stream)>>>(*p);
+  v1_postprocess_kernel<<<grid_1d((long long)p->B * p->H * p->W, 32), 256, 0, ST(stream)>>>(*p);
   return check_launch("v1_postprocess_kernel");
 }
 
@@ -1539,7 +1449,7 @@ int udb_v1_postprocess(const udb_v1_postprocess_t* p, void* stream) {
 
 // ------------------------------------------------------------------------------------------------------------------
 // UniDepthV2old (unidepthv2/decoder_old.py, unidepthv2_old.py).  CUDA-core kernels for the four steps no existing kernel
-// computes; they sit here to share the antialiased weights above (aa_axis) with V1's post-processing.
+// computes.
 // ------------------------------------------------------------------------------------------------------------------
 namespace udb {
 
@@ -1581,7 +1491,6 @@ __global__ void __launch_bounds__(256) pshuffle_dw7_relu_kernel(const __half* __
 // conv maps the 48 channels to one.  The resized maps are never stored: each of the 49 taps samples the levels where it
 // lands.  Writes the log-depth and the sigmoid of the confidence logit.  One thread per network pixel; weights in shared
 // memory ([2][48][49]: depth then confidence).
-__device__ __forceinline__ int reflect_idx(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i); }
 
 __global__ void __launch_bounds__(256) v2old_heads_kernel(const udb_v2old_heads_t p) {
   __shared__ float ws[2 * 48 * 49];
@@ -1599,19 +1508,19 @@ __global__ void __launch_bounds__(256) v2old_heads_kernel(const udb_v2old_heads_
       const float* wc = ws + 48 * 49 + (2 - lvl) * 16 * 49;
       for (int dy = 0; dy < 7; ++dy) {
         const int yy = reflect_idx(Y + dy - 3, p.net_h);
-        const float fy = fmaxf(sy * ((float)yy + 0.5f) - 0.5f, 0.f);
-        const int y0 = (int)fy, y1 = y0 + (y0 < lh - 1 ? 1 : 0);
-        const float ly = fy - (float)y0;
+        int y0, y1;
+        float ly0, ly;
+        bilinear_taps(fmaxf(sy * ((float)yy + 0.5f) - 0.5f, 0.f), lh, y0, y1, ly0, ly);
         for (int dx = 0; dx < 7; ++dx) {
           const int xx = reflect_idx(X + dx - 3, p.net_w);
-          const float fx = fmaxf(sx * ((float)xx + 0.5f) - 0.5f, 0.f);
-          const int x0 = (int)fx, x1 = x0 + (x0 < lw - 1 ? 1 : 0);
-          const float lx = fx - (float)x0;
+          int x0, x1;
+          float lx0, lx;
+          bilinear_taps(fmaxf(sx * ((float)xx + 0.5f) - 0.5f, 0.f), lw, x0, x1, lx0, lx);
           const float4* r00 = reinterpret_cast<const float4*>(src + ((long long)y0 * lw + x0) * 32);
           const float4* r01 = reinterpret_cast<const float4*>(src + ((long long)y0 * lw + x1) * 32);
           const float4* r10 = reinterpret_cast<const float4*>(src + ((long long)y1 * lw + x0) * 32);
           const float4* r11 = reinterpret_cast<const float4*>(src + ((long long)y1 * lw + x1) * 32);
-          const float w00 = (1.f - ly) * (1.f - lx), w01 = (1.f - ly) * lx, w10 = ly * (1.f - lx), w11 = ly * lx;
+          const float w00 = ly0 * lx0, w01 = ly0 * lx, w10 = ly * lx0, w11 = ly * lx;
           const int tap = dy * 7 + dx;
 #pragma unroll
           for (int q = 0; q < 8; ++q) {
@@ -1668,18 +1577,6 @@ __global__ void __launch_bounds__(1024) v2old_depth_tail_kernel(float* __restric
   }
 }
 
-// One output pixel of an antialiased bilinear resize of the row-major map m (row length ld) from the axes' weights.  The
-// confidence in v2old_postprocess_kernel keeps its own copy of this loop, so that `infer`'s code is unchanged.
-__device__ __forceinline__ float aa_sample(const float* __restrict__ m, const AAxis& ay, const AAxis& ax, int ld) {
-  float v = 0.f;
-  for (int jy = 0; jy < ay.xsize; ++jy) {
-    float r = 0.f;
-    for (int jx = 0; jx < ax.xsize; ++jx) r += ax.w(jx) * m[(long long)(ay.xmin + jy) * ld + ax.xmin + jx];
-    v += ay.w(jy) * r;
-  }
-  return v;
-}
-
 // Output assembly at the input size (unidepthv2_old.py:107-116,267-274): depth resized from the network shape with
 // bilinear (align_corners=False, no antialias) or nearest-exact, confidence with antialiased bilinear (aa_axis), and the
 // points z * (tan(theta), 1 / tan(phi) / cos(theta), 1) of the unit ray of each input pixel through k4 (fx, fy, cx, cy).
@@ -1703,32 +1600,18 @@ __global__ void __launch_bounds__(256) v2old_postprocess_kernel(const udb_v2old_
       const int yi = min((int)floorf(((float)Y + 0.5f) * sh), p.net_h - 1), xi = min((int)floorf(((float)X + 0.5f) * sw), p.net_w - 1);
       z = dm[(long long)yi * p.net_w + xi];
     } else {
-      const float fy = fmaxf(sh * ((float)Y + 0.5f) - 0.5f, 0.f), fx = fmaxf(sw * ((float)X + 0.5f) - 0.5f, 0.f);
-      const int y0 = (int)fy, x0 = (int)fx;
-      const int y1 = y0 + (y0 < p.net_h - 1 ? 1 : 0), x1 = x0 + (x0 < p.net_w - 1 ? 1 : 0);
-      const float ly = fy - (float)y0, lx = fx - (float)x0;
-      z = (1.f - ly) * ((1.f - lx) * dm[(long long)y0 * p.net_w + x0] + lx * dm[(long long)y0 * p.net_w + x1]) +
-          ly * ((1.f - lx) * dm[(long long)y1 * p.net_w + x0] + lx * dm[(long long)y1 * p.net_w + x1]);
+      int y0, y1, x0, x1;
+      float ly0, ly1, lx0, lx1;
+      bilinear_taps(fmaxf(sh * ((float)Y + 0.5f) - 0.5f, 0.f), p.net_h, y0, y1, ly0, ly1);
+      bilinear_taps(fmaxf(sw * ((float)X + 0.5f) - 0.5f, 0.f), p.net_w, x0, x1, lx0, lx1);
+      z = ly0 * (lx0 * dm[(long long)y0 * p.net_w + x0] + lx1 * dm[(long long)y0 * p.net_w + x1]) +
+          ly1 * (lx0 * dm[(long long)y1 * p.net_w + x0] + lx1 * dm[(long long)y1 * p.net_w + x1]);
     }
-    const AAxis ay = aa_axis(Y, p.net_h, sh), ax = aa_axis(X, p.net_w, sw);
-    const float* cm = p.confidence + b * nhw;
-    float conf = 0.f;
-    for (int jy = 0; jy < ay.xsize; ++jy) {
-      float r = 0.f;
-      for (int jx = 0; jx < ax.xsize; ++jx) r += ax.w(jx) * cm[(long long)(ay.xmin + jy) * p.net_w + ax.xmin + jx];
-      conf += ay.w(jy) * r;
-    }
-    const float* k = p.k4 + b * 4;
-    const float dx = ((float)X + 0.5f - k[2]) / k[0], dy = ((float)Y + 0.5f - k[3]) / k[1];
-    const float inv = 1.0f / fmaxf(sqrtf(dx * dx + dy * dy + 1.0f), 1e-12f);
-    const float rx = dx * inv, ry = dy * inv, rz = inv;
-    const float theta = atan2f(rx, rz), phi = acosf(ry);
+    const float conf = aa_sample(p.confidence + b * nhw, aa_axis(Y, p.net_h, sh), aa_axis(X, p.net_w, sw), p.net_w);
     const long long hw = (long long)p.H * p.W, pix = (long long)Y * p.W + X;
     p.out_depth[b * hw + pix] = z;
     p.out_confidence[b * hw + pix] = conf;
-    p.out_points[(b * 3 + 0) * hw + pix] = z * tanf(theta);
-    p.out_points[(b * 3 + 1) * hw + pix] = z / tanf(phi) / cosf(theta);
-    p.out_points[(b * 3 + 2) * hw + pix] = z;
+    backproject(p.k4 + b * 4, X, Y, z, p.out_points + b * 3 * hw + pix, hw);
   }
 }
 
@@ -1740,13 +1623,10 @@ __global__ void v2old_camera_kernel(const float* __restrict__ x4, const float* _
                                     float ratio, float* intr4_rays, float* k_out, float* k4_points) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
-  const float half = (float)(net_h > net_w ? net_h : net_w) / 2.f;
-  const float* x = x4 + b * 4;
-  const float fx = half * expf(x[0]), fy = half * expf(x[1]);
-  const float cx = (1.f / (1.f + expf(-x[2]))) * (float)net_w, cy = (1.f / (1.f + expf(-x[3]))) * (float)net_h;
+  const float4 k = decode_camera(x4 + b * 4, (float)(net_h > net_w ? net_h : net_w) / 2.f, net_h, net_w);
+  const float fx = k.x, fy = k.y, cx = k.z, cy = k.w;
   const float kf[4] = {fx / ratio, fy / ratio, cx / ratio, cy / ratio};
-  float* o = k_out + b * 9;
-  o[0] = kf[0]; o[1] = 0.f; o[2] = kf[2]; o[3] = 0.f; o[4] = kf[1]; o[5] = kf[3]; o[6] = 0.f; o[7] = 0.f; o[8] = 1.f;
+  store_k3(k_out + b * 9, kf[0], kf[1], kf[2], kf[3]);
   if (gt_k) {
     const float* g = gt_k + b * 9;
     const float gk[4] = {g[0], g[4], g[2], g[5]};
@@ -1763,35 +1643,27 @@ extern "C" {
 
 int udb_pshuffle_dw7_relu(const void* x, const float* w, const float* bias, void* out, int32_t B, int32_t h, int32_t wd, int32_t C,
                           int32_t ldo, void* stream) {
-  const struct { int v; const char* name; } dims[] = {{B, "B"}, {h, "h"}, {wd, "w"}, {C, "C"}};
-  for (const auto& d : dims)
-    if (d.v < 1) { set_error("udb_pshuffle_dw7_relu: %s=%d must be >= 1", d.name, d.v); return 1; }
+  if (check_dims("udb_pshuffle_dw7_relu", {{B, "B"}, {h, "h"}, {wd, "w"}, {C, "C"}})) return 1;
   if (C % 4) { set_error("udb_pshuffle_dw7_relu: C=%d must be a multiple of 4 (PixelShuffle(2))", C); return 1; }
   if (ldo < C / 4) { set_error("udb_pshuffle_dw7_relu: ldo=%d must be >= C/4=%d", ldo, C / 4); return 1; }
-  const struct { const void* p; const char* name; } ptrs[] = {{x, "x"}, {w, "w"}, {bias, "bias"}, {out, "out"}};
-  for (const auto& a : ptrs)
-    if (!a.p) { set_error("udb_pshuffle_dw7_relu: `%s` must be non-null", a.name); return 1; }
+  if (check_ptrs("udb_pshuffle_dw7_relu", {{x, "x"}, {w, "w"}, {bias, "bias"}, {out, "out"}})) return 1;
   const long long total = 4LL * B * h * wd * ldo;
   note_work(2.0 * 49 * 4.0 * B * h * wd * (C / 4), 2.0 * B * h * wd * C + 2.0 * total);
-  pshuffle_dw7_relu_kernel<<<grid_1d(total), 256, 0, ST(stream)>>>(reinterpret_cast<const __half*>(x), w, bias,
+  pshuffle_dw7_relu_kernel<<<grid_1d(total, 32), 256, 0, ST(stream)>>>(reinterpret_cast<const __half*>(x), w, bias,
                                                                     reinterpret_cast<__half*>(out), B, h, wd, C, ldo);
   return check_launch("pshuffle_dw7_relu_kernel");
 }
 
 int udb_v2old_heads(const udb_v2old_heads_t* p, void* stream) {
   if (!p) { set_error("udb_v2old_heads: null argument"); return 1; }
-  const struct { int v; const char* name; } dims[] = {{p->B, "B"}, {p->gh, "gh"}, {p->gw, "gw"}, {p->net_h, "net_h"}, {p->net_w, "net_w"}};
-  for (const auto& d : dims)
-    if (d.v < 1) { set_error("udb_v2old_heads: %s=%d must be >= 1", d.name, d.v); return 1; }
+  if (check_dims("udb_v2old_heads", {{p->B, "B"}, {p->gh, "gh"}, {p->gw, "gw"}, {p->net_h, "net_h"}, {p->net_w, "net_w"}})) return 1;
   if (p->net_h < 4 || p->net_w < 4) { set_error("udb_v2old_heads: net_h=%d net_w=%d: the 7x7 reflect padding needs >= 4", p->net_h, p->net_w); return 1; }
-  const struct { const void* q; const char* name; } ptrs[] = {{p->levels[0], "levels[0]"}, {p->levels[1], "levels[1]"},
-                                                             {p->levels[2], "levels[2]"}, {p->w, "w"}, {p->logdepth, "logdepth"},
-                                                             {p->confidence, "confidence"}};
-  for (const auto& a : ptrs)
-    if (!a.q || (reinterpret_cast<uintptr_t>(a.q) & 15)) { set_error("udb_v2old_heads: `%s` must be a non-null, 16-byte aligned pointer", a.name); return 1; }
+  if (check_ptrs("udb_v2old_heads", {{p->levels[0], "levels[0]"}, {p->levels[1], "levels[1]"}, {p->levels[2], "levels[2]"}, {p->w, "w"},
+                                     {p->logdepth, "logdepth"}, {p->confidence, "confidence"}}, 16))
+    return 1;
   const long long px = (long long)p->B * p->net_h * p->net_w;
   note_work(px * 49.0 * 3 * (8.0 * 32 + 2.0 * 32), px * 8.0);
-  v2old_heads_kernel<<<grid_1d(px), 256, 0, ST(stream)>>>(*p);
+  v2old_heads_kernel<<<grid_1d(px, 32), 256, 0, ST(stream)>>>(*p);
   return check_launch("v2old_heads_kernel");
 }
 
@@ -1805,21 +1677,17 @@ int udb_v2old_depth_tail(float* depth, const float* scale_shift, int32_t B, int6
 
 int udb_v2old_postprocess(const udb_v2old_postprocess_t* p, void* stream) {
   if (!p) { set_error("udb_v2old_postprocess: null argument"); return 1; }
-  const struct { int v; const char* name; } dims[] = {{p->B, "B"}, {p->H, "H"}, {p->W, "W"}, {p->net_h, "net_h"}, {p->net_w, "net_w"}};
-  for (const auto& d : dims)
-    if (d.v < 1) { set_error("udb_v2old_postprocess: %s=%d must be >= 1", d.name, d.v); return 1; }
+  if (check_dims("udb_v2old_postprocess", {{p->B, "B"}, {p->H, "H"}, {p->W, "W"}, {p->net_h, "net_h"}, {p->net_w, "net_w"}})) return 1;
   if (p->depth_aa != 0 && p->depth_aa != 1) { set_error("udb_v2old_postprocess: `depth_aa` %d is neither 0 nor 1", p->depth_aa); return 1; }
   if (!p->depth_aa && p->mode != UDB_V2OLD_BILINEAR && p->mode != UDB_V2OLD_NEAREST_EXACT) {
     set_error("udb_v2old_postprocess: `mode` %d is neither UDB_V2OLD_BILINEAR (0) nor UDB_V2OLD_NEAREST_EXACT (1)", p->mode);
     return 1;
   }
-  const struct { const void* q; const char* name; } ptrs[] = {{p->depth, "depth"}, {p->confidence, "confidence"}, {p->k4, "k4"},
-                                                             {p->out_depth, "out_depth"}, {p->out_confidence, "out_confidence"},
-                                                             {p->out_points, "out_points"}};
-  for (const auto& a : ptrs)
-    if (!a.q) { set_error("udb_v2old_postprocess: `%s` must be non-null", a.name); return 1; }
-  if (p->depth_aa) v2old_postprocess_kernel<true><<<grid_1d((long long)p->B * p->H * p->W), 256, 0, ST(stream)>>>(*p);
-  else v2old_postprocess_kernel<false><<<grid_1d((long long)p->B * p->H * p->W), 256, 0, ST(stream)>>>(*p);
+  if (check_ptrs("udb_v2old_postprocess", {{p->depth, "depth"}, {p->confidence, "confidence"}, {p->k4, "k4"}, {p->out_depth, "out_depth"},
+                                           {p->out_confidence, "out_confidence"}, {p->out_points, "out_points"}}))
+    return 1;
+  if (p->depth_aa) v2old_postprocess_kernel<true><<<grid_1d((long long)p->B * p->H * p->W, 32), 256, 0, ST(stream)>>>(*p);
+  else v2old_postprocess_kernel<false><<<grid_1d((long long)p->B * p->H * p->W, 32), 256, 0, ST(stream)>>>(*p);
   return check_launch("v2old_postprocess_kernel");
 }
 
