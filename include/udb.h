@@ -325,6 +325,18 @@ enum {
 int udb_camera_rays(int32_t model, const float* params, int32_t B, int32_t net_h, int32_t net_w, int32_t pad_l,
                     int32_t pad_r, int32_t pad_t, int32_t pad_b, float factor, float* rays, void* stream);
 
+/* Ground-truth point map (utils/camera.py reconstruct; the evaluation's camera.reconstruct(depth)): points [B, 3, H, W]
+ * f32, planar, of each image's camera at the pixel centres of its depth map depth [B, 1, H, W] f32.  params are the
+ * packed rows of udb_camera_rays, in the depth map's own pixels; no crop or resize is applied.  Each class's rule:
+ *   UDB_CAM_PINHOLE     unproject(uv) * clip(depth, 0)
+ *   UDB_CAM_SPHERICAL   unproject(uv) * depth                  (depth is the range)
+ *   other models        xyz / clamp(xyz_z, 1e-4) * clamp(depth, 1e-4), xyz the class's unproject before get_rays
+ * Clamps propagate NaN as torch's do, so a pixel outside the model's domain (MEI with xi > 1 far off axis) is NaN in all
+ * three planes, as the class gives it.  Checked before launch as udb_camera_rays: model known, B in [1, 65535],
+ * H, W >= 1, H * W <= 2^30, params / depth / points non-null and aligned (16 / 4 / 4 bytes). */
+int udb_camera_reconstruct(int32_t model, const float* params, int32_t B, int32_t H, int32_t W, const float* depth,
+                           float* points, void* stream);
+
 typedef struct udb_ray_embed_t {
   const float* intr4;
   const float* rays_in;

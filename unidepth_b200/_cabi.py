@@ -288,6 +288,7 @@ EXPORTS = {
     "udb_match_gt": (i32, [C.POINTER(MatchGt), vp]),
     "udb_camera_adjust_k": (i32, [vp, i32, f32, i32, i32, vp, vp]),
     "udb_camera_rays": (i32, [i32, vp, i32, i32, i32, i32, i32, i32, i32, f32, vp, vp]),
+    "udb_camera_reconstruct": (i32, [i32, vp, i32, i32, i32, vp, vp, vp]),
     "udb_create": (i32, [C.POINTER(Config), C.POINTER(vp)]),
     "udb_destroy": (None, [vp]),
     "udb_set_weight": (i32, [vp, C.c_char_p, vp, C.POINTER(i64), i32, i32]),

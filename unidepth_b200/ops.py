@@ -305,6 +305,20 @@ def camera_rays(model, params, B, net_hw, paddings, factor):
     return out
 
 
+def camera_reconstruct(model, params, depth):
+    """Ground-truth point map [B, 3, H, W] (udb_camera_reconstruct): the class's reconstruct(depth) of a packed camera,
+    params [B, CAM_STRIDE] f32 in the depth map's own pixels, depth [B, 1, H, W] f32, both contiguous on the GPU."""
+    B, _, H, W = depth.shape
+    assert params.dtype == f32 and params.is_contiguous() and tuple(params.shape) == (B, cabi.CAM_STRIDE), params.shape
+    assert depth.dtype == f32 and depth.is_contiguous() and depth.shape[1] == 1, (depth.dtype, depth.shape)
+    out = torch.empty((B, 3, H, W), device=depth.device, dtype=f32)
+    cabi.check(_launch("camera_reconstruct_kernel", 0.0,
+                       lambda: cabi.lib().udb_camera_reconstruct(int(model), _ptr(params), B, H, W, _ptr(depth), _ptr(out),
+                                                                 _stream()), _nb(out, depth)),
+               "udb_camera_reconstruct")
+    return out
+
+
 def ray_embed(intr4, scales, B, net_hw, grid_hw, out_dtype=f32, rays_in=None):
     bands = scales.numel()
     out = torch.empty((B * grid_hw[0] * grid_hw[1], 2 * bands), device=scales.device, dtype=out_dtype)

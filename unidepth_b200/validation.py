@@ -1,5 +1,6 @@
 """The reference's validation path (SURVEY.md section 8f rank 3): matching the network outputs to the ground-truth
-frame, and the depth and 3D evaluation metrics.
+frame, the depth and 3D evaluation metrics, the ground-truth point map, their accumulation over a test set and the
+evaluation loop.
 
 `match_gt`, `match_intrinsics` and `depth_metrics` are plain torch ops on small tensors (the network itself runs in
 libudb.so, UniDepthV2.forward_test).  `eval_depth`, `eval_3d` and `chamfer_distance` run their per-pixel and per-point
@@ -7,12 +8,18 @@ work in libudb.so (udb_depth_metrics, udb_nearest_neighbor, udb_point_metrics); 
 the per-image sums and counts into the metrics.
 
 Reference: unidepth/utils/misc.py:596-642 (`match_gt`), :645-690 (`match_intrinsics`),
-unidepth/utils/evaluation_depth.py (metrics), unidepth/utils/chamfer_distance.py:59-158 (`ChamferDistance`)."""
+unidepth/utils/evaluation_depth.py (metrics), unidepth/utils/chamfer_distance.py:59-158 (`ChamferDistance`),
+unidepth/datasets/base_dataset.py:155-275 (`accumulate_metrics`, `get_evaluation`), unidepth/utils/validation.py:64-91
+(`validate`), unidepth/utils/distributed.py:153-176 (`sync_tensor_across_gpus`)."""
 from __future__ import annotations
 
+import contextlib
+from math import log
 from typing import Dict, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
+import torch.distributed as dist
 import torch.nn.functional as F
 
 
@@ -251,3 +258,207 @@ def eval_3d(gts: torch.Tensor, preds: torch.Tensor, masks: torch.Tensor,
         sel = torch.tensor(keep, device=gts.device)
         res = {k: v[sel] for k, v in res.items()}
     return res
+
+
+# ------------------------------------------------------------------------------------------ ground-truth point map
+def reconstruct(camera, depth: torch.Tensor) -> torch.Tensor:
+    """The reference's `camera.reconstruct(depth)`: the ground-truth point map [B, 3, H, W] of a z-depth (range, for
+    Spherical) map [B, 1, H, W], with each camera class's own rule.  A camera that `camera.pack_camera` accepts, with one
+    row (broadcast to the batch) or one row per image, and an f32 CUDA depth map take the udb_camera_reconstruct kernel;
+    anything else (mixed-model BatchCameras, the reference's own classes, duck-typed objects, the 15-parameter layout,
+    CPU tensors) runs the object's own `reconstruct`."""
+    from .camera import pack_camera
+    packed = None
+    if isinstance(depth, torch.Tensor) and depth.is_cuda and depth.dtype == torch.float32 and depth.dim() == 4 \
+            and depth.shape[1] == 1:
+        packed = pack_camera(camera)
+    if packed is not None and packed[1].shape[0] in (1, depth.shape[0]):
+        from . import ops
+        model, rows = packed
+        rows = rows.to(depth.device).expand(depth.shape[0], -1).contiguous()
+        return ops.camera_reconstruct(model, rows, depth.contiguous())
+    return camera.reconstruct(depth)
+
+
+# ------------------------------------------------------------------------------------- accumulation over a test set
+def gather_across_ranks(t: Optional[torch.Tensor], group=None) -> Optional[torch.Tensor]:
+    """Concatenate every rank's 1-D (or leading-dimension) tensor in rank order, whatever each rank's length: gather
+    the lengths, pad to the longest, all_gather, trim, concatenate (the reference's sync_tensor_across_gpus).  The
+    tensor itself when torch.distributed is not initialised."""
+    if t is None or not (dist.is_available() and dist.is_initialized()):
+        return t
+    t = torch.atleast_1d(t)
+    world = dist.get_world_size(group)
+    n = torch.tensor([t.shape[0]], device=t.device, dtype=torch.int64)
+    sizes = [torch.zeros_like(n) for _ in range(world)]
+    dist.all_gather(sizes, n, group=group)
+    sizes = [int(v.item()) for v in sizes]
+    longest = max(sizes)
+    if longest > t.shape[0]:
+        t = torch.cat([t, t.new_zeros((longest - t.shape[0],) + tuple(t.shape[1:]))])
+    parts = [torch.empty_like(t) for _ in range(world)]
+    dist.all_gather(parts, t.contiguous(), group=group)
+    return torch.cat([p[:k] for p, k in zip(parts, sizes)])
+
+
+def _index(x, index):
+    """The reference's recursive_index: slice the tensors of a (nested) dict, leave everything else as it is."""
+    if isinstance(x, dict):
+        return {k: _index(v, index) for k, v in x.items()}
+    if isinstance(x, torch.Tensor):
+        return x[index]
+    return x
+
+
+def _no_autocast(fn):
+    """The reference accumulates in fp32 whatever autocast context the caller opened."""
+    return torch.autocast(device_type="cuda", enabled=False)(fn)
+
+
+class DatasetMetrics:
+    """Per-image evaluation metrics accumulated over a test set and reduced to its means, as the reference's
+    BaseDataset does (accumulate_metrics, get_evaluation and their helpers, same names and attributes).  It can be used
+    on its own or inherited as a mixin by a dataset class (which then calls DatasetMetrics.__init__ or sets
+    `metrics_store`, `metrics_count`, `min_depth` and `max_depth` itself); a `keyframe_idx` attribute, if the object has
+    one, selects the depth frame as in the reference.
+
+    Kept from the reference: a metric is available when it is a substring of some key of both `inputs` and `preds`;
+    `keyframe_idx` slices tensors only, and prepare_depth_eval slices again with the `keyframe_idx` attribute; a pred
+    key containing "depth" is evaluated with eval_depth and one containing "points" with eval_3d (100 F1 thresholds
+    log-spaced from min_depth to max_depth / 20) under the log name left by removing that word, so a pred dict with
+    "depth" and "points" fills one store "" with 21 metrics; `metrics_count` is gathered but unused; a metric image whose
+    mask is empty gives NaN depth metrics, which propagates to the mean.  Differences: the caller's `inputs` is not
+    modified (the point map is added to a shallow copy), and a pred selected for depth that is not a float
+    [B, 1, h, w] tensor raises ValueError naming it before any metric runs (the reference fails inside F.interpolate)."""
+
+    eval_depth = staticmethod(eval_depth)
+    eval_3d = staticmethod(eval_3d)
+
+    def __init__(self, min_depth: float = 0.01, max_depth: float = 1000.0):
+        self.min_depth = min_depth
+        self.max_depth = max_depth
+        self.metrics_store: Dict[str, Dict[str, torch.Tensor]] = {}
+        self.metrics_count: Dict[str, torch.Tensor] = {}
+
+    def add_points(self, inputs):
+        inputs["points"] = reconstruct(inputs.get("camera_original", inputs["camera"]), inputs["depth"])
+        return inputs
+
+    def prepare_depth_eval(self, inputs, preds):
+        keyframe_idx = getattr(self, "keyframe_idx", None)
+        slice_idx = slice(keyframe_idx, keyframe_idx + 1 if keyframe_idx is not None else None)
+        new_gts = inputs["depth"][slice_idx]
+        new_masks = inputs["depth_mask"][slice_idx].bool()
+        new_preds = {key: val[slice_idx] for key, val in preds.items() if "depth" in key}
+        return new_gts, new_preds, new_masks
+
+    def prepare_points_eval(self, inputs, preds):
+        new_gts = inputs["points"]
+        new_masks = inputs["points_mask"].bool() if "points_mask" in inputs else inputs["depth_mask"].bool()
+        new_preds = {key: val for key, val in preds.items() if "points" in key}
+        return new_gts, new_preds, new_masks
+
+    @_no_autocast
+    def accumulate_metrics(self, inputs, preds, keyframe_idx=None, metrics=("depth", "points", "flow_fwd", "pairwise")):
+        if "depth" in inputs and "points" not in inputs:
+            inputs = self.add_points(dict(inputs))
+        available = [m for m in metrics if any(m in k for k in inputs) and any(m in k for k in preds)]
+        if keyframe_idx is not None:
+            inputs = _index(inputs, slice(keyframe_idx, keyframe_idx + 1))
+            preds = _index(preds, slice(keyframe_idx, keyframe_idx + 1))
+        if "depth" in available:
+            gts, depth_preds, masks = self.prepare_depth_eval(inputs, preds)
+            for key, val in depth_preds.items():
+                if not isinstance(val, torch.Tensor) or not val.is_floating_point() or val.dim() != 4 \
+                        or val.shape[:2] != (gts.shape[0], 1):
+                    shape = tuple(val.shape) if isinstance(val, torch.Tensor) else type(val).__name__
+                    raise ValueError(f"accumulate_metrics: pred {key!r} is selected for the depth metrics (its key "
+                                     f"contains 'depth') but is not a float [B, 1, h, w] depth map with B = "
+                                     f"{gts.shape[0]}: {shape}")
+            self.accumulate_metrics_depth(gts, depth_preds, masks)
+        if "points" in available:
+            self.accumulate_metrics_3d(*self.prepare_points_eval(inputs, preds))
+
+    def _append(self, log_name, gts, masks, values):
+        store = self.metrics_store.setdefault(log_name, {})
+        count = self.metrics_count.get(log_name, torch.tensor([], device=gts.device))
+        self.metrics_count[log_name] = torch.cat([count, masks.view(gts.shape[0], -1).sum(dim=-1)])
+        for k, v in values.items():
+            store[k] = torch.cat([store.get(k, torch.tensor([], device=gts.device)), v])
+
+    @_no_autocast
+    def accumulate_metrics_depth(self, gts, preds, masks):
+        for eval_type, pred in preds.items():
+            log_name = eval_type.replace("depth", "").strip("-").strip("_")
+            self._append(log_name, gts, masks, self.eval_depth(gts, pred, masks, max_depth=self.max_depth))
+
+    @_no_autocast
+    def accumulate_metrics_3d(self, gts, preds, masks):
+        thresholds = torch.linspace(log(self.min_depth), log(self.max_depth / 20), steps=100, device=gts.device).exp()
+        for eval_type, pred in preds.items():
+            log_name = eval_type.replace("points", "").strip("-").strip("_")
+            self._append(log_name, gts, masks, self.eval_3d(gts, pred, masks, thresholds=thresholds))
+
+    def get_evaluation(self, metrics=None) -> Dict[str, float]:
+        """{f"{eval_type}_{name}".strip("_"): mean over every rank's images, rounded to 5 decimals}; clears the stores.
+        A store that was emptied by an earlier call and has had nothing added raises AssertionError, as in the
+        reference."""
+        values = {}
+        for eval_type in metrics if metrics is not None else list(self.metrics_store.keys()):
+            assert self.metrics_store[eval_type], f"no metrics accumulated for {eval_type!r}"
+            gather_across_ranks(self.metrics_count[eval_type])
+            for name, val in self.metrics_store[eval_type].items():
+                mean = gather_across_ranks(val).mean()
+                values[f"{eval_type}_{name}".strip("_")] = float(np.round(mean.cpu().item(), 5))
+            self.metrics_store[eval_type] = {}
+        self.metrics_count = {}
+        return values
+
+
+# --------------------------------------------------------------------------------------------------- evaluation loop
+def _rank0() -> bool:
+    return not (dist.is_available() and dist.is_initialized()) or dist.get_rank() == 0
+
+
+def _barrier() -> None:
+    if dist.is_available() and dist.is_initialized():
+        dist.barrier()
+
+
+def _dataset_metrics(dataset) -> DatasetMetrics:
+    if isinstance(dataset, DatasetMetrics):
+        return dataset
+    return DatasetMetrics(min_depth=getattr(dataset, "min_depth", 0.01), max_depth=getattr(dataset, "max_depth", 1000.0))
+
+
+def validate(model, test_loaders, step=None, context=None) -> Dict[str, Dict[str, float]]:
+    """The reference's evaluation loop over {name: DataLoader}: for each batch, move `batch["data"]` to model.device and
+    drop the loader's temporal axis (squeeze(1); an object without `squeeze`, such as a camera, is taken as already
+    squeezed), unwrap the metas ({k: v[0]} of their list values), run `model(data, metas)` under torch.no_grad() and
+    `context`, and accumulate the metrics with the first meta's keyframe_idx.  After each loader, every rank runs
+    get_evaluation (which gathers across ranks), and rank 0 prints `Metrics/{name}/{metric} {value}` lines.  Returns
+    {name: {metric: value}}.
+
+    Each loader's accumulator is its dataset if that is a DatasetMetrics, else a DatasetMetrics with the dataset's
+    min_depth / max_depth (0.01 / 1000 without them).  Differences from the reference: nothing is logged to wandb
+    (`step` is accepted and unused); `original_image` is not run, since nothing the accumulation reads depends on it; a
+    dataset's own accumulate_metrics override is only called when the dataset is a DatasetMetrics.  The caller's batches
+    are not modified."""
+    metrics_all = {}
+    for name_ds, loader in test_loaders.items():
+        acc = _dataset_metrics(loader.dataset)
+        for batch in loader:
+            with context if context is not None else contextlib.nullcontext(), torch.no_grad():
+                data = {k: (v.to(model.device) if hasattr(v, "to") else v) for k, v in batch["data"].items()}
+                data = {k: (v.squeeze(1) if hasattr(v, "squeeze") else v) for k, v in data.items()}
+                metas = [{k: v[0] for k, v in meta.items() if isinstance(v, list)} for meta in batch["img_metas"]]
+                preds = model(data, metas)
+            acc.accumulate_metrics(inputs=data, preds=preds, keyframe_idx=metas[0].get("keyframe_idx") if metas else None)
+        _barrier()
+        metrics_all[name_ds] = acc.get_evaluation()
+    _barrier()
+    if _rank0():
+        for name_ds, values in metrics_all.items():
+            for name, v in values.items():
+                print(f"Metrics/{name_ds}/{name} {round(v, 4)}")
+    return metrics_all
